@@ -33,6 +33,7 @@ LIB_PATH = _HERE / "libvmig.so"
 
 VMIG_OK, VMIG_EINVAL, VMIG_ENOGPU, VMIG_ECUDA, VMIG_EIO = 0, -1, -2, -3, -4
 VMIG_ENOMEM, VMIG_ETABLE, VMIG_EFAULT, VMIG_ENOTDIR, VMIG_ESRCCHANGED, VMIG_EVERIFY = -5, -6, -7, -8, -9, -10
+VMIG_ECORRUPT = -11
 F_MOVE_SRC, F_SKIP_HIDDEN_TOPDIRS, F_MTIME_NS, F_NO_METADATA, F_HASH_ONLY, F_VERIFY = 0x01, 0x02, 0x04, 0x08, 0x10, 0x20
 F_PRUNE, F_DIRECT_IO, F_CUFILE = 0x40, 0x80, 0x100
 BLOCK_BYTES = 4 << 20
@@ -40,7 +41,7 @@ MOVE_DIR_FLAGS = F_MOVE_SRC | F_VERIFY          # what vmig_move_dir passes (inc
 
 EXPORTS = [
     "vmig_init", "vmig_shutdown", "vmig_device_count", "vmig_strerror", "vmig_last_error", "vmig_version",
-    "vmig_migrate_tree", "vmig_copy_dir", "vmig_move_dir", "vmig_migrate_buffer", "vmig_host_alloc",
+    "vmig_migrate_tree", "vmig_restore_tree", "vmig_copy_dir", "vmig_move_dir", "vmig_migrate_buffer", "vmig_host_alloc",
     "vmig_host_free", "vmig_hash_blocks", "vmig_resident_open", "vmig_resident_close", "vmig_resident_fill",
     "vmig_resident_set_len", "vmig_resident_upload", "vmig_resident_download", "vmig_resident_flip",
     "vmig_resident_set_prior", "vmig_resident_pass", "vmig_resident_results", "vmig_table_info_read",
@@ -85,6 +86,8 @@ _sig = {
     "vmig_init": (C.c_int, [C.c_uint32]), "vmig_shutdown": (None, []), "vmig_device_count": (C.c_int, []),
     "vmig_strerror": (C.c_char_p, [C.c_int]), "vmig_last_error": (C.c_char_p, []), "vmig_version": (C.c_char_p, []),
     "vmig_migrate_tree": (C.c_int, [C.c_char_p, C.c_char_p, C.c_char_p, C.c_char_p, C.POINTER(Opts), C.POINTER(Stats)]),
+    "vmig_restore_tree": (C.c_int, [C.c_char_p, C.c_char_p, C.c_char_p, C.c_char_p, C.c_char_p, C.POINTER(Opts),
+                                    C.POINTER(Stats)]),
     "vmig_copy_dir": (C.c_int, [C.c_char_p, C.c_char_p]), "vmig_move_dir": (C.c_int, [C.c_char_p, C.c_char_p]),
     "vmig_migrate_buffer": (C.c_int, [C.c_void_p, C.c_void_p, C.c_uint64, C.c_void_p, C.c_void_p, C.c_void_p,
                                       C.POINTER(Opts), C.POINTER(Stats)]),
@@ -226,6 +229,18 @@ def migrate_tree(src, dst, prior_table=None, out_table=None, *, gpu_mask: int = 
     st = Stats()
     _check(_lib.vmig_migrate_tree(_b(src), _b(dst), _b(prior_table), _b(out_table), C.byref(o), C.byref(st)),
            f"vmig_migrate_tree({src} -> {dst})")
+    return st.as_dict()
+
+
+def restore_tree(snap, snap_table, dst, prior_table=None, out_table=None, *, gpu_mask: int = 0, flags: int = 0,
+                 block_bytes: int = 0, io_threads: int = 0, streams_per_gpu: int = 0, lanes_per_gpu: int = 0) -> dict:
+    """migrate_tree(snap, dst, ...) that first requires `snap` to still be the tree `snap_table` describes (same
+    paths and sizes, every block's hash): VMIG_ECORRUPT otherwise.  flags=F_HASH_ONLY with dst=None only checks."""
+    o = Opts(gpu_mask=gpu_mask, block_bytes=block_bytes, flags=flags, io_threads=io_threads,
+             streams_per_gpu=streams_per_gpu, lanes_per_gpu=lanes_per_gpu)
+    st = Stats()
+    _check(_lib.vmig_restore_tree(_b(snap), _b(snap_table), _b(dst), _b(prior_table), _b(out_table), C.byref(o),
+                                  C.byref(st)), f"vmig_restore_tree({snap} -> {dst})")
     return st.as_dict()
 
 

@@ -50,6 +50,10 @@ public:
     bool device_reads() override { return cufile; }
     bool device_writes() override { return cufile && !hash_only; }
     long corrupt_block = -1;             // VMIG_CORRUPT_BLOCK test hook: flip one bit of this block on its way to disk
+    uint32_t block_bytes = 4u << 20;
+    std::string block_name(const BlockRef& b) override {
+        return m->files[b.file].rel + " block " + std::to_string(b.file_off / block_bytes);
+    }
     std::unique_ptr<FS[]> fs;
     std::mutex stripes[64];
 
@@ -277,7 +281,7 @@ bool is_pinned(const void* p) {
 // run a block list over the selected GPUs: n_gpus x lanes_per_gpu lanes, whole files per lane (LPT by bytes);
 // contiguous byte-balanced ranges only when there are fewer than two files per lane
 int run_blocks(const std::vector<BlockRef>& blocks, BlockIO* io, bool has_prior, bool hash_only, const vmig_opts& o,
-               uint64_t* hashes, vmig_stats* st)
+               uint64_t* hashes, vmig_stats* st, const uint64_t* expect = nullptr)
 {
     std::vector<DeviceInfo> devs;
     int rc = ctx_select(o.gpu_mask, &devs);
@@ -339,7 +343,7 @@ int run_blocks(const std::vector<BlockRef>& blocks, BlockIO* io, bool has_prior,
     std::vector<std::thread> th;
     for (size_t i = 0; i < lanes; i++)
         th.emplace_back([&, i] {
-            run_lane(pipes[i], share[i], io, has_prior, hash_only, readers, writers, o.streams_per_gpu, hashes, &ls[i], &err, &err_msg, &err_mu);
+            run_lane(pipes[i], share[i], io, has_prior, hash_only, readers, writers, o.streams_per_gpu, expect, hashes, &ls[i], &err, &err_msg, &err_mu);
         });
     for (auto& t : th) t.join();
     for (size_t i = 0; i < lanes; i++) ctx_release_pipe(pipes[i]);
@@ -353,6 +357,31 @@ int run_blocks(const std::vector<BlockRef>& blocks, BlockIO* io, bool has_prior,
     return VMIG_OK;
 }
 
+// Restore, plan time: the walked tree must be the one the snapshot's table describes -- the same regular-file paths
+// (hard-linked ones included) with the same sizes.  ino/ctime_ns are not compared: a snapshot copied elsewhere keeps
+// its bytes, not its inodes.  Both lists are sorted bytewise, so one merge finds the first difference.  On success
+// expect[] holds the table's hashes in the manifest's block order.
+int match_table(const Manifest& man, const BlockTable& t, std::vector<uint64_t>* expect)
+{
+    size_t i = 0, j = 0;
+    while (i < man.files.size() || j < t.files.size()) {
+        if (j == t.files.size() || (i < man.files.size() && man.files[i].rel < t.files[j].rel))
+            return fail(VMIG_ECORRUPT, "%s is in the snapshot but not in its block table (extra)", man.files[i].rel.c_str());
+        if (i == man.files.size() || t.files[j].rel < man.files[i].rel)
+            return fail(VMIG_ECORRUPT, "%s is in the block table but not in the snapshot (missing)", t.files[j].rel.c_str());
+        if (man.files[i].size != t.files[j].size)
+            return fail(VMIG_ECORRUPT, "%s is %llu bytes in the snapshot, %llu in its block table (resized)", man.files[i].rel.c_str(),
+                        (unsigned long long)man.files[i].size, (unsigned long long)t.files[j].size);
+        i++; j++;
+    }
+    expect->assign(man.n_blocks, 0);
+    for (size_t f = 0; f < man.files.size(); f++) {
+        const Entry& e = man.files[f];
+        std::copy_n(t.hashes.begin() + (ptrdiff_t)t.files[f].first_block, e.n_blocks, expect->begin() + (ptrdiff_t)e.first_block);
+    }
+    return VMIG_OK;
+}
+
 vmig_opts norm_opts(const vmig_opts* in) {
     vmig_opts o; memset(&o, 0, sizeof o);
     if (in) o = *in;
@@ -362,8 +391,10 @@ vmig_opts norm_opts(const vmig_opts* in) {
     return o;
 }
 
+// snap_path non-null: vmig_restore_tree -- src_dir must match that block table (match_table before anything touches the
+// destination, every block's hash in the hash-waiter, hard-linked paths before metadata replay)
 int migrate_tree_impl(const char* src_dir, const char* dst_dir, const char* prior_path, const char* out_path,
-                      const vmig_opts* opts_in, vmig_stats* stats_out)
+                      const vmig_opts* opts_in, vmig_stats* stats_out, const char* snap_path = nullptr)
 {
     vmig_stats st; memset(&st, 0, sizeof st);
     const uint64_t t_begin = now_ns();
@@ -393,6 +424,15 @@ int migrate_tree_impl(const char* src_dir, const char* dst_dir, const char* prio
     st.ns_walk = now_ns() - t0;
 
     t0 = now_ns();
+    std::vector<uint64_t> expect;
+    if (snap_path) {
+        BlockTable snap;
+        rc = table_load(snap_path, &snap);
+        if (rc) return rc;
+        if (snap.block_bytes != o.block_bytes) return fail(VMIG_ETABLE, "snapshot table block size %u != %u", snap.block_bytes, o.block_bytes);
+        rc = match_table(man, snap, &expect);
+        if (rc) return rc;
+    }
     BlockTable prior; bool has_prior = false;
     if (prior_path && *prior_path && !hash_only) {
         rc = table_load(prior_path, &prior);
@@ -402,6 +442,7 @@ int migrate_tree_impl(const char* src_dir, const char* dst_dir, const char* prio
     }
     FileIO io;
     io.src_root = src; io.dst_root = dst; io.m = &man; io.pol = default_meta_policy(o.flags); io.hash_only = hash_only;
+    io.block_bytes = o.block_bytes;
     io.corrupt_block = env_long("VMIG_CORRUPT_BLOCK", -1);
     io.direct = (o.flags & VMIG_F_DIRECT_IO) != 0;
     io.cufile = (o.flags & VMIG_F_CUFILE) != 0;
@@ -467,7 +508,7 @@ int migrate_tree_impl(const char* src_dir, const char* dst_dir, const char* prio
     if (!hash_only) { rc = make_dirs(dst, man); if (rc) return rc; }
 
     t0 = now_ns();
-    rc = run_blocks(blocks, &io, has_prior, hash_only, o, hashes.data(), &st);
+    rc = run_blocks(blocks, &io, has_prior, hash_only, o, hashes.data(), &st, expect.empty() ? nullptr : expect.data());
     st.ns_data = now_ns() - t0;
     if (rc) { std::string keep = last_error_cstr(); io.close_all(man.files.size()); set_last_error_str(keep); return rc; }
 
@@ -475,7 +516,15 @@ int migrate_tree_impl(const char* src_dir, const char* dst_dir, const char* prio
     for (auto& e : man.files)                      // hard-linked paths share their primary's hashes
         if (e.hardlink_of >= 0) {
             const Entry& p = man.files[(size_t)e.hardlink_of];
-            for (uint64_t r = 0; r < e.n_blocks; r++) hashes[e.first_block + r] = hashes[p.first_block + r];
+            for (uint64_t r = 0; r < e.n_blocks; r++) {
+                hashes[e.first_block + r] = hashes[p.first_block + r];
+                // restore: the table hashed this path on its own; it must describe the bytes its primary now holds
+                // (checked before replay_metadata creates any link)
+                if (!expect.empty() && expect[e.first_block + r] != hashes[e.first_block + r])
+                    return fail(VMIG_ECORRUPT, "%s block %llu (a hard link to %s) hashes %016llx, its block table says %016llx",
+                                e.rel.c_str(), (unsigned long long)r, p.rel.c_str(), (unsigned long long)hashes[e.first_block + r],
+                                (unsigned long long)expect[e.first_block + r]);
+            }
         }
     if (!hash_only) {
         for (auto& e : man.files) {                // empty regular files carry no blocks
@@ -590,6 +639,7 @@ const char* vmig_strerror(int code)
     case VMIG_ENOTDIR: return "not a directory";
     case VMIG_ESRCCHANGED: return "source changed during migration";
     case VMIG_EVERIFY: return "destination does not verify against the source";
+    case VMIG_ECORRUPT: return "source tree does not match its block table";
     default: return "unknown vmig error";
     }
 }
@@ -598,6 +648,13 @@ int vmig_migrate_tree(const char* src_dir, const char* dst_dir, const char* prio
                       const vmig_opts* opts, vmig_stats* stats)
 {
     return migrate_tree_impl(src_dir, dst_dir, prior_table, out_table, opts, stats);
+}
+int vmig_restore_tree(const char* snap_dir, const char* snap_table, const char* dst_dir, const char* prior_table,
+                      const char* out_table, const vmig_opts* opts, vmig_stats* stats)
+{
+    if (!snap_table || !*snap_table) return fail(VMIG_EINVAL, "snap_table is NULL/empty: a snapshot is only restored against its block table");
+    if (opts && (opts->flags & VMIG_F_MOVE_SRC)) return fail(VMIG_EINVAL, "VMIG_F_MOVE_SRC: a restore never consumes the snapshot");
+    return migrate_tree_impl(snap_dir, dst_dir, prior_table, out_table, opts, stats, snap_table);
 }
 int vmig_copy_dir(const char* src_dir, const char* dst_dir) { return migrate_tree_impl(src_dir, dst_dir, nullptr, nullptr, nullptr, nullptr); }
 int vmig_move_dir(const char* src_dir, const char* dst_dir)

@@ -497,8 +497,8 @@ static void bind_thread(const DeviceInfo& d) {
 }
 
 int run_lane(Pipe* pipe, const std::vector<BlockRef>& blocks, BlockIO* io, bool has_prior, bool hash_only,
-             uint32_t n_readers, uint32_t n_writers, uint32_t max_slots, uint64_t* hashes_out, LaneStats* stats,
-             std::atomic<int>* err, std::string* err_msg, std::mutex* err_mu)
+             uint32_t n_readers, uint32_t n_writers, uint32_t max_slots, const uint64_t* expect, uint64_t* hashes_out,
+             LaneStats* stats, std::atomic<int>* err, std::string* err_msg, std::mutex* err_mu)
 {
     if (blocks.empty()) return VMIG_OK;
     const uint32_t slot_bytes = pipe->slot_bytes;
@@ -699,6 +699,11 @@ int run_lane(Pipe* pipe, const std::vector<BlockRef>& blocks, BlockIO* io, bool 
             const BlockRef& r = blocks[b->b0 + i];
             hashes_out[r.table_idx] = h_hash[i];
             if (fail_block >= 0 && (uint64_t)fail_block == r.table_idx) return fail(VMIG_EFAULT, "injected fault at block %ld (VMIG_FAIL_BLOCK)", fail_block);
+            // restore: checked before the prior-table skip below, so a block the destination already has cannot hide
+            // corruption; nothing of this batch has been written yet
+            if (expect && expect[r.table_idx] != h_hash[i])
+                return fail(VMIG_ECORRUPT, "%s hashes %016llx, its block table says %016llx", io->block_name(r).c_str(),
+                            (unsigned long long)h_hash[i], (unsigned long long)expect[r.table_idx]);
             if (has_prior && !h_changed[i]) { b->survive[i] = 0; skipped++; }
         }
         if (dev_dst) {

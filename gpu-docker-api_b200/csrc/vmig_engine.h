@@ -52,6 +52,8 @@ public:
     // non-null: page-locked memory the DMA engines can use directly (no staging copy)
     virtual const uint8_t* pinned_src(const BlockRef&) { return nullptr; }
     virtual uint8_t*       pinned_dst(const BlockRef&) { return nullptr; }
+    // how error messages name a block
+    virtual std::string block_name(const BlockRef& b) { return "block at offset " + std::to_string(b.file_off); }
 };
 
 struct LaneStats {
@@ -83,9 +85,11 @@ int  io_threads_default(uint32_t* readers, uint32_t* writers, uint32_t requested
 
 // Run blocks[] through one GPU.  hashes_out[b.table_idx] receives every block's hash.
 //   hash_only : no D2H of data, no writes (block_done(b,false) is still called).
+//   expect    : nullable; expect[b.table_idx] is the hash block b must have.  A block that hashes otherwise fails
+//               the call with VMIG_ECORRUPT before any block of its batch is written (skipped ones included).
 //   err       : call-wide first-error latch shared by all lanes (0 = fine).
 int run_lane(Pipe* pipe, const std::vector<BlockRef>& blocks, BlockIO* io, bool has_prior, bool hash_only,
-             uint32_t readers, uint32_t writers, uint32_t max_slots, uint64_t* hashes_out, LaneStats* stats,
-             std::atomic<int>* err, std::string* err_msg, std::mutex* err_mu);
+             uint32_t readers, uint32_t writers, uint32_t max_slots, const uint64_t* expect, uint64_t* hashes_out,
+             LaneStats* stats, std::atomic<int>* err, std::string* err_msg, std::mutex* err_mu);
 
 }  // namespace vmig

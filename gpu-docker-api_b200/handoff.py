@@ -19,7 +19,8 @@ import os
 from pathlib import Path
 from typing import Callable, Optional
 
-from . import (F_PRUNE, F_VERIFY, GetContainerMergedLayer, GetVolumeMountPoint, VmigError, manifest, migrate_tree)
+from . import (F_PRUNE, F_VERIFY, GetContainerMergedLayer, GetVolumeMountPoint, VmigError, manifest, migrate_tree,
+               restore_tree)
 
 log = logging.getLogger("vmig.handoff")
 _root: dict = {"cwd": None}
@@ -52,24 +53,37 @@ def CopyDirDiffVerified(src, dest, priorTable, outTable) -> dict:
     return CopyDirDiff(src, dest, priorTable, outTable, F_VERIFY | F_PRUNE)
 
 
+def SnapshotDirVerified(src, dest, outTable) -> dict:
+    """utils.SnapshotDirVerified of the cgo shim: a snapshot is re-read through the GPU (VMIG_F_VERIFY) before its
+    table is written, so the table describes what really landed in `dest`."""
+    return CopyDirDiff(src, dest, None, outTable, F_VERIFY)
+
+
+def RestoreDirDiffVerified(snap, snapTable, dest, priorTable, outTable) -> dict:
+    """utils.RestoreDirDiffVerified of the cgo shim: CopyDirDiffVerified from a snapshot that must still match its own
+    block table (vmig_restore_tree); a partial, edited or rotted snapshot fails with VMIG_ECORRUPT."""
+    return restore_tree(snap, snapTable, dest, priorTable or None, outTable or None, flags=F_VERIFY | F_PRUNE)
+
+
 def SnapshotVersion(ctrVersionName: str) -> dict:
     """N1: keep the layer of <rs>-<v> and the XXH64 table of its 4 MiB blocks before the container is deleted."""
     upper = GetContainerMergedLayer(ctrVersionName)
     data, table = snapshotPaths(ctrVersionName)
     data.mkdir(parents=True, exist_ok=True)
-    return CopyDirDiff(upper, data, None, table)
+    return SnapshotDirVerified(upper, data, table)
 
 
 def RollbackFromSnapshot(targetCtrVersionName: str, newContainer: str, seedTable=None) -> dict:
     """N1: fill newContainer's layer with version `target`.  seedTable = the table written FOR newContainer's layer by
     whatever put its present content there; only blocks that differ then travel.  A seed table that no longer
     describes the layer (failed earlier pass, out-of-band change) is detected per file by the engine and that file is
-    copied in full; the result is verified either way."""
-    data, _ = snapshotPaths(targetCtrVersionName)
+    copied in full; the result is verified either way.  The snapshot itself must still match the table it was taken
+    with: one without its table (a snapshot that failed part way) or one that changed since fails the rollback."""
+    data, table = snapshotPaths(targetCtrVersionName)
     upper = GetContainerMergedLayer(newContainer)
     _, newTable = snapshotPaths(newContainer)
     newTable.parent.mkdir(parents=True, exist_ok=True)
-    return CopyDirDiffVerified(data, upper, seedTable, newTable)
+    return RestoreDirDiffVerified(data, table, upper, seedTable, newTable)
 
 
 def HandoffCopy(oldContainer: str, newContainer: str, pause: Callable[[str], None], resume: Callable[[str], None]) -> dict:

@@ -53,6 +53,7 @@ extern "C" {
 #define VMIG_ENOTDIR    (-8)   /* src or dst is not a directory (reference utils/file.go:50-59)  */
 #define VMIG_ESRCCHANGED (-9)  /* a source file shrank while it was being read                  */
 #define VMIG_EVERIFY    (-10)  /* VMIG_F_VERIFY: a destination block does not hash like its source */
+#define VMIG_ECORRUPT   (-11)  /* vmig_restore_tree: the source tree is not the one its block table describes */
 
 /* ---- lifecycle --------------------------------------------------------------------------- */
 /* Idempotent, thread-safe.  gpu_mask bit i selects CUDA device i; 0 = all visible devices.
@@ -155,6 +156,29 @@ typedef struct vmig_stats {
  * written (the reference does no cleanup either: SURVEY.md §8b) but the call never reports
  * success after a short read/write or a CUDA error. */
 int vmig_migrate_tree(const char* src_dir, const char* dst_dir,
+                      const char* prior_table, const char* out_table,
+                      const vmig_opts* opts /*nullable*/, vmig_stats* stats /*nullable*/);
+
+/* Restore a snapshot (a tree a migration wrote together with snap_table, its block table) into dst_dir: exactly
+ * vmig_migrate_tree(snap_dir, dst_dir, prior_table, out_table, opts, stats), except that snap_dir must still be the
+ * tree snap_table describes.  A restore store that puts back whatever happens to be on disk -- a snapshot that
+ * failed part way, was edited, or rotted -- is refused instead:
+ *   - snap_table is required (NULL/empty: VMIG_EINVAL); it is loaded like prior_table (formats 01 and 02, algo 1)
+ *     and its block_bytes must equal the call's (VMIG_ETABLE).  VMIG_F_MOVE_SRC: VMIG_EINVAL.
+ *   - before the destination is touched (before VMIG_F_PRUNE, before any directory is made or block read): the
+ *     walked regular-file paths, hard-linked ones included, must be the table's paths, each with the table's size.
+ *     The table's ino/ctime_ns are not used (a copied snapshot keeps its bytes, not its inodes).
+ *   - every block's XXH64, computed on the GPU as it passes, must equal the table's; a block that does not is never
+ *     written, also where prior_table says the destination already holds it.  A hard-linked path's table hashes
+ *     must equal what its primary hashed, checked before any link is created.
+ * The first difference fails the call with VMIG_ECORRUPT; vmig_last_error() names the path and says whether it is
+ * missing, extra or resized, or names the block and both hashes.  Directories, symlinks, specials and metadata are
+ * not in the table and are not checked.  As always on failure, no out_table is written and the destination may
+ * be partially written (never with a block that failed the check).
+ * With VMIG_F_HASH_ONLY, dst_dir may be NULL: the snapshot is only checked against its table and no destination is
+ * touched (pass out_table = NULL to write nothing at all).
+ * The walk flags (VMIG_F_SKIP_HIDDEN_TOPDIRS) must be those the snapshot's table was written with. */
+int vmig_restore_tree(const char* snap_dir, const char* snap_table, const char* dst_dir,
                       const char* prior_table, const char* out_table,
                       const vmig_opts* opts /*nullable*/, vmig_stats* stats /*nullable*/);
 

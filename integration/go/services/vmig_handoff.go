@@ -54,16 +54,17 @@ func SnapshotVersion(ctrVersionName string) error {
 	if err := os.MkdirAll(data, 0755); err != nil {
 		return errors.Wrapf(err, "mkdir %s", data)
 	}
-	return errors.WithMessagef(utils.CopyDirDiff(upper, data, "", table), "snapshot of %s failed", ctrVersionName)
+	return errors.WithMessagef(utils.SnapshotDirVerified(upper, data, table), "snapshot of %s failed", ctrVersionName)
 }
 
 // N1 -- RollbackFromSnapshot fills newContainer's layer with version `target` of the ReplicaSet.  The new
 // layer was just created from the image, so it is seeded with a plain copy of the snapshot; when the caller
 // has first put the CURRENT version there (seedTable = that version's blocks.vmig, e.g. after a failed
-// roll-forward), only the blocks that differ between the two versions travel.  Replaces the CopyDir of
-// RollbackContainer (replicaset.go:421).
+// roll-forward), only the blocks that differ between the two versions travel.  The snapshot must still match the
+// block table it was taken with: one without its table (a SnapshotVersion that failed part way) or one changed
+// since fails the rollback instead of being restored.  Replaces the CopyDir of RollbackContainer (replicaset.go:421).
 func RollbackFromSnapshot(targetCtrVersionName, newContainer, seedTable string) error {
-	data, _ := snapshotPaths(targetCtrVersionName)
+	data, table := snapshotPaths(targetCtrVersionName)
 	upper, err := utils.GetContainerMergedLayer(newContainer)
 	if err != nil {
 		return errors.WithMessagef(err, "utils.GetContainerMergedLayer failed, container: %s", newContainer)
@@ -74,7 +75,7 @@ func RollbackFromSnapshot(targetCtrVersionName, newContainer, seedTable string) 
 	}
 	// verified + pruned: a seed table that no longer describes the layer is detected per file by the engine (inode/ctime
 	// recorded in the table) and that file is copied in full; the re-hash of the destination is the backstop
-	return errors.WithMessagef(utils.CopyDirDiffVerified(data, upper, seedTable, newTable), "rollback to %s failed", targetCtrVersionName)
+	return errors.WithMessagef(utils.RestoreDirDiffVerified(data, table, upper, seedTable, newTable), "rollback to %s failed", targetCtrVersionName)
 }
 
 // N2 -- HandoffCopy replaces utils.CopyOldMergedToNewContainerMerged in PatchContainer (replicaset.go:333):

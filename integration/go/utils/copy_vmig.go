@@ -59,7 +59,34 @@ func CopyDirDiffVerified(src, dest, priorTable, outTable string) error {
 	return copyDirDiff(src, dest, priorTable, outTable, C.VMIG_F_VERIFY|C.VMIG_F_PRUNE)
 }
 
+// SnapshotDirVerified writes a version snapshot: the copy is re-read through the GPU (VMIG_F_VERIFY) before
+// outTable is written, so the table describes what really landed in dest.
+func SnapshotDirVerified(src, dest, outTable string) error {
+	return copyDirDiff(src, dest, "", outTable, C.VMIG_F_VERIFY)
+}
+
+// RestoreDirDiffVerified is CopyDirDiffVerified from a snapshot that must still be the tree its own block table
+// snapTable describes (vmig_restore_tree): same paths and sizes before dest is touched, every block's hash as it
+// passes.  A snapshot without its table (one that failed part way) or one changed since fails with VMIG_ECORRUPT /
+// VMIG_ETABLE instead of being restored.
+func RestoreDirDiffVerified(snap, snapTable, dest, priorTable, outTable string) error {
+	ct := C.CString(snapTable)
+	defer C.free(unsafe.Pointer(ct))
+	return runDiff("vmig_restore_tree", snap, dest, priorTable, outTable, C.VMIG_F_VERIFY|C.VMIG_F_PRUNE,
+		func(cs, cd, cp, co *C.char, o *C.vmig_opts, st *C.vmig_stats) C.int {
+			return C.vmig_restore_tree(cs, ct, cd, cp, co, o, st)
+		})
+}
+
 func copyDirDiff(src, dest, priorTable, outTable string, flags C.uint32_t) error {
+	return runDiff("vmig_migrate_tree", src, dest, priorTable, outTable, flags,
+		func(cs, cd, cp, co *C.char, o *C.vmig_opts, st *C.vmig_stats) C.int {
+			return C.vmig_migrate_tree(cs, cd, cp, co, o, st)
+		})
+}
+
+func runDiff(what, src, dest, priorTable, outTable string, flags C.uint32_t,
+	call func(cs, cd, cp, co *C.char, o *C.vmig_opts, st *C.vmig_stats) C.int) error {
 	cs, cd := C.CString(src), C.CString(dest)
 	defer C.free(unsafe.Pointer(cs))
 	defer C.free(unsafe.Pointer(cd))
@@ -75,7 +102,7 @@ func copyDirDiff(src, dest, priorTable, outTable string, flags C.uint32_t) error
 	var st C.vmig_stats
 	var o C.vmig_opts // zero value = defaults (all GPUs, 4 MiB blocks)
 	o.flags = flags
-	err := lockedCall("vmig_migrate_tree", func() C.int { return C.vmig_migrate_tree(cs, cd, cp, co, &o, &st) })
+	err := lockedCall(what, func() C.int { return call(cs, cd, cp, co, &o, &st) })
 	if err == nil {
 		log.Infof("vmig: %d bytes, %d/%d blocks skipped, %d files copied in full (stale table), %d pruned, %.2f GiB/s",
 			uint64(st.bytes_total), uint64(st.blocks_skipped), uint64(st.blocks_total), uint64(st.files_untrusted),

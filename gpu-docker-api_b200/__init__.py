@@ -41,7 +41,7 @@ MOVE_DIR_FLAGS = F_MOVE_SRC | F_VERIFY          # what vmig_move_dir passes (inc
 
 EXPORTS = [
     "vmig_init", "vmig_shutdown", "vmig_device_count", "vmig_strerror", "vmig_last_error", "vmig_version",
-    "vmig_migrate_tree", "vmig_restore_tree", "vmig_copy_dir", "vmig_move_dir", "vmig_migrate_buffer", "vmig_host_alloc",
+    "vmig_migrate_tree", "vmig_restore_tree", "vmig_snapshot_tree", "vmig_copy_dir", "vmig_move_dir", "vmig_migrate_buffer", "vmig_host_alloc",
     "vmig_host_free", "vmig_hash_blocks", "vmig_resident_open", "vmig_resident_close", "vmig_resident_fill",
     "vmig_resident_set_len", "vmig_resident_upload", "vmig_resident_download", "vmig_resident_flip",
     "vmig_resident_set_prior", "vmig_resident_pass", "vmig_resident_results", "vmig_table_info_read",
@@ -61,6 +61,14 @@ class Stats(C.Structure):
         "symlinks", "hardlinks", "specials", "kernel_launches", "ns_total", "ns_walk", "ns_plan", "ns_data",
         "ns_meta", "ns_table")] + [("ms_kernel", C.c_double), ("gpus_used", C.c_uint32), ("lanes_used", C.c_uint32), ("pruned", C.c_uint64),
                                                     ("files_untrusted", C.c_uint64), ("files_direct", C.c_uint64)]
+
+    def as_dict(self) -> dict:
+        return {n: getattr(self, n) for n, _ in self._fields_ if n != "reserved"}
+
+
+class SnapshotStats(C.Structure):
+    _fields_ = [(n, C.c_uint64) for n in ("files_linked", "bytes_linked", "files_backfilled", "bytes_backfilled",
+                                          "files_base_untrusted")] + [("reserved", C.c_uint64 * 3)]
 
     def as_dict(self) -> dict:
         return {n: getattr(self, n) for n, _ in self._fields_ if n != "reserved"}
@@ -88,6 +96,8 @@ _sig = {
     "vmig_migrate_tree": (C.c_int, [C.c_char_p, C.c_char_p, C.c_char_p, C.c_char_p, C.POINTER(Opts), C.POINTER(Stats)]),
     "vmig_restore_tree": (C.c_int, [C.c_char_p, C.c_char_p, C.c_char_p, C.c_char_p, C.c_char_p, C.POINTER(Opts),
                                     C.POINTER(Stats)]),
+    "vmig_snapshot_tree": (C.c_int, [C.c_char_p, C.c_char_p, C.c_char_p, C.c_char_p, C.c_char_p, C.POINTER(Opts),
+                                     C.POINTER(Stats), C.POINTER(SnapshotStats)]),
     "vmig_copy_dir": (C.c_int, [C.c_char_p, C.c_char_p]), "vmig_move_dir": (C.c_int, [C.c_char_p, C.c_char_p]),
     "vmig_migrate_buffer": (C.c_int, [C.c_void_p, C.c_void_p, C.c_uint64, C.c_void_p, C.c_void_p, C.c_void_p,
                                       C.POINTER(Opts), C.POINTER(Stats)]),
@@ -242,6 +252,21 @@ def restore_tree(snap, snap_table, dst, prior_table=None, out_table=None, *, gpu
     _check(_lib.vmig_restore_tree(_b(snap), _b(snap_table), _b(dst), _b(prior_table), _b(out_table), C.byref(o),
                                   C.byref(st)), f"vmig_restore_tree({snap} -> {dst})")
     return st.as_dict()
+
+
+def snapshot_tree(src, dst, base=None, base_table=None, out_table=None, *, flags: int = 0, gpu_mask: int = 0,
+                  block_bytes: int = 0, io_threads: int = 0, streams_per_gpu: int = 0, lanes_per_gpu: int = 0) -> dict:
+    """Snapshot `src` into `dst` with its block table `out_table` (required), sharing what did not change with the
+    previous snapshot `base` (taken with `base_table`): unchanged files become hard links to the base's, changed files
+    take their unchanged blocks from the base file.  Without a base it is migrate_tree(src, dst, None, out_table).
+    Returns the migrate_tree counters plus files_linked, bytes_linked, files_backfilled, bytes_backfilled and
+    files_base_untrusted."""
+    o = Opts(gpu_mask=gpu_mask, block_bytes=block_bytes, flags=flags, io_threads=io_threads,
+             streams_per_gpu=streams_per_gpu, lanes_per_gpu=lanes_per_gpu)
+    st, ss = Stats(), SnapshotStats()
+    _check(_lib.vmig_snapshot_tree(_b(src), _b(dst), _b(base), _b(base_table), _b(out_table), C.byref(o), C.byref(st),
+                                   C.byref(ss)), f"vmig_snapshot_tree({src} -> {dst}, base {base})")
+    return {**st.as_dict(), **ss.as_dict()}
 
 
 def hash_tree(src, out_table, *, gpu_mask: int = 0, block_bytes: int = 0) -> dict:

@@ -36,6 +36,8 @@ public:
         bool s_direct = false, d_direct = false;         // this file's descriptor was opened with O_DIRECT
         std::atomic<void*> s_cfh{nullptr}, d_cfh{nullptr};   // cuFile handles of sfd / dfd (VMIG_F_CUFILE)
         std::atomic<bool> wrote{false};                  // at least one block of the file was written in this call
+        const TableFile* base_rec = nullptr;             // vmig_snapshot_tree: the base file still is this record
+        bool solo = true;                                // no other source path is a hard link to this file
     };
     std::string src_root, dst_root;
     int src_root_fd = -1;                // source files are opened beneath this descriptor, never by absolute path
@@ -56,6 +58,77 @@ public:
     }
     std::unique_ptr<FS[]> fs;
     std::mutex stripes[64];
+
+    // vmig_snapshot_tree: the base snapshot whose files supply the blocks K1 found unchanged
+    std::string base_root;
+    std::vector<uint8_t> skipped;                          // per table block: 1 = not written, its bytes are the base file's
+    std::mutex link_mu;
+    std::unordered_map<uint64_t, int64_t> linked_inos;     // base inode linked by this call -> its ctime after the link
+    std::vector<uint32_t> linked_files;
+    std::atomic<uint64_t> n_linked{0}, b_linked{0}, n_backfilled{0}, b_backfilled{0};
+    bool done_on_writer(const BlockRef& b) override { return fs[b.file].base_rec != nullptr; }
+
+    // Last block of a base candidate passed: link the new path to the base file when nothing was written and the link
+    // keeps the snapshot's hard-link structure and metadata equal to the source's, else copy the skipped blocks from the
+    // base file into the new file (block_done then finalizes it like any other).  Runs on a writer (done_on_writer).
+    int finish_from_base(uint32_t f, bool* linked) {
+        FS& s = fs[f];
+        const Entry& e = m->files[f];
+        const TableFile& bf = *s.base_rec;
+        bool any_skipped = false;
+        for (uint64_t r = 0; r < e.n_blocks && !any_skipped; r++) any_skipped = skipped[e.first_block + r] != 0;
+        if (!any_skipped) return VMIG_OK;
+        const std::string bp = pjoin(base_root, e.rel);
+        const int bfd = open(bp.c_str(), O_RDONLY | O_NOFOLLOW | O_CLOEXEC);
+        struct stat bs;
+        bool same = bfd >= 0 && fstat(bfd, &bs) == 0 && S_ISREG(bs.st_mode) && (uint64_t)bs.st_ino == bf.ino;
+        if (same) {
+            const int64_t ct = (int64_t)bs.st_ctim.tv_sec * 1000000000ll + bs.st_ctim.tv_nsec;
+            std::lock_guard<std::mutex> lk(link_mu);
+            auto it = linked_inos.find(bf.ino);
+            same = ct == bf.ctime_ns || (it != linked_inos.end() && it->second == ct);
+        }
+        if (!same) {
+            if (bfd >= 0) close(bfd);
+            return fail(VMIG_ESRCCHANGED, "base file %s changed during the snapshot: the bytes of its unchanged blocks are gone", bp.c_str());
+        }
+        const std::string p = pjoin(dst_root, e.rel);
+        if (!s.wrote.load() && e.size == bf.size && s.solo && file_meta_matches(bfd, e, pol)) {
+            std::lock_guard<std::mutex> lk(link_mu);
+            if (!linked_inos.count(bf.ino)) {
+                bool was_dir = false;
+                int rc = unlink_if_exists(p, &was_dir);
+                if (!rc && was_dir) rc = fail(VMIG_EIO, "%s: a directory is in the way of a regular file", p.c_str());
+                if (!rc && linkat(AT_FDCWD, bp.c_str(), AT_FDCWD, p.c_str(), 0) != 0) rc = fail(VMIG_EIO, "link %s -> %s: %s", p.c_str(), bp.c_str(), errno_str(errno).c_str());
+                struct stat ls;
+                if (!rc && (lstat(p.c_str(), &ls) != 0 || ls.st_ino != bs.st_ino)) {      // the base path was replaced after the fstat
+                    unlink(p.c_str());
+                    rc = fail(VMIG_ESRCCHANGED, "base file %s was replaced during the snapshot", bp.c_str());
+                }
+                close(bfd);
+                if (rc) return rc;
+                linked_inos[bf.ino] = (int64_t)ls.st_ctim.tv_sec * 1000000000ll + ls.st_ctim.tv_nsec;
+                linked_files.push_back(f);
+                n_linked++; b_linked += e.size;
+                *linked = true;
+                return VMIG_OK;
+            }
+        }
+        int dfd; int rc = open_dst(f, &dfd);
+        uint64_t bytes = 0;
+        for (uint64_t r = 0; r < e.n_blocks && !rc;) {
+            if (!skipped[e.first_block + r]) { r++; continue; }
+            uint64_t q = r;
+            while (q < e.n_blocks && skipped[e.first_block + q]) q++;
+            const uint64_t off = r * (uint64_t)block_bytes, len = std::min<uint64_t>(q * (uint64_t)block_bytes, e.size) - off;
+            rc = copy_range(bfd, dfd, off, len, s.d_direct, false, bp);
+            bytes += len; r = q;
+        }
+        close(bfd);
+        if (rc) return rc;
+        n_backfilled++; b_backfilled += bytes;
+        return VMIG_OK;
+    }
 
     // libcufile refuses descriptors whose open flags include O_NOFOLLOW / O_NONBLOCK ("unsupported file open flags"),
     // which is exactly how the safe opens below are made, and F_SETFL cannot clear O_NOFOLLOW.  The descriptor already
@@ -219,11 +292,17 @@ public:
         }
         return VMIG_OK;
     }
-    int block_done(const BlockRef& b, bool) override {
+    int block_done(const BlockRef& b, bool written) override {
         FS& s = fs[b.file];
+        if (!written && s.base_rec) skipped[b.table_idx] = 1;
         if (s.blocks_left.fetch_sub(1) != 1) return VMIG_OK;
         if (hash_only) return VMIG_OK;
         const Entry& e = m->files[b.file];
+        if (s.base_rec) {
+            bool linked = false;
+            int rc = finish_from_base(b.file, &linked);
+            if (rc || linked) return rc;
+        }
         int fd; int rc = open_dst(b.file, &fd);      // also covers "every block was skipped"
         if (rc) return rc;
         const std::string p = pjoin(dst_root, e.rel);
@@ -391,11 +470,21 @@ vmig_opts norm_opts(const vmig_opts* in) {
     return o;
 }
 
+struct SnapshotArgs {
+    const char* base_dir;              // both NULL: a full snapshot
+    const char* base_table;
+    vmig_snapshot_stats* out;          // nullable
+};
+
 // snap_path non-null: vmig_restore_tree -- src_dir must match that block table (match_table before anything touches the
-// destination, every block's hash in the hash-waiter, hard-linked paths before metadata replay)
+// destination, every block's hash in the hash-waiter, hard-linked paths before metadata replay).
+// snapshot non-null: vmig_snapshot_tree -- unchanged files and blocks come from the base (FileIO::finish_from_base).
 int migrate_tree_impl(const char* src_dir, const char* dst_dir, const char* prior_path, const char* out_path,
-                      const vmig_opts* opts_in, vmig_stats* stats_out, const char* snap_path = nullptr)
+                      const vmig_opts* opts_in, vmig_stats* stats_out, const char* snap_path = nullptr,
+                      const SnapshotArgs* snapshot = nullptr)
 {
+    const char* base_dir = snapshot ? snapshot->base_dir : nullptr;
+    const char* base_path = snapshot ? snapshot->base_table : nullptr;
     vmig_stats st; memset(&st, 0, sizeof st);
     const uint64_t t_begin = now_ns();
     if (!src_dir || !*src_dir) return fail(VMIG_EINVAL, "src_dir is NULL/empty");
@@ -440,6 +529,16 @@ int migrate_tree_impl(const char* src_dir, const char* dst_dir, const char* prio
         if (prior.block_bytes != o.block_bytes) return fail(VMIG_ETABLE, "prior table block size %u != %u", prior.block_bytes, o.block_bytes);
         has_prior = true;
     }
+    BlockTable base; bool has_base = false;
+    vmig_snapshot_stats sst_snap; memset(&sst_snap, 0, sizeof sst_snap);
+    if (base_path) {
+        rc = table_load(base_path, &base);
+        if (rc) return rc;
+        if (base.block_bytes != o.block_bytes) return fail(VMIG_ETABLE, "base table block size %u != %u", base.block_bytes, o.block_bytes);
+        // a hard link cannot cross devices, and a base on another filesystem shares nothing with the snapshot
+        struct stat bst, dst_st;
+        has_base = stat(base_dir, &bst) == 0 && stat(dst.c_str(), &dst_st) == 0 && bst.st_dev == dst_st.st_dev;
+    }
     FileIO io;
     io.src_root = src; io.dst_root = dst; io.m = &man; io.pol = default_meta_policy(o.flags); io.hash_only = hash_only;
     io.block_bytes = o.block_bytes;
@@ -466,20 +565,39 @@ int migrate_tree_impl(const char* src_dir, const char* dst_dir, const char* prio
                 BlockRef b; b.file = f; b.file_off = r * (uint64_t)o.block_bytes;
                 b.len = (uint32_t)std::min<uint64_t>(o.block_bytes, e.size - b.file_off);
                 b.table_idx = e.first_block + r; b.prior_hash = 0; b.prior_valid = 0;
-                if (io.fs[f].inplace) {
-                    const TableFile& pf = prior.files[prior.index[e.rel]];
-                    const uint64_t plen = r < prior.blocks_of(pf) ? std::min<uint64_t>(o.block_bytes, pf.size - b.file_off) : 0;
-                    if (plen == b.len) { b.prior_hash = prior.hashes[pf.first_block + r]; b.prior_valid = 1; }
+                // the same rule for a file patched in place and for a snapshot file whose base is trusted
+                const BlockTable* pt = io.fs[f].inplace ? &prior : io.fs[f].base_rec ? &base : nullptr;
+                if (pt) {
+                    const TableFile& pf = io.fs[f].inplace ? prior.files[prior.index[e.rel]] : *io.fs[f].base_rec;
+                    const uint64_t plen = r < pt->blocks_of(pf) ? std::min<uint64_t>(o.block_bytes, pf.size - b.file_off) : 0;
+                    if (plen == b.len) { b.prior_hash = pt->hashes[pf.first_block + r]; b.prior_valid = 1; }
                 }
                 blocks.push_back(b);
             }
         group.clear();
     };
+    bool any_base = false;
+    if (has_base) io.base_root = base_dir;
+    for (auto& e : man.files) if (e.hardlink_of >= 0) io.fs[(size_t)e.hardlink_of].solo = false;
     for (uint32_t f = 0; f < man.files.size(); f++) {
         const Entry& e = man.files[f];
         if (e.hardlink_of >= 0 || e.n_blocks == 0) continue;
         FileIO::FS& s = io.fs[f];
         s.reads_left.store((uint32_t)e.n_blocks); s.blocks_left.store((uint32_t)e.n_blocks);
+        if (has_base) {
+            auto it = base.index.find(e.rel);
+            struct stat bs;
+            // take blocks from a base file only while it still IS the one the base table was written for (its link
+            // count may exceed 1: base files are shared with older snapshots)
+            if (it != base.index.end() && base.files[it->second].ino != 0) {
+                const TableFile& bf = base.files[it->second];
+                const bool ok = lstat(pjoin(io.base_root, e.rel).c_str(), &bs) == 0 && S_ISREG(bs.st_mode) &&
+                                (uint64_t)bs.st_ino == bf.ino && (uint64_t)bs.st_size == bf.size &&
+                                (int64_t)bs.st_ctim.tv_sec * 1000000000ll + bs.st_ctim.tv_nsec == bf.ctime_ns;
+                if (ok) { s.base_rec = &bf; any_base = true; }
+                else sst_snap.files_base_untrusted++;
+            }
+        }
         if (has_prior) {
             auto it = prior.index.find(e.rel);
             struct stat ds;
@@ -499,6 +617,7 @@ int migrate_tree_impl(const char* src_dir, const char* dst_dir, const char* prio
         if (group.size() == 64) flush_group();
     }
     flush_group();
+    if (any_base) io.skipped.assign(man.n_blocks, 0);
     st.ns_plan = now_ns() - t0;
 
     // VMIG_F_PRUNE runs first: what it removes is by definition not in the source, a directory sitting where the source
@@ -508,7 +627,7 @@ int migrate_tree_impl(const char* src_dir, const char* dst_dir, const char* prio
     if (!hash_only) { rc = make_dirs(dst, man); if (rc) return rc; }
 
     t0 = now_ns();
-    rc = run_blocks(blocks, &io, has_prior, hash_only, o, hashes.data(), &st, expect.empty() ? nullptr : expect.data());
+    rc = run_blocks(blocks, &io, has_prior || any_base, hash_only, o, hashes.data(), &st, expect.empty() ? nullptr : expect.data());
     st.ns_data = now_ns() - t0;
     if (rc) { std::string keep = last_error_cstr(); io.close_all(man.files.size()); set_last_error_str(keep); return rc; }
 
@@ -582,6 +701,19 @@ int migrate_tree_impl(const char* src_dir, const char* dst_dir, const char* prio
     }
 
     t0 = now_ns();
+    // A snapshot's table records each file as the call leaves it, so that the next increment can trust it: a linked
+    // path's ctime moved with this call's link to the base inode, and a hard-linked file's with replay_metadata's link
+    // (both after block_done recorded it).  Nothing later in the call touches these inodes.
+    if (snapshot) {
+        std::vector<uint32_t> refresh = io.linked_files;
+        for (uint32_t f = 0; f < man.files.size(); f++) if (!io.fs[f].solo && man.files[f].n_blocks) refresh.push_back(f);
+        for (uint32_t f : refresh) {
+            const std::string p = pjoin(dst, man.files[f].rel);
+            struct stat ls;
+            if (lstat(p.c_str(), &ls) != 0) return fail(VMIG_EIO, "lstat %s: %s", p.c_str(), errno_str(errno).c_str());
+            io.fs[f].id_ino = (uint64_t)ls.st_ino; io.fs[f].id_ctime_ns = (int64_t)ls.st_ctim.tv_sec * 1000000000ll + ls.st_ctim.tv_nsec;
+        }
+    }
     if (out_path && *out_path) {
         BlockTable t; t.block_bytes = o.block_bytes; t.algo = 1;
         t.files.reserve(man.files.size());
@@ -612,6 +744,29 @@ int migrate_tree_impl(const char* src_dir, const char* dst_dir, const char* prio
     st.files = man.files.size(); st.dirs = man.dirs.size();
     st.ns_total = now_ns() - t_begin;
     if (stats_out) *stats_out = st;
+    if (snapshot && snapshot->out) {
+        sst_snap.files_linked = io.n_linked.load(); sst_snap.bytes_linked = io.b_linked.load();
+        sst_snap.files_backfilled = io.n_backfilled.load(); sst_snap.bytes_backfilled = io.b_backfilled.load();
+        *snapshot->out = sst_snap;
+    }
+    return VMIG_OK;
+}
+
+// vmig_snapshot_tree: a base directory equal to the destination, or either one inside the other, is refused -- a
+// link or backfill would read what the same call is writing
+int check_snapshot_paths(const char* dst_dir, const char* base_dir)
+{
+    char* d = realpath(dst_dir, nullptr);
+    if (!d) return fail(VMIG_EIO, "realpath %s: %s", dst_dir, errno_str(errno).c_str());
+    char* b = realpath(base_dir, nullptr);
+    if (!b) { const int e = errno; free(d); return fail(VMIG_EIO, "realpath %s: %s", base_dir, errno_str(e).c_str()); }
+    const std::string ds(d), bs(b);
+    free(d); free(b);
+    auto inside = [](const std::string& a, const std::string& root) {
+        return a == root || (a.size() > root.size() && a.compare(0, root.size(), root) == 0 && (root == "/" || a[root.size()] == '/'));
+    };
+    if (inside(ds, bs) || inside(bs, ds))
+        return fail(VMIG_EINVAL, "base_dir %s and dst_dir %s are the same directory or one is inside the other", bs.c_str(), ds.c_str());
     return VMIG_OK;
 }
 
@@ -655,6 +810,22 @@ int vmig_restore_tree(const char* snap_dir, const char* snap_table, const char* 
     if (!snap_table || !*snap_table) return fail(VMIG_EINVAL, "snap_table is NULL/empty: a snapshot is only restored against its block table");
     if (opts && (opts->flags & VMIG_F_MOVE_SRC)) return fail(VMIG_EINVAL, "VMIG_F_MOVE_SRC: a restore never consumes the snapshot");
     return migrate_tree_impl(snap_dir, dst_dir, prior_table, out_table, opts, stats, snap_table);
+}
+int vmig_snapshot_tree(const char* src_dir, const char* dst_dir, const char* base_dir, const char* base_table,
+                       const char* out_table, const vmig_opts* opts, vmig_stats* stats, vmig_snapshot_stats* snap_stats)
+{
+    const bool has_dir = base_dir && *base_dir, has_table = base_table && *base_table;
+    if (has_dir != has_table) return fail(VMIG_EINVAL, "base_dir and base_table go together: one of them is NULL/empty");
+    if (!out_table || !*out_table) return fail(VMIG_EINVAL, "out_table is NULL/empty: a snapshot is only restored against its block table");
+    const uint32_t flags = norm_opts(opts).flags;          // VMIG_CUFILE=1 in the environment is refused too
+    if (flags & VMIG_F_MOVE_SRC) return fail(VMIG_EINVAL, "VMIG_F_MOVE_SRC: a snapshot never consumes its source");
+    if (flags & VMIG_F_HASH_ONLY) return fail(VMIG_EINVAL, "VMIG_F_HASH_ONLY: a snapshot writes its destination");
+    if (flags & VMIG_F_CUFILE) return fail(VMIG_EINVAL, "VMIG_F_CUFILE: not supported for snapshots (a backfilled file would mix cuFile and buffered writes)");
+    if (!dst_dir || !*dst_dir) return fail(VMIG_EINVAL, "dst_dir is NULL/empty");
+    if (has_dir) { const int rc = check_snapshot_paths(dst_dir, base_dir); if (rc) return rc; }
+    if (snap_stats) memset(snap_stats, 0, sizeof *snap_stats);
+    const SnapshotArgs sa{has_dir ? base_dir : nullptr, has_table ? base_table : nullptr, snap_stats};
+    return migrate_tree_impl(src_dir, dst_dir, nullptr, out_table, opts, stats, nullptr, &sa);
 }
 int vmig_copy_dir(const char* src_dir, const char* dst_dir) { return migrate_tree_impl(src_dir, dst_dir, nullptr, nullptr, nullptr, nullptr); }
 int vmig_move_dir(const char* src_dir, const char* dst_dir)

@@ -487,7 +487,7 @@ struct Batch {
     std::vector<uint8_t> survive;   // per block, filled after hashing
     uint64_t t_disp = 0, t_read = 0, t_sub = 0, t_hash = 0, t_d2h = 0, t_done = 0;   // VMIG_TRACE
 };
-struct IoTask { Batch* batch; size_t i0, i1; };
+struct IoTask { Batch* batch; size_t i0, i1; bool done_only = false; };   // done_only: skipped blocks, block_done alone
 
 static void bind_thread(const DeviceInfo& d) {
     if (d.cpus.empty()) return;
@@ -765,11 +765,16 @@ int run_lane(Pipe* pipe, const std::vector<BlockRef>& blocks, BlockIO* io, bool 
                 }
             }
             // blocks that need no write are complete now
+            const bool writes = !tasks.empty();
             for (size_t i = 0; i < n; i++) {
-                const bool written_later = !tasks.empty() && b->survive[i];
+                const bool written_later = writes && b->survive[i];
                 if (!written_later) {
                     const bool was_written = !b->failed && !hash_only && direct_dst && b->survive[i];
                     if (b->failed) continue;            // do not finalize files of a failed call
+                    if (!was_written && !hash_only && io->done_on_writer(blocks[b->b0 + i])) {
+                        tasks.push_back({b, b->b0 + i, b->b0 + i + 1, true});
+                        continue;
+                    }
                     int rc = io->block_done(blocks[b->b0 + i], was_written);
                     if (rc) set_err(rc);
                     if (was_written) { std::lock_guard<std::mutex> lk(stat_mu); stats->bytes_written += blocks[b->b0 + i].len; }
@@ -795,8 +800,12 @@ int run_lane(Pipe* pipe, const std::vector<BlockRef>& blocks, BlockIO* io, bool 
                 const uint64_t w0 = now_ns();
                 for (size_t i = k.i0; i < k.i1; i++) {
                     if (err->load()) break;
-                    int rc = dev_dst ? io->write_block_dev(blocks[i], sl.d_buf, slot_off[i]) : io->write_block(blocks[i], sl.h_out + slot_off[i]);
-                    if (!rc) { wrote += blocks[i].len; rc = io->block_done(blocks[i], true); }
+                    int rc = VMIG_OK;
+                    if (!k.done_only) {
+                        rc = dev_dst ? io->write_block_dev(blocks[i], sl.d_buf, slot_off[i]) : io->write_block(blocks[i], sl.h_out + slot_off[i]);
+                        if (!rc) wrote += blocks[i].len;
+                    }
+                    if (!rc) rc = io->block_done(blocks[i], !k.done_only);
                     if (rc) { set_err(rc); break; }
                 }
                 wr_busy += now_ns() - w0;

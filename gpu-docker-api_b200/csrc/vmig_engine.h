@@ -37,6 +37,9 @@ public:
     virtual int  write_block(const BlockRef& b, const uint8_t* src) = 0;
     // called exactly once per block when it needs nothing more (written == false: skipped)
     virtual int  block_done(const BlockRef&, bool /*written*/) { return VMIG_OK; }
+    // true: block_done of this block, if skipped, may do file-sized work (vmig_snapshot_tree links or backfills the file
+    // when its last block passes); it then runs on a writer thread under the block's write key, not on the d2h-waiter
+    virtual bool done_on_writer(const BlockRef&) { return false; }
     // writes with the same key are issued by one writer thread, in order (a file takes writes from one
     // thread at a time anyway); backends without such a constraint spread the keys
     virtual uint32_t write_key(const BlockRef& b) { return b.file; }

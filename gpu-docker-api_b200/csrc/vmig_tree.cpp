@@ -268,6 +268,51 @@ int unlink_if_exists(const std::string& path, bool* was_dir)
     return VMIG_OK;
 }
 
+int copy_range(int in_fd, int out_fd, uint64_t off, uint64_t len, bool out_direct, bool rw_only, const std::string& what)
+{
+    uint64_t done = 0;
+    if (!out_direct && !rw_only) {
+        while (done < len) {
+            loff_t a = (loff_t)(off + done), b = a;
+            const ssize_t n = copy_file_range(in_fd, &a, out_fd, &b, (size_t)(len - done), 0);
+            if (n > 0) { done += (uint64_t)n; continue; }
+            if (n == 0) return fail(VMIG_ESRCCHANGED, "%s ends at %llu, before %llu", what.c_str(), (unsigned long long)(off + done), (unsigned long long)(off + len));
+            if (errno == EINTR) continue;
+            if (errno == ENOSYS || errno == EXDEV || errno == EINVAL || errno == EOPNOTSUPP) break;     // the rest by pread/pwrite
+            return fail(VMIG_EIO, "copy_file_range %s: %s", what.c_str(), errno_str(errno).c_str());
+        }
+    }
+    const size_t kSector = 4096, kChunk = 1u << 20;
+    void* mem = nullptr;
+    if (done < len && posix_memalign(&mem, kSector, kChunk) != 0) return fail(VMIG_ENOMEM, "copy buffer for %s", what.c_str());
+    uint8_t* buf = (uint8_t*)mem;
+    int rc = VMIG_OK;
+    while (done < len && !rc) {
+        const size_t want = (size_t)std::min<uint64_t>(kChunk, len - done);
+        size_t got = 0;
+        while (got < want && !rc) {
+            const ssize_t r = pread(in_fd, buf + got, want - got, (off_t)(off + done + got));
+            if (r < 0 && errno == EINTR) continue;
+            if (r < 0) rc = fail(VMIG_EIO, "pread %s: %s", what.c_str(), errno_str(errno).c_str());
+            else if (r == 0) rc = fail(VMIG_ESRCCHANGED, "%s ends at %llu, before %llu", what.c_str(), (unsigned long long)(off + done + got), (unsigned long long)(off + len));
+            else got += (size_t)r;
+        }
+        const size_t out_len = out_direct ? (size_t)align_up(want, kSector) : want;
+        if (!rc) memset(buf + want, 0, out_len - want);
+        size_t put = 0;
+        while (put < out_len && !rc) {
+            const ssize_t w = pwrite(out_fd, buf + put, out_len - put, (off_t)(off + done + put));
+            if (w < 0 && errno == EINTR) continue;
+            if (w < 0) rc = fail(VMIG_EIO, "pwrite (copy of %s): %s", what.c_str(), errno_str(errno).c_str());
+            else if (w == 0) rc = fail(VMIG_EIO, "pwrite (copy of %s): wrote 0 bytes", what.c_str());
+            else put += (size_t)w;
+        }
+        done += want;
+    }
+    free(mem);
+    return rc;
+}
+
 int make_dirs(const std::string& dst_root, const Manifest& m)
 {
     for (size_t i = 1; i < m.dirs.size(); i++) {

@@ -78,5 +78,11 @@ int remove_source(const std::string& src_root, const Manifest& m);
 int prune_extras(const std::string& dst_root, const Manifest& m, bool dry_run, uint64_t* n_extras);
 // Remove whatever non-directory sits at path (tar replaces existing entries).  ENOENT is fine.
 int unlink_if_exists(const std::string& path, bool* was_dir);
+// Copy bytes [off, off + len) of in_fd to the same offsets of out_fd (a snapshot file's unchanged blocks, taken from
+// the base snapshot's file).  copy_file_range, which may share extents on filesystems that reflink; pread/pwrite where
+// the kernel or filesystem refuses it (ENOSYS, EXDEV, EINVAL, EOPNOTSUPP) or rw_only is set.  out_direct: out_fd was
+// opened O_DIRECT, off must be a multiple of 4096, and the bytes go out in whole sectors through an aligned buffer,
+// zero-padded past off + len (the caller truncates the file to its size).  in_fd ending early is VMIG_ESRCCHANGED.
+int copy_range(int in_fd, int out_fd, uint64_t off, uint64_t len, bool out_direct, bool rw_only, const std::string& what);
 
 }  // namespace vmig

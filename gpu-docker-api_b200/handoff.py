@@ -20,7 +20,7 @@ from pathlib import Path
 from typing import Callable, Optional
 
 from . import (F_PRUNE, F_VERIFY, GetContainerMergedLayer, GetVolumeMountPoint, VmigError, manifest, migrate_tree,
-               restore_tree)
+               restore_tree, snapshot_tree)
 
 log = logging.getLogger("vmig.handoff")
 _root: dict = {"cwd": None}
@@ -59,6 +59,13 @@ def SnapshotDirVerified(src, dest, outTable) -> dict:
     return CopyDirDiff(src, dest, None, outTable, F_VERIFY)
 
 
+def SnapshotDirIncrementalVerified(src, dest, baseDir, baseTable, outTable) -> dict:
+    """utils.SnapshotDirIncrementalVerified of the cgo shim: SnapshotDirVerified that shares what did not change with
+    the previous snapshot baseDir (vmig_snapshot_tree).  The re-read covers linked files too, so a base that rotted
+    without moving its ctime is caught when the snapshot is taken."""
+    return snapshot_tree(src, dest, baseDir, baseTable, outTable, flags=F_VERIFY)
+
+
 def RestoreDirDiffVerified(snap, snapTable, dest, priorTable, outTable) -> dict:
     """utils.RestoreDirDiffVerified of the cgo shim: CopyDirDiffVerified from a snapshot that must still match its own
     block table (vmig_restore_tree); a partial, edited or rotted snapshot fails with VMIG_ECORRUPT."""
@@ -71,6 +78,36 @@ def SnapshotVersion(ctrVersionName: str) -> dict:
     data, table = snapshotPaths(ctrVersionName)
     data.mkdir(parents=True, exist_ok=True)
     return SnapshotDirVerified(upper, data, table)
+
+
+def baseVersion(ctrVersionName: str) -> Optional[str]:
+    """The newest earlier version <rs>-<k> (k < v) whose directory holds both diff/ and blocks.vmig, or None."""
+    rs, v = ctrVersionName.split("-")[0], int(ctrVersionName.rsplit("-", 1)[1])
+    best = -1
+    parent = versionDir(ctrVersionName).parent
+    for d in (parent.iterdir() if parent.is_dir() else ()):
+        k = d.name[len(rs) + 1:]
+        if not d.name.startswith(rs + "-") or not k.isdigit() or not best < int(k) < v:
+            continue
+        if (d / "diff").is_dir() and (d / "blocks.vmig").is_file():
+            best = int(k)
+    return None if best < 0 else f"{rs}-{best}"
+
+
+def SnapshotVersionIncremental(ctrVersionName: str) -> dict:
+    """N1, as setToMergeMap calls it: SnapshotVersion that shares unchanged files and blocks with the newest earlier
+    snapshot of the ReplicaSet (a full SnapshotDirVerified when there is none).  That version's blocks.vmig may have
+    been written last by HandoffCopy for the container's layer, not for diff/ (a snapshot of it that failed part
+    way): the identities it records then name no file under diff/, the engine trusts none of them, and the result is
+    a plain verified copy."""
+    upper = GetContainerMergedLayer(ctrVersionName)
+    data, table = snapshotPaths(ctrVersionName)
+    data.mkdir(parents=True, exist_ok=True)
+    base = baseVersion(ctrVersionName)
+    if base is None:
+        return SnapshotDirVerified(upper, data, table)
+    baseData, baseTable = snapshotPaths(base)
+    return SnapshotDirIncrementalVerified(upper, data, baseData, baseTable, table)
 
 
 def RollbackFromSnapshot(targetCtrVersionName: str, newContainer: str, seedTable=None) -> dict:

@@ -182,6 +182,51 @@ int vmig_restore_tree(const char* snap_dir, const char* snap_table, const char* 
                       const char* prior_table, const char* out_table,
                       const vmig_opts* opts /*nullable*/, vmig_stats* stats /*nullable*/);
 
+/* Incremental version snapshot: what vmig_snapshot_tree took from the base snapshot instead of the GPU's staging ring. */
+typedef struct vmig_snapshot_stats {
+    uint64_t files_linked;          /* regular files that are a hard link to the base snapshot's file: no data written */
+    uint64_t bytes_linked;
+    uint64_t files_backfilled;      /* new files whose unchanged blocks were copied from the base file, not the ring */
+    uint64_t bytes_backfilled;
+    uint64_t files_base_untrusted;  /* base table names the path but the base file is no longer the one it recorded */
+    uint64_t reserved[3];
+} vmig_snapshot_stats;
+
+/* Write a version snapshot of src_dir into dst_dir (a new, empty directory, or a partial earlier attempt with
+ * VMIG_F_PRUNE) and its block table into out_table, sharing what did not change with the previous snapshot:
+ * base_dir, written together with base_table by an earlier vmig_snapshot_tree / vmig_migrate_tree.
+ *   - base_dir == base_table == NULL: a full snapshot, the copy vmig_migrate_tree(src_dir, dst_dir, NULL, out_table,
+ *     opts, stats) makes.  Only one of them given: VMIG_EINVAL.  out_table NULL/empty: VMIG_EINVAL (a snapshot is restored against it).
+ *   - VMIG_F_MOVE_SRC, VMIG_F_HASH_ONLY and VMIG_F_CUFILE: VMIG_EINVAL.  So is a base_dir that is dst_dir, or lies
+ *     inside it, or contains it (compared by real path).  VMIG_F_VERIFY, VMIG_F_PRUNE, VMIG_F_DIRECT_IO,
+ *     lanes_per_gpu and gpu_mask act as in a migration.
+ *   - base_table loads like a prior table (formats 01 and 02); its block_bytes must equal the call's (VMIG_ETABLE).
+ * A source regular file is a base candidate when dst_dir and base_dir are on one device, the base table records the
+ * path with an inode, and the base file is still that regular file with that inode, ctime and size (its link count
+ * may exceed 1: base files are shared with older snapshots).  A candidate's blocks are compared on the GPU with the
+ * base table's hashes, exactly as the in-place diff path compares with a prior table; unchanged blocks are neither
+ * copied back from HBM nor written.  When the file's last block has passed:
+ *   - link: the new path becomes a hard link to the base file if no block was written, the sizes are equal, the
+ *     source file has no hard-link partner in src_dir, no other path of this call was linked to that base inode, and
+ *     the base inode already carries the owner, mode and mtime the copy would get.  A linked inode's metadata is
+ *     never changed (that would change older snapshots too);
+ *   - backfill: otherwise the file is written new: changed blocks from the ring, unchanged ones copied from the base
+ *     file at the same offsets (copy_file_range, or pread/pwrite where that is refused), then its metadata applied.
+ * Before it links or copies from a base file the call re-checks its inode and ctime; a base file that changed during
+ * the call fails it with VMIG_ESRCCHANGED naming the path (a retry copies that file in full).  Files that are not
+ * candidates are copied as by vmig_migrate_tree; where the base table named the path, files_base_untrusted counts it.
+ * Empty files are never linked.  out_table records the inode and ctime of every file as this call leaves it, linked
+ * and hard-linked files included (vmig_migrate_tree records a hard-linked file before its links are made), so that the
+ * next snapshot can use each one as a base.
+ * Linking moves the base inode's ctime, so the base table's own record of that file goes stale: a later snapshot
+ * against that same base copies the file in full, and vmig_restore_tree does not read identities at all.
+ * snap_stats (nullable) receives the counters above; stats as for vmig_migrate_tree (bytes_written counts ring
+ * writes only). */
+int vmig_snapshot_tree(const char* src_dir, const char* dst_dir,
+                       const char* base_dir /*nullable*/, const char* base_table /*nullable*/,
+                       const char* out_table, const vmig_opts* opts /*nullable*/,
+                       vmig_stats* stats /*nullable*/, vmig_snapshot_stats* snap_stats /*nullable*/);
+
 /* utils.CopyDir(src, dest) (reference utils/copy.go:21-27) == vmig_migrate_tree with defaults. */
 int vmig_copy_dir(const char* src_dir, const char* dst_dir);
 

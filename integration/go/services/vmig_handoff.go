@@ -19,6 +19,7 @@ import (
 	"os"
 	"path/filepath"
 	"runtime"
+	"strconv"
 	"strings"
 	"unsafe"
 
@@ -55,6 +56,58 @@ func SnapshotVersion(ctrVersionName string) error {
 		return errors.Wrapf(err, "mkdir %s", data)
 	}
 	return errors.WithMessagef(utils.SnapshotDirVerified(upper, data, table), "snapshot of %s failed", ctrVersionName)
+}
+
+// baseVersion returns the newest earlier version <rs>-<k> (k < v) whose directory holds both diff/ and blocks.vmig.
+func baseVersion(ctrVersionName string) (string, bool) {
+	rs := strings.Split(ctrVersionName, "-")[0]
+	v, err := strconv.Atoi(ctrVersionName[strings.LastIndex(ctrVersionName, "-")+1:])
+	if err != nil {
+		return "", false
+	}
+	entries, _ := os.ReadDir(filepath.Dir(versionDir(ctrVersionName)))
+	best := -1
+	for _, e := range entries {
+		k, err := strconv.Atoi(strings.TrimPrefix(e.Name(), rs+"-"))
+		if !strings.HasPrefix(e.Name(), rs+"-") || err != nil || k <= best || k >= v {
+			continue
+		}
+		d := filepath.Join(filepath.Dir(versionDir(ctrVersionName)), e.Name())
+		if st, err := os.Stat(filepath.Join(d, "diff")); err != nil || !st.IsDir() {
+			continue
+		}
+		if st, err := os.Stat(filepath.Join(d, "blocks.vmig")); err != nil || !st.Mode().IsRegular() {
+			continue
+		}
+		best = k
+	}
+	if best < 0 {
+		return "", false
+	}
+	return rs + "-" + strconv.Itoa(best), true
+}
+
+// N1 -- SnapshotVersionIncremental is what setToMergeMap calls: SnapshotVersion that shares unchanged files and blocks
+// with the newest earlier snapshot of the ReplicaSet (a full SnapshotDirVerified when there is none).  That version's
+// blocks.vmig may have been written last by HandoffCopy for the container's layer, not for diff/ (a snapshot of it that
+// failed part way): the identities it records then name no file under diff/, the engine trusts none of them, and the
+// result is a plain verified copy.
+func SnapshotVersionIncremental(ctrVersionName string) error {
+	upper, err := utils.GetContainerMergedLayer(ctrVersionName)
+	if err != nil {
+		return errors.WithMessagef(err, "utils.GetContainerMergedLayer failed, container: %s", ctrVersionName)
+	}
+	data, table := snapshotPaths(ctrVersionName)
+	if err := os.MkdirAll(data, 0755); err != nil {
+		return errors.Wrapf(err, "mkdir %s", data)
+	}
+	base, ok := baseVersion(ctrVersionName)
+	if !ok {
+		return errors.WithMessagef(utils.SnapshotDirVerified(upper, data, table), "snapshot of %s failed", ctrVersionName)
+	}
+	baseData, baseTable := snapshotPaths(base)
+	return errors.WithMessagef(utils.SnapshotDirIncrementalVerified(upper, data, baseData, baseTable, table),
+		"snapshot of %s against %s failed", ctrVersionName, base)
 }
 
 // N1 -- RollbackFromSnapshot fills newContainer's layer with version `target` of the ReplicaSet.  The new

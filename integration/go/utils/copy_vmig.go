@@ -73,20 +73,34 @@ func RestoreDirDiffVerified(snap, snapTable, dest, priorTable, outTable string) 
 	ct := C.CString(snapTable)
 	defer C.free(unsafe.Pointer(ct))
 	return runDiff("vmig_restore_tree", snap, dest, priorTable, outTable, C.VMIG_F_VERIFY|C.VMIG_F_PRUNE,
-		func(cs, cd, cp, co *C.char, o *C.vmig_opts, st *C.vmig_stats) C.int {
+		func(cs, cd, cp, co *C.char, o *C.vmig_opts, st *C.vmig_stats, _ *C.vmig_snapshot_stats) C.int {
 			return C.vmig_restore_tree(cs, ct, cd, cp, co, o, st)
+		})
+}
+
+// SnapshotDirIncrementalVerified is SnapshotDirVerified that shares what did not change with the previous snapshot
+// baseDir, taken with baseTable (vmig_snapshot_tree): an unchanged file becomes a hard link to the base's, a changed
+// file takes its unchanged blocks from the base file.  The re-read (VMIG_F_VERIFY) covers linked files too, so a base
+// that rotted without moving its ctime is caught when the snapshot is taken.
+func SnapshotDirIncrementalVerified(src, dest, baseDir, baseTable, outTable string) error {
+	cb, ct := C.CString(baseDir), C.CString(baseTable)
+	defer C.free(unsafe.Pointer(cb))
+	defer C.free(unsafe.Pointer(ct))
+	return runDiff("vmig_snapshot_tree", src, dest, "", outTable, C.VMIG_F_VERIFY,
+		func(cs, cd, _, co *C.char, o *C.vmig_opts, st *C.vmig_stats, ss *C.vmig_snapshot_stats) C.int {
+			return C.vmig_snapshot_tree(cs, cd, cb, ct, co, o, st, ss)
 		})
 }
 
 func copyDirDiff(src, dest, priorTable, outTable string, flags C.uint32_t) error {
 	return runDiff("vmig_migrate_tree", src, dest, priorTable, outTable, flags,
-		func(cs, cd, cp, co *C.char, o *C.vmig_opts, st *C.vmig_stats) C.int {
+		func(cs, cd, cp, co *C.char, o *C.vmig_opts, st *C.vmig_stats, _ *C.vmig_snapshot_stats) C.int {
 			return C.vmig_migrate_tree(cs, cd, cp, co, o, st)
 		})
 }
 
 func runDiff(what, src, dest, priorTable, outTable string, flags C.uint32_t,
-	call func(cs, cd, cp, co *C.char, o *C.vmig_opts, st *C.vmig_stats) C.int) error {
+	call func(cs, cd, cp, co *C.char, o *C.vmig_opts, st *C.vmig_stats, ss *C.vmig_snapshot_stats) C.int) error {
 	cs, cd := C.CString(src), C.CString(dest)
 	defer C.free(unsafe.Pointer(cs))
 	defer C.free(unsafe.Pointer(cd))
@@ -100,13 +114,16 @@ func runDiff(what, src, dest, priorTable, outTable string, flags C.uint32_t,
 		defer C.free(unsafe.Pointer(co))
 	}
 	var st C.vmig_stats
-	var o C.vmig_opts // zero value = defaults (all GPUs, 4 MiB blocks)
+	var ss C.vmig_snapshot_stats // filled by vmig_snapshot_tree only
+	var o C.vmig_opts            // zero value = defaults (all GPUs, 4 MiB blocks)
 	o.flags = flags
-	err := lockedCall(what, func() C.int { return call(cs, cd, cp, co, &o, &st) })
+	err := lockedCall(what, func() C.int { return call(cs, cd, cp, co, &o, &st, &ss) })
 	if err == nil {
-		log.Infof("vmig: %d bytes, %d/%d blocks skipped, %d files copied in full (stale table), %d pruned, %.2f GiB/s",
+		log.Infof("vmig: %d bytes, %d/%d blocks skipped, %d files copied in full (stale table), %d pruned, "+
+			"%d files linked to the base snapshot (%d bytes), %d backfilled from it (%d bytes), %d base files stale, %.2f GiB/s",
 			uint64(st.bytes_total), uint64(st.blocks_skipped), uint64(st.blocks_total), uint64(st.files_untrusted),
-			uint64(st.pruned), float64(st.bytes_total)/float64(st.ns_total)*1e9/(1<<30))
+			uint64(st.pruned), uint64(ss.files_linked), uint64(ss.bytes_linked), uint64(ss.files_backfilled),
+			uint64(ss.bytes_backfilled), uint64(ss.files_base_untrusted), float64(st.bytes_total)/float64(st.ns_total)*1e9/(1<<30))
 	}
 	return err
 }

@@ -69,11 +69,8 @@ def test_k1_ragged_blocks_vs_oracle(vm, orc):
     assert ms > 0
 
 
-def test_k1_chunk_and_ring_boundaries_vs_oracle(vm, orc):
-    """The kernel stages 1 KiB chunks through a 6-stage shared-memory ring: every length k*1024 + {-33..33 around the
-    stripe and chunk edges} for k = 1..14 (two wraps of the ring), plus the 6 KiB / 12 KiB wrap points +-1 and lengths that
-    end exactly where a stage is refilled.  One launch holds all of them next to full 4 MiB blocks (long and short
-    quads share a ring)."""
+def ring_boundary_case():
+    """(buf, offs, lens) of test_k1_chunk_and_ring_boundaries_vs_oracle."""
     rng = np.random.default_rng(22)
     deltas = (-33, -32, -31, -1, 0, 1, 31, 32, 33)
     lens = sorted({k * 1024 + d for k in range(1, 15) for d in deltas} | {6 * 1024 * m + d for m in (1, 2, 3, 4) for d in (-1, 0, 1)}
@@ -82,6 +79,15 @@ def test_k1_chunk_and_ring_boundaries_vs_oracle(vm, orc):
     rng.shuffle(lens)
     offs = np.cumsum(np.concatenate([[3], lens[:-1].astype(np.uint64) + rng.integers(0, 17, len(lens) - 1).astype(np.uint64)])).astype(np.uint64)
     buf = rng.integers(0, 256, int(offs[-1] + lens[-1]), dtype=np.uint8)
+    return buf, offs, lens
+
+
+def test_k1_chunk_and_ring_boundaries_vs_oracle(vm, orc):
+    """The kernel stages 1 KiB chunks through a 6-stage shared-memory ring: every length k*1024 + {-33..33 around the
+    stripe and chunk edges} for k = 1..14 (two wraps of the ring), plus the 6 KiB / 12 KiB wrap points +-1 and lengths that
+    end exactly where a stage is refilled.  One launch holds all of them next to full 4 MiB blocks (long and short
+    quads share a ring)."""
+    buf, offs, lens = ring_boundary_case()
     got, _ = vm.hash_blocks(buf, offs, lens)
     want = orc.hash_blocks(buf, offs, lens)
     bad = np.nonzero(got != want)[0]

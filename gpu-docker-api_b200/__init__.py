@@ -33,7 +33,8 @@ LIB_PATH = _HERE / "libvmig.so"
 
 VMIG_OK, VMIG_EINVAL, VMIG_ENOGPU, VMIG_ECUDA, VMIG_EIO = 0, -1, -2, -3, -4
 VMIG_ENOMEM, VMIG_ETABLE, VMIG_EFAULT, VMIG_ENOTDIR, VMIG_ESRCCHANGED, VMIG_EVERIFY = -5, -6, -7, -8, -9, -10
-VMIG_ECORRUPT = -11
+VMIG_ECORRUPT, VMIG_ECANCELED = -11, -12
+PHASES = ("IDLE", "WALK", "DATA", "VERIFY", "META", "PRUNE", "TABLE", "UNLINK", "DONE")     # VMIG_PHASE_* by value
 F_MOVE_SRC, F_SKIP_HIDDEN_TOPDIRS, F_MTIME_NS, F_NO_METADATA, F_HASH_ONLY, F_VERIFY = 0x01, 0x02, 0x04, 0x08, 0x10, 0x20
 F_PRUNE, F_DIRECT_IO, F_CUFILE = 0x40, 0x80, 0x100
 BLOCK_BYTES = 4 << 20
@@ -46,13 +47,20 @@ EXPORTS = [
     "vmig_resident_set_len", "vmig_resident_upload", "vmig_resident_download", "vmig_resident_flip",
     "vmig_resident_set_prior", "vmig_resident_pass", "vmig_resident_results", "vmig_table_info_read",
     "vmig_table_hashes", "vmig_dir_size", "vmig_to_bytes", "vmig_datagen_files", "vmig_manifest", "vmig_link_probe", "vmig_thread_plan",
+    "vmig_ctl_open", "vmig_ctl_cancel", "vmig_ctl_progress", "vmig_ctl_close",
 ]
 
 
 class Opts(C.Structure):
     _fields_ = [("gpu_mask", C.c_uint32), ("block_bytes", C.c_uint32), ("streams_per_gpu", C.c_uint32),
                 ("flags", C.c_uint32), ("io_threads", C.c_uint32), ("lanes_per_gpu", C.c_uint32),
-                ("reserved", C.c_uint32 * 2)]
+                ("ctl", C.c_uint32), ("reserved", C.c_uint32)]
+
+
+class Progress(C.Structure):
+    _fields_ = [("phase", C.c_uint32), ("running", C.c_uint32)] + [(n, C.c_uint64) for n in (
+        "bytes_total", "blocks_total", "bytes_hashed", "blocks_hashed", "bytes_written", "bytes_verified")] + \
+        [("reserved", C.c_uint64 * 4)]
 
 
 class Stats(C.Structure):
@@ -121,6 +129,8 @@ _sig = {
     "vmig_manifest": (C.c_int, [C.c_char_p, C.c_uint32, C.c_uint32, C.c_char_p, C.POINTER(Stats)]),
     "vmig_link_probe": (C.c_int, [C.c_int, C.c_uint64, C.POINTER(C.c_double)]),
     "vmig_thread_plan": (C.c_int, [C.c_uint32, C.c_uint32, C.c_uint32, C.c_int, C.POINTER(C.c_uint32), C.POINTER(C.c_uint32)]),
+    "vmig_ctl_open": (C.c_int, [C.POINTER(C.c_uint32)]), "vmig_ctl_cancel": (C.c_int, [C.c_uint32]),
+    "vmig_ctl_progress": (C.c_int, [C.c_uint32, C.POINTER(Progress)]), "vmig_ctl_close": (C.c_int, [C.c_uint32]),
 }
 for _n, (_r, _a) in _sig.items():
     _f = getattr(_lib, _n)
@@ -165,6 +175,42 @@ def device_count() -> int:
 
 def _b(p) -> Optional[bytes]:
     return None if p is None else os.fsencode(p)
+
+
+class Ctl:
+    """A call control (vmig_ctl_*): pass it as ``ctl=`` to migrate_tree, restore_tree, snapshot_tree or migrate_buffer,
+    then cancel() from any thread (the call raises VmigError(VMIG_ECANCELED)) or read progress() while it runs.  ctypes
+    releases the GIL during the call.  One control serves one call at a time; a deadline is a threading.Timer."""
+
+    def __init__(self):
+        i = C.c_uint32(0)
+        _check(_lib.vmig_ctl_open(C.byref(i)), "vmig_ctl_open")
+        self.id = i.value
+
+    def cancel(self) -> None:
+        _check(_lib.vmig_ctl_cancel(self.id), "vmig_ctl_cancel")
+
+    def progress(self) -> dict:
+        p = Progress()
+        _check(_lib.vmig_ctl_progress(self.id, C.byref(p)), "vmig_ctl_progress")
+        d = {n: getattr(p, n) for n, _ in p._fields_ if n != "reserved"}
+        d["phase_name"] = PHASES[d["phase"]] if d["phase"] < len(PHASES) else "?"
+        return d
+
+    def close(self) -> None:
+        if self.id:
+            _check(_lib.vmig_ctl_close(self.id), "vmig_ctl_close")
+            self.id = 0
+
+    def __enter__(self) -> "Ctl":
+        return self
+
+    def __exit__(self, *exc) -> None:
+        self.close()
+
+
+def _ctl_id(ctl: Optional[Ctl]) -> int:
+    return 0 if ctl is None else ctl.id
 
 
 # ------------------------------------------------------------------------------------------------
@@ -233,9 +279,10 @@ def ToBytes(origin: str) -> int:
 # ------------------------------------------------------------------------------------------------
 # engine entry points
 def migrate_tree(src, dst, prior_table=None, out_table=None, *, gpu_mask: int = 0, flags: int = 0,
-                 block_bytes: int = 0, io_threads: int = 0, streams_per_gpu: int = 0, lanes_per_gpu: int = 0) -> dict:
+                 block_bytes: int = 0, io_threads: int = 0, streams_per_gpu: int = 0, lanes_per_gpu: int = 0,
+                 ctl: Optional[Ctl] = None) -> dict:
     o = Opts(gpu_mask=gpu_mask, block_bytes=block_bytes, flags=flags, io_threads=io_threads,
-             streams_per_gpu=streams_per_gpu, lanes_per_gpu=lanes_per_gpu)
+             streams_per_gpu=streams_per_gpu, lanes_per_gpu=lanes_per_gpu, ctl=_ctl_id(ctl))
     st = Stats()
     _check(_lib.vmig_migrate_tree(_b(src), _b(dst), _b(prior_table), _b(out_table), C.byref(o), C.byref(st)),
            f"vmig_migrate_tree({src} -> {dst})")
@@ -243,11 +290,12 @@ def migrate_tree(src, dst, prior_table=None, out_table=None, *, gpu_mask: int = 
 
 
 def restore_tree(snap, snap_table, dst, prior_table=None, out_table=None, *, gpu_mask: int = 0, flags: int = 0,
-                 block_bytes: int = 0, io_threads: int = 0, streams_per_gpu: int = 0, lanes_per_gpu: int = 0) -> dict:
+                 block_bytes: int = 0, io_threads: int = 0, streams_per_gpu: int = 0, lanes_per_gpu: int = 0,
+                 ctl: Optional[Ctl] = None) -> dict:
     """migrate_tree(snap, dst, ...) that first requires `snap` to still be the tree `snap_table` describes (same
     paths and sizes, every block's hash): VMIG_ECORRUPT otherwise.  flags=F_HASH_ONLY with dst=None only checks."""
     o = Opts(gpu_mask=gpu_mask, block_bytes=block_bytes, flags=flags, io_threads=io_threads,
-             streams_per_gpu=streams_per_gpu, lanes_per_gpu=lanes_per_gpu)
+             streams_per_gpu=streams_per_gpu, lanes_per_gpu=lanes_per_gpu, ctl=_ctl_id(ctl))
     st = Stats()
     _check(_lib.vmig_restore_tree(_b(snap), _b(snap_table), _b(dst), _b(prior_table), _b(out_table), C.byref(o),
                                   C.byref(st)), f"vmig_restore_tree({snap} -> {dst})")
@@ -255,14 +303,15 @@ def restore_tree(snap, snap_table, dst, prior_table=None, out_table=None, *, gpu
 
 
 def snapshot_tree(src, dst, base=None, base_table=None, out_table=None, *, flags: int = 0, gpu_mask: int = 0,
-                  block_bytes: int = 0, io_threads: int = 0, streams_per_gpu: int = 0, lanes_per_gpu: int = 0) -> dict:
+                  block_bytes: int = 0, io_threads: int = 0, streams_per_gpu: int = 0, lanes_per_gpu: int = 0,
+                  ctl: Optional[Ctl] = None) -> dict:
     """Snapshot `src` into `dst` with its block table `out_table` (required), sharing what did not change with the
     previous snapshot `base` (taken with `base_table`): unchanged files become hard links to the base's, changed files
     take their unchanged blocks from the base file.  Without a base it is migrate_tree(src, dst, None, out_table).
     Returns the migrate_tree counters plus files_linked, bytes_linked, files_backfilled, bytes_backfilled and
     files_base_untrusted."""
     o = Opts(gpu_mask=gpu_mask, block_bytes=block_bytes, flags=flags, io_threads=io_threads,
-             streams_per_gpu=streams_per_gpu, lanes_per_gpu=lanes_per_gpu)
+             streams_per_gpu=streams_per_gpu, lanes_per_gpu=lanes_per_gpu, ctl=_ctl_id(ctl))
     st, ss = Stats(), SnapshotStats()
     _check(_lib.vmig_snapshot_tree(_b(src), _b(dst), _b(base), _b(base_table), _b(out_table), C.byref(o), C.byref(st),
                                    C.byref(ss)), f"vmig_snapshot_tree({src} -> {dst}, base {base})")
@@ -303,7 +352,7 @@ class PinnedBuffer:
 
 
 def migrate_buffer(src: np.ndarray, dst: Optional[np.ndarray], prior_hashes=None, prior_valid=None, *,
-                   gpu_mask: int = 0, flags: int = 0, block_bytes: int = 0):
+                   gpu_mask: int = 0, flags: int = 0, block_bytes: int = 0, ctl: Optional[Ctl] = None):
     """Host buffer -> host buffer through H2D / hash / diff / D2H.  Returns (hashes, stats)."""
     bb = block_bytes or BLOCK_BYTES
     n = src.size
@@ -311,7 +360,7 @@ def migrate_buffer(src: np.ndarray, dst: Optional[np.ndarray], prior_hashes=None
     out = np.zeros(nb, dtype=np.uint64)
     ph = None if prior_hashes is None else np.ascontiguousarray(prior_hashes, dtype=np.uint64)
     pv = None if prior_valid is None else np.ascontiguousarray(prior_valid, dtype=np.uint8)
-    o = Opts(gpu_mask=gpu_mask, block_bytes=block_bytes, flags=flags)
+    o = Opts(gpu_mask=gpu_mask, block_bytes=block_bytes, flags=flags, ctl=_ctl_id(ctl))
     st = Stats()
     _check(_lib.vmig_migrate_buffer(src.ctypes.data, None if dst is None else dst.ctypes.data, n,
                                     None if ph is None else ph.ctypes.data, None if pv is None else pv.ctypes.data,

@@ -13,15 +13,100 @@
 #include <unistd.h>
 #include <sys/stat.h>
 #include <algorithm>
+#include <condition_variable>
 #include <unordered_map>
+#include <unordered_set>
 #include <thread>
 #include <cmath>
 
 using namespace vmig;
 
+void vmig::CallCtl::cancel()
+{
+    cancelled.store(1);
+    {
+        std::lock_guard<std::mutex> lk(mu);
+        int none = 0;
+        if (latch) latch->compare_exchange_strong(none, VMIG_ECANCELED);
+    }
+    ctx_wake_waiters();             // a call waiting for a staging pipe
+}
+
 namespace {
 
 inline std::string pjoin(const std::string& a, const std::string& b) { return b == "." ? a : a + "/" + b; }
+
+// ---------------------------------------------------------------------------------------------
+// controls (vmig_ctl_*) and the calls in flight (vmig_shutdown cancels them and waits for them)
+std::mutex g_ctl_mu;
+std::unordered_map<uint32_t, std::shared_ptr<CallCtl>> g_ctls;
+uint32_t g_ctl_next = 1;
+std::mutex g_calls_mu;
+std::condition_variable g_calls_cv;
+std::unordered_set<CallCtl*> g_calls;
+
+const char* phase_name(uint32_t p)
+{
+    static const char* const names[] = {"IDLE", "WALK", "DATA", "VERIFY", "META", "PRUNE", "TABLE", "UNLINK", "DONE"};
+    return p <= VMIG_PHASE_DONE ? names[p] : "?";
+}
+
+// One data-path call: attached to the caller's control (vmig_opts.ctl) or to a private one, and counted as in flight.
+class CallScope {
+    std::shared_ptr<CallCtl> held;
+public:
+    CallCtl* ctl = nullptr;
+    int attach(uint32_t id) {
+        if (id) {
+            std::lock_guard<std::mutex> lk(g_ctl_mu);
+            auto it = g_ctls.find(id);
+            if (it == g_ctls.end()) return fail(VMIG_EINVAL, "vmig_opts.ctl %u is not an open control", id);
+            if (it->second->running.load()) return fail(VMIG_EINVAL, "control %u is already attached to a call in flight", id);
+            held = it->second;
+            held->running.store(1);
+        } else {
+            held = std::make_shared<CallCtl>();
+            held->running.store(1);
+        }
+        ctl = held.get();
+        ctl->phase.store(VMIG_PHASE_IDLE);
+        for (auto* c : {&ctl->bytes_total, &ctl->blocks_total, &ctl->bytes_hashed, &ctl->blocks_hashed, &ctl->bytes_written, &ctl->bytes_verified})
+            c->store(0);
+        std::lock_guard<std::mutex> lk(g_calls_mu);
+        g_calls.insert(ctl);
+        return VMIG_OK;
+    }
+    const std::atomic<int>* cancel() const { return &ctl->cancelled; }
+    void phase(uint32_t p) { ctl->phase.store(p); }
+    // VMIG_ECANCELED: vmig_last_error() names the phase the call stopped in
+    int finish(int rc) {
+        if (rc == VMIG_OK) ctl->phase.store(VMIG_PHASE_DONE);
+        if (rc == VMIG_ECANCELED) {
+            const std::string why = last_error_cstr();
+            fail(VMIG_ECANCELED, "cancelled in phase %s: %s", phase_name(ctl->phase.load()), why.c_str());
+        }
+        return rc;
+    }
+    ~CallScope() {
+        if (!ctl) return;
+        { std::lock_guard<std::mutex> lk(g_ctl_mu); ctl->running.store(0); }
+        std::lock_guard<std::mutex> lk(g_calls_mu);
+        g_calls.erase(ctl);
+        g_calls_cv.notify_all();
+    }
+};
+
+// The block pipeline's first-error latch, reachable by CallCtl::cancel while run_blocks runs
+struct LatchLink {
+    CallCtl* c;
+    LatchLink(CallCtl* ctl, std::atomic<int>* latch) : c(ctl) {
+        std::lock_guard<std::mutex> lk(c->mu);
+        c->latch = latch;
+        int none = 0;
+        if (c->cancelled.load()) latch->compare_exchange_strong(none, VMIG_ECANCELED);
+    }
+    ~LatchLink() { std::lock_guard<std::mutex> lk(c->mu); c->latch = nullptr; }
+};
 
 // ---------------------------------------------------------------------------------------------
 // file-backed BlockIO
@@ -66,6 +151,7 @@ public:
     std::unordered_map<uint64_t, int64_t> linked_inos;     // base inode linked by this call -> its ctime after the link
     std::vector<uint32_t> linked_files;
     std::atomic<uint64_t> n_linked{0}, b_linked{0}, n_backfilled{0}, b_backfilled{0};
+    const std::atomic<int>* cancel = nullptr;              // the call's cancel flag: checked per backfill chunk
     bool done_on_writer(const BlockRef& b) override { return fs[b.file].base_rec != nullptr; }
 
     // Last block of a base candidate passed: link the new path to the base file when nothing was written and the link
@@ -121,7 +207,7 @@ public:
             uint64_t q = r;
             while (q < e.n_blocks && skipped[e.first_block + q]) q++;
             const uint64_t off = r * (uint64_t)block_bytes, len = std::min<uint64_t>(q * (uint64_t)block_bytes, e.size) - off;
-            rc = copy_range(bfd, dfd, off, len, s.d_direct, false, bp);
+            rc = copy_range(bfd, dfd, off, len, s.d_direct, false, bp, cancel);
             bytes += len; r = q;
         }
         close(bfd);
@@ -359,8 +445,9 @@ bool is_pinned(const void* p) {
 // ---------------------------------------------------------------------------------------------
 // run a block list over the selected GPUs: n_gpus x lanes_per_gpu lanes, whole files per lane (LPT by bytes);
 // contiguous byte-balanced ranges only when there are fewer than two files per lane
+// ctl: the call's control; a cancel sets this pipeline's first-error latch.  verify: progress goes to bytes_verified.
 int run_blocks(const std::vector<BlockRef>& blocks, BlockIO* io, bool has_prior, bool hash_only, const vmig_opts& o,
-               uint64_t* hashes, vmig_stats* st, const uint64_t* expect = nullptr)
+               uint64_t* hashes, vmig_stats* st, CallCtl* ctl, bool verify, const uint64_t* expect = nullptr)
 {
     std::vector<DeviceInfo> devs;
     int rc = ctx_select(o.gpu_mask, &devs);
@@ -407,9 +494,14 @@ int run_blocks(const std::vector<BlockRef>& blocks, BlockIO* io, bool has_prior,
             }
         }
     }
+    std::atomic<int> err{0}; std::string err_msg; std::mutex err_mu;
+    LatchLink link(ctl, &err);
     std::vector<Pipe*> pipes;
-    rc = ctx_acquire_pipes(lane_devs, &pipes);
+    rc = ctx_acquire_pipes(lane_devs, &pipes, &ctl->cancelled);
     if (rc) return rc;
+    LaneProgress prog;
+    if (verify) prog.hashed_bytes = &ctl->bytes_verified;
+    else { prog.hashed_bytes = &ctl->bytes_hashed; prog.hashed_blocks = &ctl->blocks_hashed; prog.written = &ctl->bytes_written; }
     uint32_t readers, writers;       // sized AFTER the pipes are checked out: the count of lanes in flight includes this call's
     {
         std::unordered_map<uint32_t, int> seen;                  // blocks are interleaved across <= 64 files
@@ -417,12 +509,12 @@ int run_blocks(const std::vector<BlockRef>& blocks, BlockIO* io, bool has_prior,
         // "many files" is a property of what ONE lane sees: 100 x 1 GiB over 8 lanes is 12 large files per lane
         io_threads_default(&readers, &writers, o.io_threads, lanes, std::min(n_gpus, lanes), seen.size() / lanes >= 32, has_prior, hash_only);
     }
-    std::atomic<int> err{0}; std::string err_msg; std::mutex err_mu;
     std::vector<LaneStats> ls(lanes);
     std::vector<std::thread> th;
     for (size_t i = 0; i < lanes; i++)
         th.emplace_back([&, i] {
-            run_lane(pipes[i], share[i], io, has_prior, hash_only, readers, writers, o.streams_per_gpu, expect, hashes, &ls[i], &err, &err_msg, &err_mu);
+            run_lane(pipes[i], share[i], io, has_prior, hash_only, readers, writers, o.streams_per_gpu, expect, hashes, &ls[i], &err, &err_msg,
+                     &err_mu, prog);
         });
     for (auto& t : th) t.join();
     for (size_t i = 0; i < lanes; i++) ctx_release_pipe(pipes[i]);
@@ -432,6 +524,7 @@ int run_blocks(const std::vector<BlockRef>& blocks, BlockIO* io, bool has_prior,
     }
     st->gpus_used = (uint32_t)std::min(n_gpus, lanes);
     st->lanes_used = (uint32_t)lanes;          // lanes the block list was sharded over
+    if (err.load() == VMIG_ECANCELED && err_msg.empty()) return fail(VMIG_ECANCELED, "the block pipeline issued no new work after the cancel");
     if (err.load()) { set_last_error_str(err_msg); return err.load(); }
     return VMIG_OK;
 }
@@ -479,16 +572,30 @@ struct SnapshotArgs {
 // snap_path non-null: vmig_restore_tree -- src_dir must match that block table (match_table before anything touches the
 // destination, every block's hash in the hash-waiter, hard-linked paths before metadata replay).
 // snapshot non-null: vmig_snapshot_tree -- unchanged files and blocks come from the base (FileIO::finish_from_base).
+int migrate_tree_body(CallScope& call, const char* src_dir, const char* dst_dir, const char* prior_path, const char* out_path,
+                      const vmig_opts& o, vmig_stats* stats_out, const char* snap_path, const SnapshotArgs* snapshot);
+
 int migrate_tree_impl(const char* src_dir, const char* dst_dir, const char* prior_path, const char* out_path,
                       const vmig_opts* opts_in, vmig_stats* stats_out, const char* snap_path = nullptr,
                       const SnapshotArgs* snapshot = nullptr)
 {
+    const vmig_opts o = norm_opts(opts_in);
+    CallScope call;
+    const int rc = call.attach(o.ctl);
+    if (rc) return rc;
+    return call.finish(migrate_tree_body(call, src_dir, dst_dir, prior_path, out_path, o, stats_out, snap_path, snapshot));
+}
+
+int migrate_tree_body(CallScope& call, const char* src_dir, const char* dst_dir, const char* prior_path, const char* out_path,
+                      const vmig_opts& o, vmig_stats* stats_out, const char* snap_path, const SnapshotArgs* snapshot)
+{
     const char* base_dir = snapshot ? snapshot->base_dir : nullptr;
     const char* base_path = snapshot ? snapshot->base_table : nullptr;
+    CallCtl* ctl = call.ctl;
+    const std::atomic<int>* cancel = call.cancel();
     vmig_stats st; memset(&st, 0, sizeof st);
     const uint64_t t_begin = now_ns();
     if (!src_dir || !*src_dir) return fail(VMIG_EINVAL, "src_dir is NULL/empty");
-    vmig_opts o = norm_opts(opts_in);
     const bool hash_only = (o.flags & VMIG_F_HASH_ONLY) != 0;
     if (!hash_only && (!dst_dir || !*dst_dir)) return fail(VMIG_EINVAL, "dst_dir is NULL/empty");
     if (o.block_bytes & 4095u) return fail(VMIG_EINVAL, "block_bytes %u is not a multiple of 4096", o.block_bytes);
@@ -501,6 +608,7 @@ int migrate_tree_impl(const char* src_dir, const char* dst_dir, const char* prio
         if (stat(dst.c_str(), &sst) != 0) return fail(VMIG_EIO, "stat %s: %s", dst.c_str(), errno_str(errno).c_str());
         if (!S_ISDIR(sst.st_mode)) return fail(VMIG_ENOTDIR, "%s is not a directory", dst.c_str());
     }
+    if (cancel->load()) return fail(VMIG_ECANCELED, "the control was cancelled before the call started");
     // make sure a GPU is there before touching the destination: no CPU fallback
     std::vector<DeviceInfo> devs;
     int rc = ctx_select(o.gpu_mask, &devs);
@@ -508,9 +616,11 @@ int migrate_tree_impl(const char* src_dir, const char* dst_dir, const char* prio
 
     Manifest man;
     uint64_t t0 = now_ns();
-    rc = walk_tree(src, o.block_bytes, (o.flags & VMIG_F_SKIP_HIDDEN_TOPDIRS) != 0, &man);
+    call.phase(VMIG_PHASE_WALK);
+    rc = walk_tree(src, o.block_bytes, (o.flags & VMIG_F_SKIP_HIDDEN_TOPDIRS) != 0, &man, cancel);
     if (rc) return rc;
     st.ns_walk = now_ns() - t0;
+    ctl->bytes_total.store(man.bytes_total); ctl->blocks_total.store(man.n_blocks);
 
     t0 = now_ns();
     std::vector<uint64_t> expect;
@@ -545,6 +655,7 @@ int migrate_tree_impl(const char* src_dir, const char* dst_dir, const char* prio
     io.corrupt_block = env_long("VMIG_CORRUPT_BLOCK", -1);
     io.direct = (o.flags & VMIG_F_DIRECT_IO) != 0;
     io.cufile = (o.flags & VMIG_F_CUFILE) != 0;
+    io.cancel = cancel;
     if (io.cufile) { rc = cufile_open(); if (rc) return rc; }
     rc = io.open_root(); if (rc) return rc;
     io.fs.reset(new FileIO::FS[man.files.size() ? man.files.size() : 1]);
@@ -623,15 +734,23 @@ int migrate_tree_impl(const char* src_dir, const char* dst_dir, const char* prio
     // VMIG_F_PRUNE runs first: what it removes is by definition not in the source, a directory sitting where the source
     // now has a file (or the reverse) is out of the way before anything is created, and the directory mtimes restored
     // at the end are not disturbed by unlinks
-    if ((o.flags & VMIG_F_PRUNE) && !hash_only) { rc = prune_extras(dst, man, false, &st.pruned); if (rc) return rc; }
+    if ((o.flags & VMIG_F_PRUNE) && !hash_only) {
+        call.phase(VMIG_PHASE_PRUNE);
+        rc = prune_extras(dst, man, false, &st.pruned, cancel);
+        if (rc) return rc;
+    }
+    call.phase(VMIG_PHASE_DATA);
+    if (cancel->load()) return fail(VMIG_ECANCELED, "before the destination's directories were made");
     if (!hash_only) { rc = make_dirs(dst, man); if (rc) return rc; }
 
     t0 = now_ns();
-    rc = run_blocks(blocks, &io, has_prior || any_base, hash_only, o, hashes.data(), &st, expect.empty() ? nullptr : expect.data());
+    rc = run_blocks(blocks, &io, has_prior || any_base, hash_only, o, hashes.data(), &st, ctl, false, expect.empty() ? nullptr : expect.data());
     st.ns_data = now_ns() - t0;
     if (rc) { std::string keep = last_error_cstr(); io.close_all(man.files.size()); set_last_error_str(keep); return rc; }
 
     t0 = now_ns();
+    call.phase(VMIG_PHASE_META);
+    if (cancel->load()) return fail(VMIG_ECANCELED, "after the data pass, before any metadata step");
     for (auto& e : man.files)                      // hard-linked paths share their primary's hashes
         if (e.hardlink_of >= 0) {
             const Entry& p = man.files[(size_t)e.hardlink_of];
@@ -646,8 +765,10 @@ int migrate_tree_impl(const char* src_dir, const char* dst_dir, const char* prio
             }
         }
     if (!hash_only) {
+        size_t steps = 0;
         for (auto& e : man.files) {                // empty regular files carry no blocks
             if (e.hardlink_of >= 0 || e.n_blocks) continue;
+            if (steps++ % kMetaCheckEvery == 0 && cancel->load()) return fail(VMIG_ECANCELED, "before creating %s", e.rel.c_str());
             const std::string p = pjoin(dst, e.rel);
             bool was_dir = false;
             rc = unlink_if_exists(p, &was_dir); if (rc) return rc;
@@ -663,12 +784,13 @@ int migrate_tree_impl(const char* src_dir, const char* dst_dir, const char* prio
             close(fd);
             if (rc) return rc;
         }
-        rc = replay_metadata(dst, man, io.pol, &st.symlinks, &st.hardlinks, &st.specials);
+        rc = replay_metadata(dst, man, io.pol, &st.symlinks, &st.hardlinks, &st.specials, cancel);
         if (rc) return rc;
     }
     st.ns_meta = now_ns() - t0;
 
     if ((o.flags & VMIG_F_VERIFY) && !hash_only) {
+        call.phase(VMIG_PHASE_VERIFY);
         // read the destination back through the same GPU path (hash only) and compare block tables
         FileIO vio;
         vio.src_root = dst; vio.dst_root = dst; vio.m = &man; vio.pol = io.pol; vio.hash_only = true;
@@ -685,7 +807,7 @@ int migrate_tree_impl(const char* src_dir, const char* dst_dir, const char* prio
         for (auto& b : vblocks) { b.prior_hash = 0; b.prior_valid = 0; }
         std::vector<uint64_t> vh(man.n_blocks, 0);
         vmig_stats vst; memset(&vst, 0, sizeof vst);
-        rc = run_blocks(vblocks, &vio, false, true, o, vh.data(), &vst);
+        rc = run_blocks(vblocks, &vio, false, true, o, vh.data(), &vst, ctl, true);
         if (rc) { std::string keep = last_error_cstr(); vio.close_all(man.files.size()); set_last_error_str(keep); return rc; }
         st.kernel_launches += vst.kernel_launches; st.ms_kernel += vst.ms_kernel; st.bytes_h2d += vst.bytes_h2d;
         for (auto& b : vblocks)
@@ -695,12 +817,13 @@ int migrate_tree_impl(const char* src_dir, const char* dst_dir, const char* prio
                             (unsigned long long)vh[b.table_idx], (unsigned long long)hashes[b.table_idx]);
         if (o.flags & VMIG_F_PRUNE) {               // the destination's entry set must now equal the source's
             uint64_t extras = 0;
-            rc = prune_extras(dst, man, true, &extras); if (rc) return rc;
+            rc = prune_extras(dst, man, true, &extras, cancel); if (rc) return rc;
             if (extras) return fail(VMIG_EVERIFY, "verify: %llu destination entries are not in the source after pruning", (unsigned long long)extras);
         }
     }
 
     t0 = now_ns();
+    call.phase(VMIG_PHASE_TABLE);
     // A snapshot's table records each file as the call leaves it, so that the next increment can trust it: a linked
     // path's ctime moved with this call's link to the base inode, and a hard-linked file's with replay_metadata's link
     // (both after block_done recorded it).  Nothing later in the call touches these inodes.
@@ -723,7 +846,7 @@ int migrate_tree_impl(const char* src_dir, const char* dst_dir, const char* prio
             t.files.push_back({e.rel, e.size, e.first_block, own ? io.fs[f].id_ino : 0, own ? io.fs[f].id_ctime_ns : 0});
         }
         t.hashes = hashes;
-        rc = table_store(out_path, t);
+        rc = table_store(out_path, t, cancel);
         if (rc) return rc;
     }
     st.ns_table = now_ns() - t0;
@@ -731,11 +854,20 @@ int migrate_tree_impl(const char* src_dir, const char* dst_dir, const char* prio
     if ((o.flags & VMIG_F_MOVE_SRC) && !hash_only) {
         // the old volume's data is about to be unlinked: deferred write-back errors (ENOSPC / EIO on delayed
         // allocation, network filesystems) must surface first.  A no-op on tmpfs; one flush on a disk.
+        // a cancelled call leaves no table, also when the cancel comes after the table was renamed into place
+        auto cancelled = [&](const char* when) {
+            if (out_path && *out_path) unlink(out_path);
+            return fail(VMIG_ECANCELED, "%s (source left in place)", when);
+        };
+        if (cancel->load()) return cancelled("before the destination was flushed");
         int dfd = open(dst.c_str(), O_RDONLY | O_DIRECTORY | O_CLOEXEC);
         if (dfd < 0) return fail(VMIG_EIO, "open %s: %s", dst.c_str(), errno_str(errno).c_str());
         const int sr = syncfs(dfd); const int se = errno;
         close(dfd);
         if (sr != 0) return fail(VMIG_EIO, "syncfs %s: %s (source left in place)", dst.c_str(), errno_str(se).c_str());
+        if (cancel->load()) return cancelled("before the first unlink");
+        // the point of no return: a half-unlinked source is worse than a finished move, so a cancel is no longer honoured
+        call.phase(VMIG_PHASE_UNLINK);
         rc = remove_source(src, man); if (rc) return rc;
     }
 
@@ -776,7 +908,67 @@ int check_snapshot_paths(const char* dst_dir, const char* base_dir)
 extern "C" {
 
 int vmig_init(uint32_t gpu_mask) { return ctx_init(gpu_mask); }
-void vmig_shutdown(void) { ctx_shutdown(); cufile_shutdown(); }
+void vmig_shutdown(void)
+{
+    {
+        // calls in flight hold pipes and cuFile handles: cancel them and wait until they have returned
+        std::unique_lock<std::mutex> lk(g_calls_mu);
+        while (!g_calls.empty()) {
+            for (CallCtl* c : g_calls) c->cancel();
+            g_calls_cv.wait(lk);
+        }
+    }
+    ctx_shutdown(); cufile_shutdown();
+}
+
+int vmig_ctl_open(uint32_t* id)
+{
+    if (!id) return fail(VMIG_EINVAL, "null id pointer");
+    std::lock_guard<std::mutex> lk(g_ctl_mu);
+    if (g_ctl_next == 0) return fail(VMIG_ENOMEM, "control ids exhausted (they are never reused within a process)");
+    *id = g_ctl_next++;
+    g_ctls.emplace(*id, std::make_shared<CallCtl>());
+    return VMIG_OK;
+}
+int vmig_ctl_cancel(uint32_t id)
+{
+    std::shared_ptr<CallCtl> c;
+    {
+        std::lock_guard<std::mutex> lk(g_ctl_mu);
+        auto it = g_ctls.find(id);
+        if (it == g_ctls.end()) return fail(VMIG_EINVAL, "control %u is not open", id);
+        c = it->second;
+    }
+    c->cancel();
+    return VMIG_OK;
+}
+int vmig_ctl_progress(uint32_t id, vmig_progress* out)
+{
+    if (!out) return fail(VMIG_EINVAL, "null progress pointer");
+    std::shared_ptr<CallCtl> c;
+    {
+        std::lock_guard<std::mutex> lk(g_ctl_mu);
+        auto it = g_ctls.find(id);
+        if (it == g_ctls.end()) return fail(VMIG_EINVAL, "control %u is not open", id);
+        c = it->second;
+    }
+    memset(out, 0, sizeof *out);
+    out->phase = c->phase.load(); out->running = c->running.load();
+    const auto r = std::memory_order_relaxed;
+    out->bytes_total = c->bytes_total.load(r); out->blocks_total = c->blocks_total.load(r);
+    out->bytes_hashed = c->bytes_hashed.load(r); out->blocks_hashed = c->blocks_hashed.load(r);
+    out->bytes_written = c->bytes_written.load(r); out->bytes_verified = c->bytes_verified.load(r);
+    return VMIG_OK;
+}
+int vmig_ctl_close(uint32_t id)
+{
+    std::lock_guard<std::mutex> lk(g_ctl_mu);
+    auto it = g_ctls.find(id);
+    if (it == g_ctls.end()) return fail(VMIG_EINVAL, "control %u is not open", id);
+    if (it->second->running.load()) return fail(VMIG_EINVAL, "control %u is attached to a call in flight", id);
+    g_ctls.erase(it);
+    return VMIG_OK;
+}
 int vmig_device_count(void) { return ctx_device_count(); }
 const char* vmig_last_error(void) { return last_error_cstr(); }
 const char* vmig_version(void) { return "libvmig 0.2 (abi 2, sm_90a)"; }
@@ -795,6 +987,7 @@ const char* vmig_strerror(int code)
     case VMIG_ESRCCHANGED: return "source changed during migration";
     case VMIG_EVERIFY: return "destination does not verify against the source";
     case VMIG_ECORRUPT: return "source tree does not match its block table";
+    case VMIG_ECANCELED: return "call cancelled";
     default: return "unknown vmig error";
     }
 }
@@ -861,8 +1054,13 @@ int vmig_migrate_buffer(const void* src, void* dst, uint64_t nbytes, const uint6
     const bool hash_only = (o.flags & VMIG_F_HASH_ONLY) != 0;
     if (!src || (!dst && !hash_only)) return fail(VMIG_EINVAL, "null buffer");
     if ((o.block_bytes & 4095u) || o.block_bytes > pipe_slot_bytes()) return fail(VMIG_EINVAL, "bad block_bytes %u", o.block_bytes);
-    std::vector<DeviceInfo> devs; int rc = ctx_select(o.gpu_mask, &devs); if (rc) return rc;
+    CallScope call;
+    int rc = call.attach(o.ctl); if (rc) return rc;
+    if (call.cancel()->load()) return call.finish(fail(VMIG_ECANCELED, "the control was cancelled before the call started"));
+    std::vector<DeviceInfo> devs; rc = ctx_select(o.gpu_mask, &devs); if (rc) return rc;
     const uint64_t nb = (nbytes + o.block_bytes - 1) / o.block_bytes;
+    call.ctl->bytes_total.store(nbytes); call.ctl->blocks_total.store(nb);
+    call.phase(VMIG_PHASE_DATA);
     std::vector<BlockRef> blocks(nb);
     const bool has_prior = prior_hashes != nullptr && prior_valid != nullptr;
     for (uint64_t i = 0; i < nb; i++) {
@@ -873,12 +1071,12 @@ int vmig_migrate_buffer(const void* src, void* dst, uint64_t nbytes, const uint6
     MemIO io; io.src = (const uint8_t*)src; io.dst = (uint8_t*)dst;
     io.src_pinned = is_pinned(src); io.dst_pinned = !hash_only && is_pinned(dst);
     std::vector<uint64_t> hashes(nb);
-    rc = run_blocks(blocks, &io, has_prior, hash_only, o, hashes.data(), &st);
-    if (rc) return rc;
+    rc = run_blocks(blocks, &io, has_prior, hash_only, o, hashes.data(), &st, call.ctl, false);
+    if (rc) return call.finish(rc);
     if (out_hashes && nb) memcpy(out_hashes, hashes.data(), nb * 8);
     st.bytes_total = nbytes; st.blocks_total = nb; st.ns_total = st.ns_data = now_ns() - t0;
     if (stats) *stats = st;
-    return VMIG_OK;
+    return call.finish(VMIG_OK);
 }
 
 int vmig_hash_blocks(int gpu, const void* host_buf, const uint64_t* offs, const uint32_t* lens, uint64_t n,
@@ -896,7 +1094,10 @@ int vmig_hash_blocks(int gpu, const void* host_buf, const uint64_t* offs, const 
     }
     MemIO io; io.src = (const uint8_t*)host_buf; io.dst = nullptr;   // staged: arbitrary offsets become 512-B aligned in HBM
     vmig_stats st; memset(&st, 0, sizeof st);
-    rc = run_blocks(blocks, &io, false, true, o, out_hashes, &st);
+    CallScope call;                  // not cancellable by the caller; vmig_shutdown still waits for it
+    rc = call.attach(0); if (rc) return rc;
+    call.phase(VMIG_PHASE_DATA);
+    rc = call.finish(run_blocks(blocks, &io, false, true, o, out_hashes, &st, call.ctl, false));
     if (kernel_ms) *kernel_ms = st.ms_kernel;
     return rc;
 }

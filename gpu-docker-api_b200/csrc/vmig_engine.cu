@@ -327,7 +327,7 @@ static std::atomic<long> g_active_lanes{0};     // pipes checked out by calls in
 // whole set is reserved in ONE step under the lock -- a call that needs k pipes of one GPU never holds
 // some of them while waiting for the rest, so two such calls cannot deadlock each other.  The per-GPU
 // cap (VMIG_PIPES_PER_GPU) grows to what a single call asks for.
-int ctx_acquire_pipes(const std::vector<DeviceInfo>& lane_devs, std::vector<Pipe*>* out)
+int ctx_acquire_pipes(const std::vector<DeviceInfo>& lane_devs, std::vector<Pipe*>* out, const std::atomic<int>* cancel)
 {
     out->assign(lane_devs.size(), nullptr);
     std::vector<int> need_dev; std::vector<uint32_t> need_cnt;
@@ -350,6 +350,7 @@ int ctx_acquire_pipes(const std::vector<DeviceInfo>& lane_devs, std::vector<Pipe
                 if (dp->free_pipes.size() + room < need_cnt[k]) ok = false;
             }
             if (ok) break;
+            if (cancel && cancel->load()) return fail(VMIG_ECANCELED, "cancelled while waiting for a staging pipe");
             g_cv.wait(lk);
         }
         for (size_t k = 0; k < need_dev.size(); k++) {
@@ -402,6 +403,11 @@ int ctx_acquire_pipe(const DeviceInfo& d, Pipe** out)
     int rc = ctx_acquire_pipes(one, &v);
     if (!rc) *out = v[0];
     return rc;
+}
+void ctx_wake_waiters()
+{
+    { std::lock_guard<std::mutex> lk(g_mu); }      // a waiter between its check and its wait would miss the notify
+    g_cv.notify_all();
 }
 void ctx_release_pipe(Pipe* p)
 {
@@ -498,7 +504,7 @@ static void bind_thread(const DeviceInfo& d) {
 
 int run_lane(Pipe* pipe, const std::vector<BlockRef>& blocks, BlockIO* io, bool has_prior, bool hash_only,
              uint32_t n_readers, uint32_t n_writers, uint32_t max_slots, const uint64_t* expect, uint64_t* hashes_out,
-             LaneStats* stats, std::atomic<int>* err, std::string* err_msg, std::mutex* err_mu)
+             LaneStats* stats, std::atomic<int>* err, std::string* err_msg, std::mutex* err_mu, LaneProgress prog)
 {
     if (blocks.empty()) return VMIG_OK;
     const uint32_t slot_bytes = pipe->slot_bytes;
@@ -694,10 +700,11 @@ int run_lane(Pipe* pipe, const std::vector<BlockRef>& blocks, BlockIO* io, bool 
         float ms = 0; CU_TRY(cudaEventElapsedTime(&ms, sl.ev_k0, sl.ev_k1));
         const uint64_t* h_hash = (const uint64_t*)sl.h_res; const uint8_t* h_changed = (const uint8_t*)(h_hash + n);
         b->survive.assign(n, 1);
-        uint64_t skipped = 0, d2h = 0;
+        uint64_t skipped = 0, d2h = 0, hashed = 0;
         for (uint32_t i = 0; i < n; i++) {
             const BlockRef& r = blocks[b->b0 + i];
             hashes_out[r.table_idx] = h_hash[i];
+            hashed += r.len;
             if (fail_block >= 0 && (uint64_t)fail_block == r.table_idx) return fail(VMIG_EFAULT, "injected fault at block %ld (VMIG_FAIL_BLOCK)", fail_block);
             // restore: checked before the prior-table skip below, so a block the destination already has cannot hide
             // corruption; nothing of this batch has been written yet
@@ -724,6 +731,8 @@ int run_lane(Pipe* pipe, const std::vector<BlockRef>& blocks, BlockIO* io, bool 
             }
             CU_TRY(cudaEventRecord(sl.ev_d2h, sl.stream));
         }
+        if (prog.hashed_bytes) prog.hashed_bytes->fetch_add(hashed, std::memory_order_relaxed);
+        if (prog.hashed_blocks) prog.hashed_blocks->fetch_add(n, std::memory_order_relaxed);
         std::lock_guard<std::mutex> lk(stat_mu);
         stats->ms_kernel += ms; stats->blocks_skipped += skipped; stats->bytes_d2h += d2h;
         return VMIG_OK;
@@ -766,6 +775,7 @@ int run_lane(Pipe* pipe, const std::vector<BlockRef>& blocks, BlockIO* io, bool 
             }
             // blocks that need no write are complete now
             const bool writes = !tasks.empty();
+            uint64_t direct_written = 0;
             for (size_t i = 0; i < n; i++) {
                 const bool written_later = writes && b->survive[i];
                 if (!written_later) {
@@ -777,9 +787,10 @@ int run_lane(Pipe* pipe, const std::vector<BlockRef>& blocks, BlockIO* io, bool 
                     }
                     int rc = io->block_done(blocks[b->b0 + i], was_written);
                     if (rc) set_err(rc);
-                    if (was_written) { std::lock_guard<std::mutex> lk(stat_mu); stats->bytes_written += blocks[b->b0 + i].len; }
+                    if (was_written) { std::lock_guard<std::mutex> lk(stat_mu); stats->bytes_written += blocks[b->b0 + i].len; direct_written += blocks[b->b0 + i].len; }
                 }
             }
+            if (direct_written && prog.written) prog.written->fetch_add(direct_written, std::memory_order_relaxed);
             if (tasks.empty()) { finish_batch(b); continue; }
             b->writes_left.store((int)tasks.size());
             for (auto& t : tasks) wsched.push(key_rank[io->write_key(blocks[t.i0])], t);
@@ -811,6 +822,7 @@ int run_lane(Pipe* pipe, const std::vector<BlockRef>& blocks, BlockIO* io, bool 
                 wr_busy += now_ns() - w0;
                 wsched.done(krank);
                 { std::lock_guard<std::mutex> lk(stat_mu); stats->bytes_written += wrote; }
+                if (wrote && prog.written) prog.written->fetch_add(wrote, std::memory_order_relaxed);
                 if (k.batch->writes_left.fetch_sub(1) == 1) finish_batch(k.batch);
             }
         });

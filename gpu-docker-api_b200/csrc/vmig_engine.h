@@ -64,6 +64,24 @@ struct LaneStats {
     double   ms_kernel = 0;
 };
 
+// Cancellation and progress of one call (include/vmig.h, vmig_ctl_*).  Every data-path call has one, a caller's
+// control (vmig_opts.ctl) or a private one, so that vmig_shutdown can cancel whatever is in flight.
+struct CallCtl {
+    std::atomic<int> cancelled{0};
+    std::atomic<uint32_t> phase{VMIG_PHASE_IDLE}, running{0};
+    std::atomic<uint64_t> bytes_total{0}, blocks_total{0}, bytes_hashed{0}, blocks_hashed{0}, bytes_written{0}, bytes_verified{0};
+    std::mutex mu;
+    std::atomic<int>* latch = nullptr;    // first-error latch of the block pipeline in progress (under mu)
+    void cancel();                        // vmig_api.cu
+};
+
+// Where run_lane reports progress (relaxed adds: once per batch in the hash-waiter, once per write task)
+struct LaneProgress {
+    std::atomic<uint64_t>* hashed_bytes = nullptr;
+    std::atomic<uint64_t>* hashed_blocks = nullptr;
+    std::atomic<uint64_t>* written = nullptr;
+};
+
 struct DeviceInfo {
     int dev = -1;
     int sm_count = 0;
@@ -79,8 +97,10 @@ int  ctx_device_count();
 // devices selected by `mask` (0 = all initialised); error if none
 int  ctx_select(uint32_t mask, std::vector<DeviceInfo>* out);
 int  ctx_acquire_pipe(const DeviceInfo& d, Pipe** out);
-// one Pipe per lane, all reserved atomically (a device may repeat: lanes_per_gpu)
-int  ctx_acquire_pipes(const std::vector<DeviceInfo>& lane_devs, std::vector<Pipe*>* out);
+// one Pipe per lane, all reserved atomically (a device may repeat: lanes_per_gpu).  While it waits for pipes other calls
+// hold, a non-zero *cancel makes it return VMIG_ECANCELED with nothing reserved (the canceller calls ctx_wake_waiters).
+int  ctx_acquire_pipes(const std::vector<DeviceInfo>& lane_devs, std::vector<Pipe*>* out, const std::atomic<int>* cancel = nullptr);
+void ctx_wake_waiters();
 void ctx_release_pipe(Pipe* p);
 uint32_t pipe_slot_bytes();
 int  io_threads_default(uint32_t* readers, uint32_t* writers, uint32_t requested, size_t lanes, size_t n_gpus, bool many_files,
@@ -90,9 +110,9 @@ int  io_threads_default(uint32_t* readers, uint32_t* writers, uint32_t requested
 //   hash_only : no D2H of data, no writes (block_done(b,false) is still called).
 //   expect    : nullable; expect[b.table_idx] is the hash block b must have.  A block that hashes otherwise fails
 //               the call with VMIG_ECORRUPT before any block of its batch is written (skipped ones included).
-//   err       : call-wide first-error latch shared by all lanes (0 = fine).
+//   err       : call-wide first-error latch shared by all lanes (0 = fine); a cancel sets it from outside.
 int run_lane(Pipe* pipe, const std::vector<BlockRef>& blocks, BlockIO* io, bool has_prior, bool hash_only,
              uint32_t readers, uint32_t writers, uint32_t max_slots, const uint64_t* expect, uint64_t* hashes_out,
-             LaneStats* stats, std::atomic<int>* err, std::string* err_msg, std::mutex* err_mu);
+             LaneStats* stats, std::atomic<int>* err, std::string* err_msg, std::mutex* err_mu, LaneProgress prog = LaneProgress());
 
 }  // namespace vmig

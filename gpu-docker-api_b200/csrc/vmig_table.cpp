@@ -58,8 +58,9 @@ int table_load(const std::string& path, BlockTable* t)
     return VMIG_OK;
 }
 
-int table_store(const std::string& path, const BlockTable& t)
+int table_store(const std::string& path, const BlockTable& t, const std::atomic<int>* cancel)
 {
+    if (cancel && cancel->load()) return fail(VMIG_ECANCELED, "cancelled before the block table %s was written", path.c_str());
     std::string raw;
     size_t need = 32 + 8 * t.hashes.size();
     for (auto& f : t.files) need += 4 + f.rel.size() + 32;
@@ -87,6 +88,7 @@ int table_store(const std::string& path, const BlockTable& t)
     }
     if (fsync(fd) != 0) { close(fd); unlink(tmp.c_str()); return fail(VMIG_EIO, "fsync %s: %s", tmp.c_str(), errno_str(errno).c_str()); }
     close(fd);
+    if (cancel && cancel->load()) { unlink(tmp.c_str()); return fail(VMIG_ECANCELED, "cancelled before the block table %s was renamed into place", path.c_str()); }
     if (rename(tmp.c_str(), path.c_str()) != 0) { unlink(tmp.c_str()); return fail(VMIG_EIO, "rename %s: %s", path.c_str(), errno_str(errno).c_str()); }
     return VMIG_OK;
 }

@@ -5,6 +5,7 @@
 // internal/version/merge.go:16 (ContainerMergeMap) records.
 #pragma once
 #include <stdint.h>
+#include <atomic>
 #include <string>
 #include <vector>
 #include <unordered_map>
@@ -28,7 +29,8 @@ struct BlockTable {
 };
 
 int table_load(const std::string& path, BlockTable* out);
-// Atomic: writes path.tmp.<pid>.<tid>, fsyncs, renames over path.
-int table_store(const std::string& path, const BlockTable& t);
+// Atomic: writes path.tmp.<pid>.<tid>, fsyncs, renames over path.  A non-zero *cancel (nullable) before the rename
+// removes the .tmp and returns VMIG_ECANCELED: no table at all.
+int table_store(const std::string& path, const BlockTable& t, const std::atomic<int>* cancel = nullptr);
 
 }  // namespace vmig

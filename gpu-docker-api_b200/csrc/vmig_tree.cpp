@@ -78,8 +78,10 @@ int open_beneath_walk(int root_fd, const std::string& rel, int flags, int* out_f
 // dfd: open descriptor of the directory `rel`; consumed (closed) by this call.
 // defer_subdirs != nullptr: do not descend; list the sub-directories (name, rel) for the caller to walk (in parallel).
 static int walk_dir(int dfd, const std::string& rel, uint32_t block_bytes, bool skip_hidden_topdirs,
-                    Manifest* m, int depth, std::vector<std::pair<std::string, std::string>>* defer_subdirs = nullptr)
+                    Manifest* m, int depth, const std::atomic<int>* cancel,
+                    std::vector<std::pair<std::string, std::string>>* defer_subdirs = nullptr)
 {
+    if (cancel && cancel->load()) { close(dfd); return fail(VMIG_ECANCELED, "cancelled during the walk, before %s", rel.c_str()); }
     const int dfd_dup = dup(dfd);
     DIR* d = dfd_dup >= 0 ? fdopendir(dfd) : nullptr;
     if (!d) { const int e = errno; close(dfd); if (dfd_dup >= 0) close(dfd_dup); return fail(VMIG_EIO, "opendir %s: %s", rel.c_str(), errno_str(e).c_str()); }
@@ -147,14 +149,14 @@ static int walk_dir(int dfd, const std::string& rel, uint32_t block_bytes, bool 
                         "open directory %s: %s%s", sd.second.c_str(), errno_str(e).c_str(),
                         e == ELOOP || e == ENOTDIR ? " (it was a directory a moment ago: not following)" : "");
         }
-        int rc = walk_dir(cfd, sd.second, block_bytes, skip_hidden_topdirs, m, depth + 1);
+        int rc = walk_dir(cfd, sd.second, block_bytes, skip_hidden_topdirs, m, depth + 1, cancel);
         if (rc) { close(dfd_dup); return rc; }
     }
     close(dfd_dup);
     return VMIG_OK;
 }
 
-int walk_tree(const std::string& src_root, uint32_t block_bytes, bool skip_hidden_topdirs, Manifest* m)
+int walk_tree(const std::string& src_root, uint32_t block_bytes, bool skip_hidden_topdirs, Manifest* m, const std::atomic<int>* cancel)
 {
     *m = Manifest();
     struct stat st;
@@ -171,7 +173,7 @@ int walk_tree(const std::string& src_root, uint32_t block_bytes, bool skip_hidde
     // (a 40 960-file layer: 71 ms -> ~15 ms; the lstat()s are the cost).  Merged in name order, which is the order
     // the single-threaded descent produced: parents before children, files sorted afterwards anyway.
     std::vector<std::pair<std::string, std::string>> top;
-    int rc = walk_dir(rfd, ".", block_bytes, skip_hidden_topdirs, m, 0, &top);
+    int rc = walk_dir(rfd, ".", block_bytes, skip_hidden_topdirs, m, 0, cancel, &top);
     if (rc) { if (rfd2 >= 0) close(rfd2); return rc; }
     if (!top.empty()) {
         if (rfd2 < 0) return fail(VMIG_EIO, "dup: %s", errno_str(errno).c_str());
@@ -189,7 +191,7 @@ int walk_tree(const std::string& src_root, uint32_t block_bytes, bool skip_hidde
                     r = fail(e == ELOOP || e == ENOTDIR || e == ENOENT ? VMIG_ESRCCHANGED : VMIG_EIO, "open directory %s: %s%s", top[i].second.c_str(),
                              errno_str(e).c_str(), e == ELOOP || e == ENOTDIR ? " (it was a directory a moment ago: not following)" : "");
                 } else {
-                    r = walk_dir(cfd, top[i].second, block_bytes, skip_hidden_topdirs, &sub[i], 1);
+                    r = walk_dir(cfd, top[i].second, block_bytes, skip_hidden_topdirs, &sub[i], 1, cancel);
                 }
                 if (r) { std::lock_guard<std::mutex> lk(bad_mu); if (!bad.load()) { bad_msg = last_error_cstr(); bad.store(r); } return; }
             }
@@ -268,18 +270,28 @@ int unlink_if_exists(const std::string& path, bool* was_dir)
     return VMIG_OK;
 }
 
-int copy_range(int in_fd, int out_fd, uint64_t off, uint64_t len, bool out_direct, bool rw_only, const std::string& what)
+int copy_range(int in_fd, int out_fd, uint64_t off, uint64_t len, bool out_direct, bool rw_only, const std::string& what,
+               const std::atomic<int>* cancel)
 {
+    auto cancelled = [&](uint64_t at) {
+        return fail(VMIG_ECANCELED, "cancelled while copying %s from the base, at byte %llu of %llu", what.c_str(),
+                    (unsigned long long)at, (unsigned long long)(off + len));
+    };
     uint64_t done = 0;
     if (!out_direct && !rw_only) {
-        while (done < len) {
-            loff_t a = (loff_t)(off + done), b = a;
-            const ssize_t n = copy_file_range(in_fd, &a, out_fd, &b, (size_t)(len - done), 0);
-            if (n > 0) { done += (uint64_t)n; continue; }
-            if (n == 0) return fail(VMIG_ESRCCHANGED, "%s ends at %llu, before %llu", what.c_str(), (unsigned long long)(off + done), (unsigned long long)(off + len));
-            if (errno == EINTR) continue;
-            if (errno == ENOSYS || errno == EXDEV || errno == EINVAL || errno == EOPNOTSUPP) break;     // the rest by pread/pwrite
-            return fail(VMIG_EIO, "copy_file_range %s: %s", what.c_str(), errno_str(errno).c_str());
+        bool fallback = false;
+        while (done < len && !fallback) {
+            if (cancel && cancel->load()) return cancelled(off + done);
+            const uint64_t end = std::min<uint64_t>(len, done + kCopyChunk);
+            while (done < end) {
+                loff_t a = (loff_t)(off + done), b = a;
+                const ssize_t n = copy_file_range(in_fd, &a, out_fd, &b, (size_t)(end - done), 0);
+                if (n > 0) { done += (uint64_t)n; continue; }
+                if (n == 0) return fail(VMIG_ESRCCHANGED, "%s ends at %llu, before %llu", what.c_str(), (unsigned long long)(off + done), (unsigned long long)(off + len));
+                if (errno == EINTR) continue;
+                if (errno == ENOSYS || errno == EXDEV || errno == EINVAL || errno == EOPNOTSUPP) { fallback = true; break; }     // the rest by pread/pwrite
+                return fail(VMIG_EIO, "copy_file_range %s: %s", what.c_str(), errno_str(errno).c_str());
+            }
         }
     }
     const size_t kSector = 4096, kChunk = 1u << 20;
@@ -287,7 +299,12 @@ int copy_range(int in_fd, int out_fd, uint64_t off, uint64_t len, bool out_direc
     if (done < len && posix_memalign(&mem, kSector, kChunk) != 0) return fail(VMIG_ENOMEM, "copy buffer for %s", what.c_str());
     uint8_t* buf = (uint8_t*)mem;
     int rc = VMIG_OK;
+    uint64_t since_check = kCopyChunk;
     while (done < len && !rc) {
+        if (since_check >= kCopyChunk) {
+            since_check = 0;
+            if (cancel && cancel->load()) { rc = cancelled(off + done); break; }
+        }
         const size_t want = (size_t)std::min<uint64_t>(kChunk, len - done);
         size_t got = 0;
         while (got < want && !rc) {
@@ -307,7 +324,7 @@ int copy_range(int in_fd, int out_fd, uint64_t off, uint64_t len, bool out_direc
             else if (w == 0) rc = fail(VMIG_EIO, "pwrite (copy of %s): wrote 0 bytes", what.c_str());
             else put += (size_t)w;
         }
-        done += want;
+        done += want; since_check += want;
     }
     free(mem);
     return rc;
@@ -359,10 +376,16 @@ int apply_file_meta(int fd, const std::string& path, const Entry& e, const MetaP
 }
 
 int replay_metadata(const std::string& dst_root, const Manifest& m, const MetaPolicy& pol,
-                    uint64_t* n_symlinks, uint64_t* n_hardlinks, uint64_t* n_specials)
+                    uint64_t* n_symlinks, uint64_t* n_hardlinks, uint64_t* n_specials, const std::atomic<int>* cancel)
 {
+    size_t steps = 0;
+    auto stop = [&](const std::string& rel) {
+        if (!cancel || steps++ % kMetaCheckEvery || !cancel->load()) return VMIG_OK;
+        return fail(VMIG_ECANCELED, "cancelled during metadata replay, before %s", rel.c_str());
+    };
     struct timespec ts[2];
     for (const auto& e : m.symlinks) {
+        if (int rc = stop(e.rel)) return rc;
         const std::string p = join(dst_root, e.rel);
         bool was_dir = false;
         int rc = unlink_if_exists(p, &was_dir);
@@ -377,6 +400,7 @@ int replay_metadata(const std::string& dst_root, const Manifest& m, const MetaPo
         if (n_symlinks) (*n_symlinks)++;
     }
     for (const auto& e : m.specials) {
+        if (int rc = stop(e.rel)) return rc;
         const std::string p = join(dst_root, e.rel);
         bool was_dir = false;
         int rc = unlink_if_exists(p, &was_dir);
@@ -389,6 +413,7 @@ int replay_metadata(const std::string& dst_root, const Manifest& m, const MetaPo
     }
     for (const auto& e : m.files) {
         if (e.hardlink_of < 0) continue;
+        if (int rc = stop(e.rel)) return rc;
         const std::string p = join(dst_root, e.rel);
         const std::string prim = join(dst_root, m.files[(size_t)e.hardlink_of].rel);
         bool was_dir = false;
@@ -401,6 +426,7 @@ int replay_metadata(const std::string& dst_root, const Manifest& m, const MetaPo
     if (!pol.no_metadata) {
         for (size_t i = m.dirs.size(); i-- > 0;) {     // children before parents
             const Entry& e = m.dirs[i];
+            if (int rc = stop(e.rel)) return rc;
             const std::string p = join(dst_root, e.rel);
             if (pol.is_root && chown(p.c_str(), e.uid, e.gid) != 0) return fail(VMIG_EIO, "chown %s: %s", p.c_str(), errno_str(errno).c_str());
             if (chmod(p.c_str(), eff_mode(e, pol)) != 0) return fail(VMIG_EIO, "chmod %s: %s", p.c_str(), errno_str(errno).c_str());
@@ -455,7 +481,13 @@ int remove_source(const std::string& src_root, const Manifest& m)
 // ---------------------------------------------------------------------------------------------
 // VMIG_F_PRUNE: make the destination hold nothing the source does not (the final pass of a hand-off: a file the
 // tenant deleted or renamed between the live pass and the paused pass must not reappear in the new container).
-static int rm_tree_at(int dfd, const char* name, uint64_t* n)
+static int prune_cancelled(const std::atomic<int>* cancel, const char* name)
+{
+    if (!cancel || !cancel->load()) return VMIG_OK;
+    return fail(VMIG_ECANCELED, "cancelled during prune, before %s", name);
+}
+
+static int rm_tree_at(int dfd, const char* name, uint64_t* n, const std::atomic<int>* cancel)
 {
     int fd = openat(dfd, name, O_RDONLY | O_DIRECTORY | O_NOFOLLOW | O_CLOEXEC);
     if (fd < 0) return fail(VMIG_EIO, "prune: open %s: %s", name, errno_str(errno).c_str());
@@ -464,9 +496,10 @@ static int rm_tree_at(int dfd, const char* name, uint64_t* n)
     int rc = VMIG_OK;
     while (struct dirent* de = readdir(d)) {
         if (!strcmp(de->d_name, ".") || !strcmp(de->d_name, "..")) continue;
+        if ((rc = prune_cancelled(cancel, de->d_name))) break;
         struct stat st;
         if (fstatat(fd, de->d_name, &st, AT_SYMLINK_NOFOLLOW) != 0) continue;
-        if (S_ISDIR(st.st_mode)) { rc = rm_tree_at(fd, de->d_name, n); if (rc) break; }
+        if (S_ISDIR(st.st_mode)) { rc = rm_tree_at(fd, de->d_name, n, cancel); if (rc) break; }
         else if (unlinkat(fd, de->d_name, 0) != 0 && errno != ENOENT) { rc = fail(VMIG_EIO, "prune: unlink %s: %s", de->d_name, errno_str(errno).c_str()); break; }
         else (*n)++;
     }
@@ -478,7 +511,7 @@ static int rm_tree_at(int dfd, const char* name, uint64_t* n)
 }
 
 static int prune_dir(int dfd, const std::string& prefix, const std::unordered_set<std::string>& keep_dirs,
-                     const std::unordered_set<std::string>& keep_other, bool dry, uint64_t* n)
+                     const std::unordered_set<std::string>& keep_other, bool dry, uint64_t* n, const std::atomic<int>* cancel)
 {
     DIR* d = fdopendir(dfd);                       // takes ownership of dfd
     if (!d) { close(dfd); return fail(VMIG_EIO, "prune: fdopendir: %s", errno_str(errno).c_str()); }
@@ -487,18 +520,19 @@ static int prune_dir(int dfd, const std::string& prefix, const std::unordered_se
     while (struct dirent* de = readdir(d)) if (strcmp(de->d_name, ".") && strcmp(de->d_name, "..")) names.push_back(de->d_name);
     for (const auto& name : names) {
         const std::string rel = prefix.empty() ? name : prefix + "/" + name;
+        if ((rc = prune_cancelled(cancel, rel.c_str()))) break;
         struct stat st;
         if (fstatat(dfd, name.c_str(), &st, AT_SYMLINK_NOFOLLOW) != 0) continue;
         if (S_ISDIR(st.st_mode) && keep_dirs.count(rel)) {
             int sub = openat(dfd, name.c_str(), O_RDONLY | O_DIRECTORY | O_NOFOLLOW | O_CLOEXEC);
             if (sub < 0) { rc = fail(VMIG_EIO, "prune: open %s: %s", rel.c_str(), errno_str(errno).c_str()); break; }
-            rc = prune_dir(sub, rel, keep_dirs, keep_other, dry, n);
+            rc = prune_dir(sub, rel, keep_dirs, keep_other, dry, n, cancel);
             if (rc) break;
             continue;
         }
         if (!S_ISDIR(st.st_mode) && keep_other.count(rel)) continue;
         if (dry) { (*n)++; continue; }
-        if (S_ISDIR(st.st_mode)) { rc = rm_tree_at(dfd, name.c_str(), n); if (rc) break; }
+        if (S_ISDIR(st.st_mode)) { rc = rm_tree_at(dfd, name.c_str(), n, cancel); if (rc) break; }
         else if (unlinkat(dfd, name.c_str(), 0) != 0 && errno != ENOENT) { rc = fail(VMIG_EIO, "prune: unlink %s: %s", rel.c_str(), errno_str(errno).c_str()); break; }
         else (*n)++;
     }
@@ -506,7 +540,7 @@ static int prune_dir(int dfd, const std::string& prefix, const std::unordered_se
     return rc;
 }
 
-int prune_extras(const std::string& dst_root, const Manifest& m, bool dry_run, uint64_t* n_extras)
+int prune_extras(const std::string& dst_root, const Manifest& m, bool dry_run, uint64_t* n_extras, const std::atomic<int>* cancel)
 {
     std::unordered_set<std::string> keep_dirs, keep_other;
     keep_dirs.reserve(m.dirs.size() * 2); keep_other.reserve((m.files.size() + m.symlinks.size() + m.specials.size()) * 2);
@@ -517,7 +551,7 @@ int prune_extras(const std::string& dst_root, const Manifest& m, bool dry_run, u
     *n_extras = 0;
     int fd = open(dst_root.c_str(), O_RDONLY | O_DIRECTORY | O_CLOEXEC);
     if (fd < 0) return fail(VMIG_EIO, "prune: open %s: %s", dst_root.c_str(), errno_str(errno).c_str());
-    return prune_dir(fd, "", keep_dirs, keep_other, dry_run, n_extras);
+    return prune_dir(fd, "", keep_dirs, keep_other, dry_run, n_extras, cancel);
 }
 
 }  // namespace vmig

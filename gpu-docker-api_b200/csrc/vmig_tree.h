@@ -8,6 +8,7 @@
 // replaced, extras are kept.
 #pragma once
 #include <stdint.h>
+#include <atomic>
 #include <string>
 #include <vector>
 #include <sys/stat.h>
@@ -49,8 +50,11 @@ struct Manifest {
 int open_beneath(int root_fd, const std::string& rel, int flags, int* out_fd);
 int open_beneath_walk(int root_fd, const std::string& rel, int flags, int* out_fd);   // the fallback, exposed for tests/tree_unit.cpp
 
+// The `cancel` arguments below: nullable; once *cancel is non-zero the function starts no new step (directory, metadata
+// entry, prune entry, copy chunk) and returns VMIG_ECANCELED.
 // Walk src_root.  skip_hidden_topdirs reproduces `mv /root/src/*` (reference utils/copy.go:116).
-int walk_tree(const std::string& src_root, uint32_t block_bytes, bool skip_hidden_topdirs, Manifest* out);
+int walk_tree(const std::string& src_root, uint32_t block_bytes, bool skip_hidden_topdirs, Manifest* out,
+              const std::atomic<int>* cancel = nullptr);
 
 struct MetaPolicy {
     bool is_root;        // euid == 0: chown + exact modes (tar -p --same-owner defaults for root)
@@ -63,9 +67,11 @@ MetaPolicy default_meta_policy(uint32_t flags);
 
 // Create every directory of the manifest under dst_root (parents first, traversable by us).
 int make_dirs(const std::string& dst_root, const Manifest& m);
-// Symlinks, specials, hard links and empty regular files; then directory metadata bottom-up.
+// Symlinks, specials, hard links and empty regular files; then directory metadata bottom-up.  Checks cancel every
+// kMetaCheckEvery entries.
+static constexpr size_t kMetaCheckEvery = 1024;
 int replay_metadata(const std::string& dst_root, const Manifest& m, const MetaPolicy& pol,
-                    uint64_t* n_symlinks, uint64_t* n_hardlinks, uint64_t* n_specials);
+                    uint64_t* n_symlinks, uint64_t* n_hardlinks, uint64_t* n_specials, const std::atomic<int>* cancel = nullptr);
 // True if the open file already carries the owner/mode/mtime apply_file_meta would give it (then it is left alone: a
 // diff pass that skips every block of a file must not move its ctime, the block table identifies files by it).
 bool file_meta_matches(int fd, const Entry& e, const MetaPolicy& pol);
@@ -75,7 +81,8 @@ int apply_file_meta(int fd, const std::string& path, const Entry& e, const MetaP
 int remove_source(const std::string& src_root, const Manifest& m);
 // VMIG_F_PRUNE: remove every destination entry the manifest does not list (directories recursively); entries are
 // handled by descriptor, symlinks are never followed.  dry_run only counts them (the verify pass uses that).
-int prune_extras(const std::string& dst_root, const Manifest& m, bool dry_run, uint64_t* n_extras);
+int prune_extras(const std::string& dst_root, const Manifest& m, bool dry_run, uint64_t* n_extras,
+                 const std::atomic<int>* cancel = nullptr);
 // Remove whatever non-directory sits at path (tar replaces existing entries).  ENOENT is fine.
 int unlink_if_exists(const std::string& path, bool* was_dir);
 // Copy bytes [off, off + len) of in_fd to the same offsets of out_fd (a snapshot file's unchanged blocks, taken from
@@ -83,6 +90,9 @@ int unlink_if_exists(const std::string& path, bool* was_dir);
 // the kernel or filesystem refuses it (ENOSYS, EXDEV, EINVAL, EOPNOTSUPP) or rw_only is set.  out_direct: out_fd was
 // opened O_DIRECT, off must be a multiple of 4096, and the bytes go out in whole sectors through an aligned buffer,
 // zero-padded past off + len (the caller truncates the file to its size).  in_fd ending early is VMIG_ESRCCHANGED.
-int copy_range(int in_fd, int out_fd, uint64_t off, uint64_t len, bool out_direct, bool rw_only, const std::string& what);
+// The range is copied in chunks of kCopyChunk bytes; cancel is checked before each one.
+static constexpr uint64_t kCopyChunk = 64ull << 20;
+int copy_range(int in_fd, int out_fd, uint64_t off, uint64_t len, bool out_direct, bool rw_only, const std::string& what,
+               const std::atomic<int>* cancel = nullptr);
 
 }  // namespace vmig

@@ -19,8 +19,10 @@ import os
 from pathlib import Path
 from typing import Callable, Optional
 
-from . import (F_PRUNE, F_VERIFY, GetContainerMergedLayer, GetVolumeMountPoint, VmigError, manifest, migrate_tree,
-               restore_tree, snapshot_tree)
+import threading
+
+from . import (F_PRUNE, F_VERIFY, VMIG_ECANCELED, Ctl, GetContainerMergedLayer, GetVolumeMountPoint, VmigError, manifest,
+               migrate_tree, restore_tree, snapshot_tree)
 
 log = logging.getLogger("vmig.handoff")
 _root: dict = {"cwd": None}
@@ -42,15 +44,17 @@ def snapshotPaths(ctrVersionName: str):
     return d / "diff", d / "blocks.vmig"
 
 
-def CopyDirDiff(src, dest, priorTable: Optional[os.PathLike], outTable: Optional[os.PathLike], flags: int = 0) -> dict:
-    """utils.CopyDirDiff of the cgo shim: CopyDir with the block tables of the diff-skip path."""
-    return migrate_tree(src, dest, priorTable or None, outTable or None, flags=flags)
+def CopyDirDiff(src, dest, priorTable: Optional[os.PathLike], outTable: Optional[os.PathLike], flags: int = 0,
+                ctl: Optional[Ctl] = None) -> dict:
+    """utils.CopyDirDiff of the cgo shim: CopyDir with the block tables of the diff-skip path.  ctl: the mirror of the
+    shim's ...Context variants (a cancelled control raises VmigError(VMIG_ECANCELED))."""
+    return migrate_tree(src, dest, priorTable or None, outTable or None, flags=flags, ctl=ctl)
 
 
-def CopyDirDiffVerified(src, dest, priorTable, outTable) -> dict:
+def CopyDirDiffVerified(src, dest, priorTable, outTable, ctl: Optional[Ctl] = None) -> dict:
     """The pass after which the old container is deleted: the destination is re-read through the GPU and must hash
     like the source (VMIG_F_VERIFY), and holds nothing the source does not (VMIG_F_PRUNE)."""
-    return CopyDirDiff(src, dest, priorTable, outTable, F_VERIFY | F_PRUNE)
+    return CopyDirDiff(src, dest, priorTable, outTable, F_VERIFY | F_PRUNE, ctl)
 
 
 def SnapshotDirVerified(src, dest, outTable) -> dict:
@@ -123,11 +127,16 @@ def RollbackFromSnapshot(targetCtrVersionName: str, newContainer: str, seedTable
     return RestoreDirDiffVerified(data, table, upper, seedTable, newTable)
 
 
-def HandoffCopy(oldContainer: str, newContainer: str, pause: Callable[[str], None], resume: Callable[[str], None]) -> dict:
+def HandoffCopy(oldContainer: str, newContainer: str, pause: Callable[[str], None], resume: Callable[[str], None],
+                pauseBudget: float = 0.0, ctl: Optional[Ctl] = None) -> dict:
     """N2: replaces utils.CopyOldMergedToNewContainerMerged in PatchContainer (replicaset.go:333).  The old container
     keeps running during pass 1 (the bulk of the bytes), is paused for pass 2, which re-reads the source and moves
     only the blocks whose hash changed in between, prunes what the tenant deleted meanwhile, verifies, and leaves the
-    old container paused for the caller to delete.  Any engine error resumes the old container and is raised."""
+    old container paused for the caller to delete.  Any engine error resumes the old container and is raised.
+    pauseBudget (seconds, 0 = no limit) bounds how long the old container stays paused: pass 2 is cancelled when it
+    runs out, the old container is resumed, and a VmigError(VMIG_ECANCELED) with pause_budget_exceeded = True is
+    raised; the new layer then has no table.  ctl (the Go version's ctx) cancels pass 1: the hand-off is aborted, the
+    paused-pass fallback is only for a live source that changed under the reader."""
     src = GetContainerMergedLayer(oldContainer)
     dst = GetContainerMergedLayer(newContainer)
     _, table = snapshotPaths(newContainer)
@@ -136,17 +145,37 @@ def HandoffCopy(oldContainer: str, newContainer: str, pause: Callable[[str], Non
     out = {"pass1": None, "pass1_error": None}
     try:
         try:
-            out["pass1"] = CopyDirDiff(src, dst, None, pass1)
+            out["pass1"] = CopyDirDiff(src, dst, None, pass1, ctl=ctl)
         except VmigError as e:      # live source: a file that shrinks under the reader, a directory swapped for a symlink
+            if e.code == VMIG_ECANCELED:
+                raise
             log.warning("vmig: live pass of %s failed (%s); falling back to one paused pass", oldContainer, e)
             out["pass1_error"] = e.code
             pass1 = None
         pause(oldContainer)
-        try:
-            out["pass2"] = CopyDirDiffVerified(src, dst, pass1, table)
-        except VmigError:
-            resume(oldContainer)
-            raise
+        # once the tenant is paused the hand-off ends by finishing or by its budget, whatever happens to the request
+        with Ctl() as budget:
+            expired = threading.Event()
+
+            def expire():
+                expired.set()
+                budget.cancel()
+            timer = threading.Timer(pauseBudget, expire) if pauseBudget > 0 else None
+            if timer is not None:
+                timer.start()
+            try:
+                out["pass2"] = CopyDirDiffVerified(src, dst, pass1, table, ctl=budget)
+            except VmigError as e:
+                resume(oldContainer)
+                if e.code == VMIG_ECANCELED and expired.is_set():
+                    e.pause_budget_exceeded = True
+                    log.warning("vmig: final pass of %s exceeded its pause budget of %.3f s; old container resumed",
+                                oldContainer, pauseBudget)
+                raise
+            finally:
+                if timer is not None:
+                    timer.cancel()
+                    timer.join()
         return out
     finally:
         if pass1 is not None and pass1.exists():

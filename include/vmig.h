@@ -54,13 +54,15 @@ extern "C" {
 #define VMIG_ESRCCHANGED (-9)  /* a source file shrank while it was being read                  */
 #define VMIG_EVERIFY    (-10)  /* VMIG_F_VERIFY: a destination block does not hash like its source */
 #define VMIG_ECORRUPT   (-11)  /* vmig_restore_tree: the source tree is not the one its block table describes */
+#define VMIG_ECANCELED  (-12)  /* the call's control was cancelled (vmig_ctl_cancel, vmig_shutdown) */
 
 /* ---- lifecycle --------------------------------------------------------------------------- */
 /* Idempotent, thread-safe.  gpu_mask bit i selects CUDA device i; 0 = all visible devices.
  * Creates the per-GPU contexts lazily (streams, pinned staging rings, HBM slots).  Hook:
  * reference cmd/gpu-docker-api/main.go:53-97 (Init); optional -- every call inits on demand. */
 int  vmig_init(uint32_t gpu_mask);
-/* Frees every pooled resource.  Hook: reference cmd/gpu-docker-api/main.go:139-154 (Stop). */
+/* Frees every pooled resource.  Hook: reference cmd/gpu-docker-api/main.go:139-154 (Stop).  Calls still in flight are
+ * cancelled first (they return VMIG_ECANCELED) and shutdown waits for them to return before it frees anything. */
 void vmig_shutdown(void);
 int  vmig_device_count(void);                 /* usable sm_90 devices, or VMIG_ENOGPU           */
 const char* vmig_strerror(int code);
@@ -118,7 +120,9 @@ typedef struct vmig_opts {
                                   n_gpus*k lanes exactly as it is over n_gpus*k GPUs (more host
                                   copy parallelism per link; also how the multi-GPU split is
                                   exercised on a 1-GPU box).  Env VMIG_LANES_PER_GPU overrides 0. */
-    uint32_t reserved[2];
+    uint32_t ctl;              /* 0 = no control; else an id from vmig_ctl_open: the call can be cancelled and
+                                  reports its progress through it (see "Cancellation and progress")             */
+    uint32_t reserved;
 } vmig_opts;
 
 typedef struct vmig_stats {
@@ -246,6 +250,58 @@ int vmig_migrate_buffer(const void* src, void* dst, uint64_t nbytes,
                         uint64_t* out_hashes, const vmig_opts* opts, vmig_stats* stats);
 int  vmig_host_alloc(void** p, uint64_t nbytes);   /* pinned host memory                        */
 void vmig_host_free(void* p);
+
+/* ---- cancellation and progress ------------------------------------------------------------------
+ * A control is a numeric id (cgo passes it in vmig_opts.ctl without any pointer rules).  It serves the entry points
+ * that take vmig_opts: vmig_migrate_tree, vmig_restore_tree, vmig_snapshot_tree and vmig_migrate_buffer (a caller that
+ * wants to cancel a copy or a move calls vmig_migrate_tree with the flags vmig_copy_dir / vmig_move_dir use).  One
+ * control serves one call at a time: attaching it to a second concurrent call fails with VMIG_EINVAL.  The engine has
+ * no deadline of its own; a deadline is the caller's timer calling vmig_ctl_cancel.
+ *   - A control cancelled before the call starts: the call returns VMIG_ECANCELED right after argument validation,
+ *     before the GPU check and before the destination, the tables or the base are touched.  A cancel is never undone.
+ *   - After a cancel no new work is issued: no read, H2D copy, kernel launch, D2H copy, write, link, backfill chunk or
+ *     metadata step starts.  Work already issued finishes (at most one read or write task per copy thread -- <= 1 MiB
+ *     or 64 blocks -- plus what is enqueued on the slot streams), then the call returns VMIG_ECANCELED and
+ *     vmig_last_error() names the phase it stopped in.  A cancel latches like any other first error: a real error that
+ *     happened first keeps its own code.  Outside the block pipeline the call checks the control per directory of the
+ *     walk, while it waits for a staging pipe, per <= 64 MiB chunk of a snapshot's backfill, per <= 1024 metadata
+ *     entries, per entry of VMIG_F_PRUNE, in the VMIG_F_VERIFY re-read, and before the table is renamed into place.
+ *   - A cancelled call gives the guarantees of any failed call: no out_table (and no .tmp of it); prior_table,
+ *     snap_table and base_table untouched; the base snapshot's contents, modes and mtimes unchanged (inode ctimes may
+ *     move, as a snapshot's links always move them); the destination possibly partly written, never with a block that
+ *     failed a check; a file patched in place part way no longer matches its table's identity, so the next pass
+ *     copies it in full.  Every lane thread is joined, the slot streams are synchronised, the pipes are back in the
+ *     pool, no descriptor is left open, and the next call succeeds.
+ *   - VMIG_F_MOVE_SRC: a cancel is honoured up to the first unlink of the source (phase VMIG_PHASE_UNLINK).  From then
+ *     on the move runs to completion and returns VMIG_OK: the source is either intact or the move is complete.
+ *   - Progress: the counters never decrease during a call and start from zero each time the control is attached.
+ *     After a successful call bytes_total, blocks_total and bytes_written equal vmig_stats' fields of the same name,
+ *     and bytes_hashed + bytes_verified equals vmig_stats.bytes_h2d.  The phases of a tree call follow the order
+ *     WALK, (PRUNE), DATA, META, (VERIFY), TABLE, (UNLINK), DONE; a call that fails keeps the phase it stopped in. */
+#define VMIG_PHASE_IDLE    0u   /* attached to no call yet                                                  */
+#define VMIG_PHASE_WALK    1u   /* reading the source tree's metadata                                       */
+#define VMIG_PHASE_DATA    2u   /* the block pipeline (read, hash, diff, write; a snapshot's backfill)     */
+#define VMIG_PHASE_VERIFY  3u   /* VMIG_F_VERIFY: re-reading the destination through the GPU                */
+#define VMIG_PHASE_META    4u   /* empty files, symlinks, specials, hard links, directory metadata          */
+#define VMIG_PHASE_PRUNE   5u   /* VMIG_F_PRUNE: removing destination entries the source does not have      */
+#define VMIG_PHASE_TABLE   6u   /* writing out_table                                                        */
+#define VMIG_PHASE_UNLINK  7u   /* VMIG_F_MOVE_SRC: unlinking the source; a cancel is no longer honoured    */
+#define VMIG_PHASE_DONE    8u   /* the call returned VMIG_OK                                                */
+
+typedef struct vmig_progress {
+    uint32_t phase;            /* VMIG_PHASE_*                                                              */
+    uint32_t running;          /* 1 while a call is attached                                               */
+    uint64_t bytes_total, blocks_total;      /* known once the walk is done                                */
+    uint64_t bytes_hashed, blocks_hashed;    /* data pass: blocks whose hash is back from the GPU          */
+    uint64_t bytes_written;                  /* ring writes so far (the count of vmig_stats.bytes_written) */
+    uint64_t bytes_verified;                 /* VMIG_F_VERIFY re-read                                      */
+    uint64_t reserved[4];
+} vmig_progress;
+
+int vmig_ctl_open(uint32_t* id);                        /* a new control id; ids are never reused within a process */
+int vmig_ctl_cancel(uint32_t id);                       /* any thread, any time, idempotent; unknown/closed id: VMIG_EINVAL */
+int vmig_ctl_progress(uint32_t id, vmig_progress* out); /* any thread, while a call runs or afterwards              */
+int vmig_ctl_close(uint32_t id);                        /* VMIG_EINVAL while a call is still attached              */
 
 /* K1 direct: canonical XXH64(seed 0) of n blocks (host_buf + offs[i], lens[i]); the blocks are
  * staged to HBM at 16-byte-aligned offsets and hashed by the xxh64_blocks kernel.  kernel_ms

@@ -16,11 +16,14 @@ package services
 import "C"
 
 import (
+	"context"
+	stderrors "errors"
 	"os"
 	"path/filepath"
 	"runtime"
 	"strconv"
 	"strings"
+	"time"
 	"unsafe"
 
 	"github.com/ngaut/log"
@@ -137,7 +140,12 @@ func RollbackFromSnapshot(targetCtrVersionName, newContainer, seedTable string) 
 // started the new container and deleted the old one.  Any engine error resumes the old container and is
 // returned BEFORE DeleteContainerForUpdate (replicaset.go:350) can run -- the reference ignores the tar pipe's
 // exit status (utils/copy.go:23).  pause/resume are rs.PauseContainer (replicaset.go:641) and its inverse.
-func HandoffCopy(oldContainer, newContainer string, pause, resume func(name string) error) error {
+// pauseBudget (0 = no limit) bounds how long the old container stays paused: when pass 2 has not finished by then
+// it is cancelled, the old container is resumed and ErrPauseBudgetExceeded is returned; the new layer then has no
+// table.  ctx (the request's) cancels pass 1, which aborts the hand-off: the fallback to one paused pass is for a live
+// source that changed under the reader, not for a caller who gave up.  Once the tenant is paused the hand-off ends by
+// finishing or by its budget.
+func HandoffCopy(ctx context.Context, oldContainer, newContainer string, pauseBudget time.Duration, pause, resume func(name string) error) error {
 	src, err := utils.GetContainerMergedLayer(oldContainer)
 	if err != nil {
 		return errors.WithMessagef(err, "utils.GetContainerMergedLayer failed, container: %s", oldContainer)
@@ -154,19 +162,35 @@ func HandoffCopy(oldContainer, newContainer string, pause, resume func(name stri
 	defer os.Remove(pass1)
 	// pass 1, live: a file that shrinks under the reader fails with VMIG_ESRCCHANGED, a directory swapped for a
 	// symlink is never followed (DESIGN.md, source-side path safety); both are retried once, paused.
-	if err := utils.CopyDirDiff(src, dst, "", pass1); err != nil {
+	if err := utils.CopyDirDiffContext(ctx, src, dst, "", pass1); err != nil {
+		if ctx.Err() != nil {
+			return errors.WithMessage(err, "hand-off cancelled during the live pass; old container untouched")
+		}
 		log.Warnf("vmig: live pass of %s failed (%v); falling back to one paused pass", oldContainer, err)
 		pass1 = ""
 	}
 	if err := pause(oldContainer); err != nil {
 		return errors.WithMessage(err, "pause before the final pass failed")
 	}
-	if err := utils.CopyDirDiffVerified(src, dst, pass1, table); err != nil {
+	budget, cancel := context.Background(), context.CancelFunc(func() {})
+	if pauseBudget > 0 {
+		budget, cancel = context.WithTimeout(context.Background(), pauseBudget)
+	}
+	defer cancel()
+	if err := utils.CopyDirDiffVerifiedContext(budget, src, dst, pass1, table); err != nil {
 		_ = resume(oldContainer)
+		if errors.Is(err, context.DeadlineExceeded) {
+			log.Warnf("vmig: final pass of %s exceeded its pause budget of %v; old container resumed", oldContainer, pauseBudget)
+			return errors.WithMessagef(ErrPauseBudgetExceeded, "%v", err)
+		}
 		return errors.WithMessage(err, "final pass failed; old container resumed, nothing deleted")
 	}
 	return nil
 }
+
+// ErrPauseBudgetExceeded: HandoffCopy's final pass did not finish within its pause budget; the old container was
+// resumed and nothing was deleted.  Test with errors.Is.
+var ErrPauseBudgetExceeded = stderrors.New("vmig: final pass exceeded the pause budget")
 
 // N3 -- UsedBytes replaces utils.DirSize in PatchVolumeSize's shrink check (volume.go:126-140): the engine's
 // metadata walk (no GPU work) returns the same sum of regular-file sizes; with a non-empty tablePath it also

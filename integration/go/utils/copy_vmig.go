@@ -10,6 +10,8 @@ package utils
 import "C"
 
 import (
+	"context"
+	"fmt"
 	"runtime"
 	"unsafe"
 
@@ -48,7 +50,13 @@ func CopyDir(src, dest string) error {
 // under the per-version directory setToMergeMap already creates
 // (internal/services/replicaset.go:681-704): merges/<rs>/<rs>-<v>/blocks.vmig.
 func CopyDirDiff(src, dest, priorTable, outTable string) error {
-	return copyDirDiff(src, dest, priorTable, outTable, 0)
+	return CopyDirDiffContext(context.Background(), src, dest, priorTable, outTable)
+}
+
+// CopyDirDiffContext is CopyDirDiff that stops when ctx is done: the engine issues no new work, returns
+// VMIG_ECANCELED, and the error wraps ctx.Err().  As after any failure, outTable is not written.
+func CopyDirDiffContext(ctx context.Context, src, dest, priorTable, outTable string) error {
+	return copyDirDiff(ctx, src, dest, priorTable, outTable, 0)
 }
 
 // CopyDirDiffVerified additionally re-reads the destination through the GPU and compares block tables
@@ -56,13 +64,23 @@ func CopyDirDiff(src, dest, priorTable, outTable string) error {
 // deleted or renamed since an earlier pass must not reappear), before it reports success: for the pass after which
 // the old container is deleted, and for rollbacks onto a seeded layer.
 func CopyDirDiffVerified(src, dest, priorTable, outTable string) error {
-	return copyDirDiff(src, dest, priorTable, outTable, C.VMIG_F_VERIFY|C.VMIG_F_PRUNE)
+	return CopyDirDiffVerifiedContext(context.Background(), src, dest, priorTable, outTable)
+}
+
+// CopyDirDiffVerifiedContext is CopyDirDiffVerified that stops when ctx is done (see CopyDirDiffContext).
+func CopyDirDiffVerifiedContext(ctx context.Context, src, dest, priorTable, outTable string) error {
+	return copyDirDiff(ctx, src, dest, priorTable, outTable, C.VMIG_F_VERIFY|C.VMIG_F_PRUNE)
 }
 
 // SnapshotDirVerified writes a version snapshot: the copy is re-read through the GPU (VMIG_F_VERIFY) before
 // outTable is written, so the table describes what really landed in dest.
 func SnapshotDirVerified(src, dest, outTable string) error {
-	return copyDirDiff(src, dest, "", outTable, C.VMIG_F_VERIFY)
+	return SnapshotDirVerifiedContext(context.Background(), src, dest, outTable)
+}
+
+// SnapshotDirVerifiedContext is SnapshotDirVerified that stops when ctx is done (see CopyDirDiffContext).
+func SnapshotDirVerifiedContext(ctx context.Context, src, dest, outTable string) error {
+	return copyDirDiff(ctx, src, dest, "", outTable, C.VMIG_F_VERIFY)
 }
 
 // RestoreDirDiffVerified is CopyDirDiffVerified from a snapshot that must still be the tree its own block table
@@ -70,9 +88,15 @@ func SnapshotDirVerified(src, dest, outTable string) error {
 // passes.  A snapshot without its table (one that failed part way) or one changed since fails with VMIG_ECORRUPT /
 // VMIG_ETABLE instead of being restored.
 func RestoreDirDiffVerified(snap, snapTable, dest, priorTable, outTable string) error {
+	return RestoreDirDiffVerifiedContext(context.Background(), snap, snapTable, dest, priorTable, outTable)
+}
+
+// RestoreDirDiffVerifiedContext is RestoreDirDiffVerified that stops when ctx is done (see CopyDirDiffContext);
+// the snapshot and its table are untouched either way.
+func RestoreDirDiffVerifiedContext(ctx context.Context, snap, snapTable, dest, priorTable, outTable string) error {
 	ct := C.CString(snapTable)
 	defer C.free(unsafe.Pointer(ct))
-	return runDiff("vmig_restore_tree", snap, dest, priorTable, outTable, C.VMIG_F_VERIFY|C.VMIG_F_PRUNE,
+	return runDiff(ctx, "vmig_restore_tree", snap, dest, priorTable, outTable, C.VMIG_F_VERIFY|C.VMIG_F_PRUNE,
 		func(cs, cd, cp, co *C.char, o *C.vmig_opts, st *C.vmig_stats, _ *C.vmig_snapshot_stats) C.int {
 			return C.vmig_restore_tree(cs, ct, cd, cp, co, o, st)
 		})
@@ -83,23 +107,31 @@ func RestoreDirDiffVerified(snap, snapTable, dest, priorTable, outTable string) 
 // file takes its unchanged blocks from the base file.  The re-read (VMIG_F_VERIFY) covers linked files too, so a base
 // that rotted without moving its ctime is caught when the snapshot is taken.
 func SnapshotDirIncrementalVerified(src, dest, baseDir, baseTable, outTable string) error {
+	return SnapshotDirIncrementalVerifiedContext(context.Background(), src, dest, baseDir, baseTable, outTable)
+}
+
+// SnapshotDirIncrementalVerifiedContext is SnapshotDirIncrementalVerified that stops when ctx is done (see
+// CopyDirDiffContext); the base snapshot's contents, modes and mtimes are unchanged either way.
+func SnapshotDirIncrementalVerifiedContext(ctx context.Context, src, dest, baseDir, baseTable, outTable string) error {
 	cb, ct := C.CString(baseDir), C.CString(baseTable)
 	defer C.free(unsafe.Pointer(cb))
 	defer C.free(unsafe.Pointer(ct))
-	return runDiff("vmig_snapshot_tree", src, dest, "", outTable, C.VMIG_F_VERIFY,
+	return runDiff(ctx, "vmig_snapshot_tree", src, dest, "", outTable, C.VMIG_F_VERIFY,
 		func(cs, cd, _, co *C.char, o *C.vmig_opts, st *C.vmig_stats, ss *C.vmig_snapshot_stats) C.int {
 			return C.vmig_snapshot_tree(cs, cd, cb, ct, co, o, st, ss)
 		})
 }
 
-func copyDirDiff(src, dest, priorTable, outTable string, flags C.uint32_t) error {
-	return runDiff("vmig_migrate_tree", src, dest, priorTable, outTable, flags,
+func copyDirDiff(ctx context.Context, src, dest, priorTable, outTable string, flags C.uint32_t) error {
+	return runDiff(ctx, "vmig_migrate_tree", src, dest, priorTable, outTable, flags,
 		func(cs, cd, cp, co *C.char, o *C.vmig_opts, st *C.vmig_stats, _ *C.vmig_snapshot_stats) C.int {
 			return C.vmig_migrate_tree(cs, cd, cp, co, o, st)
 		})
 }
 
-func runDiff(what, src, dest, priorTable, outTable string, flags C.uint32_t,
+// runDiff makes one engine call under a control of its own: context.AfterFunc cancels it when ctx is done (a
+// deadline is ctx's timer; the engine has none), and VMIG_ECANCELED comes back as an error that wraps ctx.Err().
+func runDiff(ctx context.Context, what, src, dest, priorTable, outTable string, flags C.uint32_t,
 	call func(cs, cd, cp, co *C.char, o *C.vmig_opts, st *C.vmig_stats, ss *C.vmig_snapshot_stats) C.int) error {
 	cs, cd := C.CString(src), C.CString(dest)
 	defer C.free(unsafe.Pointer(cs))
@@ -117,7 +149,19 @@ func runDiff(what, src, dest, priorTable, outTable string, flags C.uint32_t,
 	var ss C.vmig_snapshot_stats // filled by vmig_snapshot_tree only
 	var o C.vmig_opts            // zero value = defaults (all GPUs, 4 MiB blocks)
 	o.flags = flags
-	err := lockedCall(what, func() C.int { return call(cs, cd, cp, co, &o, &st, &ss) })
+	var id C.uint32_t
+	if err := lockedCall("vmig_ctl_open", func() C.int { return C.vmig_ctl_open(&id) }); err != nil {
+		return err
+	}
+	defer C.vmig_ctl_close(id) // runs after stop(): the call has returned, nothing is attached any more
+	stop := context.AfterFunc(ctx, func() { C.vmig_ctl_cancel(id) })
+	defer stop()
+	o.ctl = id
+	var rc C.int
+	err := lockedCall(what, func() C.int { rc = call(cs, cd, cp, co, &o, &st, &ss); return rc })
+	if rc == C.VMIG_ECANCELED && ctx.Err() != nil {
+		return fmt.Errorf("%w: %v", ctx.Err(), err)
+	}
 	if err == nil {
 		log.Infof("vmig: %d bytes, %d/%d blocks skipped, %d files copied in full (stale table), %d pruned, "+
 			"%d files linked to the base snapshot (%d bytes), %d backfilled from it (%d bytes), %d base files stale, %.2f GiB/s",

@@ -8,6 +8,7 @@
 #include "vmig_tree.h"
 #include "vmig_table.h"
 #include "vmig_cufile.h"
+#include "vmig_reuse.h"
 
 #include <fcntl.h>
 #include <unistd.h>
@@ -122,6 +123,7 @@ public:
         std::atomic<void*> s_cfh{nullptr}, d_cfh{nullptr};   // cuFile handles of sfd / dfd (VMIG_F_CUFILE)
         std::atomic<bool> wrote{false};                  // at least one block of the file was written in this call
         const TableFile* base_rec = nullptr;             // vmig_snapshot_tree: the base file still is this record
+        std::atomic<bool> reused{false};                 // vmig_snapshot_tree: a changed block was found elsewhere in the base
         bool solo = true;                                // no other source path is a hard link to this file
     };
     std::string src_root, dst_root;
@@ -144,33 +146,36 @@ public:
     std::unique_ptr<FS[]> fs;
     std::mutex stripes[64];
 
-    // vmig_snapshot_tree: the base snapshot whose files supply the blocks K1 found unchanged
+    // vmig_snapshot_tree: the base snapshot whose files supply the blocks K1 found unchanged, at the same path and offset
+    // or anywhere else in the base (bidx: every block of every trusted base file, by hash and length)
     std::string base_root;
-    std::vector<uint8_t> skipped;                          // per table block: 1 = not written, its bytes are the base file's
+    BaseIndex bidx;
+    const uint64_t* hashes = nullptr;                      // the call's block hashes (a file's are all there when it finalizes)
+    std::vector<uint8_t> skipped;                          // per table block: 1 = not written, its bytes are in the base
     std::mutex link_mu;
     std::unordered_map<uint64_t, int64_t> linked_inos;     // base inode linked by this call -> its ctime after the link
     std::vector<uint32_t> linked_files;
     std::atomic<uint64_t> n_linked{0}, b_linked{0}, n_backfilled{0}, b_backfilled{0};
     const std::atomic<int>* cancel = nullptr;              // the call's cancel flag: checked per backfill chunk
-    bool done_on_writer(const BlockRef& b) override { return fs[b.file].base_rec != nullptr; }
+    static constexpr size_t kLinkTries = 16;               // base files of equal content tried as a link target, per file
+    bool done_on_writer(const BlockRef& b) override { return fs[b.file].base_rec != nullptr || fs[b.file].reused.load(); }
+    bool reusable(const BlockRef& b, uint64_t hash) override {
+        if (bidx.empty() || !bidx.contains(hash, b.len)) return false;
+        skipped[b.table_idx] = 1;
+        fs[b.file].reused.store(true);
+        return true;
+    }
 
-    // Last block of a base candidate passed: link the new path to the base file when nothing was written and the link
-    // keeps the snapshot's hard-link structure and metadata equal to the source's, else copy the skipped blocks from the
-    // base file into the new file (block_done then finalizes it like any other).  Runs on a writer (done_on_writer).
-    int finish_from_base(uint32_t f, bool* linked) {
-        FS& s = fs[f];
-        const Entry& e = m->files[f];
-        const TableFile& bf = *s.base_rec;
-        bool any_skipped = false;
-        for (uint64_t r = 0; r < e.n_blocks && !any_skipped; r++) any_skipped = skipped[e.first_block + r] != 0;
-        if (!any_skipped) return VMIG_OK;
-        const std::string bp = pjoin(base_root, e.rel);
+    // Open base file g and check that it still is the file its record describes: same inode, and the recorded ctime or
+    // the one this call's own link to it left.  Anything else changed it, and the bytes it was to supply are gone.
+    int open_base(uint32_t g, int* out, struct stat* bs) {
+        const TableFile& bf = bidx.t->files[g];
+        const std::string bp = pjoin(base_root, bf.rel);
         const int bfd = open(bp.c_str(), O_RDONLY | O_NOFOLLOW | O_CLOEXEC);
-        struct stat bs;
-        bool same = bfd >= 0 && fstat(bfd, &bs) == 0 && S_ISREG(bs.st_mode) && (uint64_t)bs.st_ino == bf.ino;
+        bool same = bfd >= 0 && fstat(bfd, bs) == 0 && S_ISREG(bs->st_mode) && (uint64_t)bs->st_ino == bf.ino;
         if (same) {
-            const int64_t ct = (int64_t)bs.st_ctim.tv_sec * 1000000000ll + bs.st_ctim.tv_nsec;
-            std::lock_guard<std::mutex> lk(link_mu);
+            const int64_t ct = (int64_t)bs->st_ctim.tv_sec * 1000000000ll + bs->st_ctim.tv_nsec;
+            std::lock_guard<std::mutex> lk(link_mu);     // a link in flight holds it from before linkat until linked_inos has its ctime
             auto it = linked_inos.find(bf.ino);
             same = ct == bf.ctime_ns || (it != linked_inos.end() && it->second == ct);
         }
@@ -178,12 +183,38 @@ public:
             if (bfd >= 0) close(bfd);
             return fail(VMIG_ESRCCHANGED, "base file %s changed during the snapshot: the bytes of its unchanged blocks are gone", bp.c_str());
         }
+        *out = bfd;
+        return VMIG_OK;
+    }
+
+    // Last block of a file with blocks in the base passed: link the new path to a base file of the same content when
+    // nothing was written and the link keeps the snapshot's hard-link structure and metadata equal to the source's
+    // (the same-path file first, then the others in table order), else copy the skipped blocks from the base files that
+    // hold them into the new file (block_done then finalizes it like any other).  Runs on a writer (done_on_writer).
+    int finish_from_base(uint32_t f, bool* linked) {
+        FS& s = fs[f];
+        const Entry& e = m->files[f];
+        bool any_skipped = false;
+        for (uint64_t r = 0; r < e.n_blocks && !any_skipped; r++) any_skipped = skipped[e.first_block + r] != 0;
+        if (!any_skipped) return VMIG_OK;
+        const int same = s.base_rec ? (int)(s.base_rec - bidx.t->files.data()) : -1;
+        const uint64_t* h = hashes + e.first_block;
         const std::string p = pjoin(dst_root, e.rel);
-        if (!s.wrote.load() && e.size == bf.size && s.solo && file_meta_matches(bfd, e, pol)) {
-            std::lock_guard<std::mutex> lk(link_mu);
-            if (!linked_inos.count(bf.ino)) {
+        if (!s.wrote.load() && s.solo) {
+            std::vector<uint32_t> cands;
+            link_candidates(bidx, same, e.size, block_bytes, h, &cands, kLinkTries);
+            for (uint32_t g : cands) {
+                const TableFile& bf = bidx.t->files[g];
+                { std::lock_guard<std::mutex> lk(link_mu); if (linked_inos.count(bf.ino)) continue; }
+                int bfd; struct stat bs;
+                int rc = open_base(g, &bfd, &bs);
+                if (rc) return rc;
+                if (!file_meta_matches(bfd, e, pol)) { close(bfd); continue; }
+                std::lock_guard<std::mutex> lk(link_mu);
+                if (linked_inos.count(bf.ino)) { close(bfd); continue; }
+                const std::string bp = pjoin(base_root, bf.rel);
                 bool was_dir = false;
-                int rc = unlink_if_exists(p, &was_dir);
+                rc = unlink_if_exists(p, &was_dir);
                 if (!rc && was_dir) rc = fail(VMIG_EIO, "%s: a directory is in the way of a regular file", p.c_str());
                 if (!rc && linkat(AT_FDCWD, bp.c_str(), AT_FDCWD, p.c_str(), 0) != 0) rc = fail(VMIG_EIO, "link %s -> %s: %s", p.c_str(), bp.c_str(), errno_str(errno).c_str());
                 struct stat ls;
@@ -200,17 +231,25 @@ public:
                 return VMIG_OK;
             }
         }
-        int dfd; int rc = open_dst(f, &dfd);
+        std::vector<ReuseRun> runs;
+        int rc = plan_backfill(bidx, same, e.size, block_bytes, h, &skipped[e.first_block], e.rel, &runs);
+        if (rc) return rc;
+        int dfd; rc = open_dst(f, &dfd);
+        std::unordered_map<uint32_t, int> bfds;              // base files this file takes bytes from, each checked once
         uint64_t bytes = 0;
-        for (uint64_t r = 0; r < e.n_blocks && !rc;) {
-            if (!skipped[e.first_block + r]) { r++; continue; }
-            uint64_t q = r;
-            while (q < e.n_blocks && skipped[e.first_block + q]) q++;
-            const uint64_t off = r * (uint64_t)block_bytes, len = std::min<uint64_t>(q * (uint64_t)block_bytes, e.size) - off;
-            rc = copy_range(bfd, dfd, off, len, s.d_direct, false, bp, cancel);
-            bytes += len; r = q;
+        for (const ReuseRun& u : runs) {
+            if (rc) break;
+            auto it = bfds.find(u.file);
+            if (it == bfds.end()) {
+                int bfd; struct stat bs;
+                rc = open_base(u.file, &bfd, &bs);
+                if (rc) break;
+                it = bfds.emplace(u.file, bfd).first;
+            }
+            rc = copy_range_at(it->second, u.src_off, dfd, u.dst_off, u.len, s.d_direct, false, pjoin(base_root, bidx.t->files[u.file].rel), cancel);
+            bytes += u.len;
         }
-        close(bfd);
+        for (auto& kv : bfds) close(kv.second);
         if (rc) return rc;
         n_backfilled++; b_backfilled += bytes;
         return VMIG_OK;
@@ -380,11 +419,11 @@ public:
     }
     int block_done(const BlockRef& b, bool written) override {
         FS& s = fs[b.file];
-        if (!written && s.base_rec) skipped[b.table_idx] = 1;
+        if (!written && s.base_rec) skipped[b.table_idx] = 1;          // (a reused block was marked by reusable())
         if (s.blocks_left.fetch_sub(1) != 1) return VMIG_OK;
         if (hash_only) return VMIG_OK;
         const Entry& e = m->files[b.file];
-        if (s.base_rec) {
+        if (s.base_rec || s.reused.load()) {
             bool linked = false;
             int rc = finish_from_base(b.file, &linked);
             if (rc || linked) return rc;
@@ -688,7 +727,23 @@ int migrate_tree_body(CallScope& call, const char* src_dir, const char* dst_dir,
         group.clear();
     };
     bool any_base = false;
-    if (has_base) io.base_root = base_dir;
+    std::vector<uint8_t> base_trusted(base.files.size(), 0);
+    if (has_base) {
+        io.base_root = base_dir;
+        // take blocks from a base file only while it still IS the one the base table was written for (its link count may
+        // exceed 1: base files are shared with older snapshots).  Every record is checked, once: a source file may find
+        // its bytes in any base file, whatever its path.
+        for (size_t i = 0; i < base.files.size(); i++) {
+            const TableFile& bf = base.files[i];
+            if (i % kMetaCheckEvery == 0 && cancel->load()) return fail(VMIG_ECANCELED, "while checking the base's files");
+            struct stat bs;
+            base_trusted[i] = bf.ino != 0 && lstat(pjoin(io.base_root, bf.rel).c_str(), &bs) == 0 && S_ISREG(bs.st_mode) &&
+                              (uint64_t)bs.st_ino == bf.ino && (uint64_t)bs.st_size == bf.size &&
+                              (int64_t)bs.st_ctim.tv_sec * 1000000000ll + bs.st_ctim.tv_nsec == bf.ctime_ns;
+        }
+        io.bidx.build(base, base_trusted);
+        io.hashes = hashes.data();
+    }
     for (auto& e : man.files) if (e.hardlink_of >= 0) io.fs[(size_t)e.hardlink_of].solo = false;
     for (uint32_t f = 0; f < man.files.size(); f++) {
         const Entry& e = man.files[f];
@@ -697,15 +752,8 @@ int migrate_tree_body(CallScope& call, const char* src_dir, const char* dst_dir,
         s.reads_left.store((uint32_t)e.n_blocks); s.blocks_left.store((uint32_t)e.n_blocks);
         if (has_base) {
             auto it = base.index.find(e.rel);
-            struct stat bs;
-            // take blocks from a base file only while it still IS the one the base table was written for (its link
-            // count may exceed 1: base files are shared with older snapshots)
             if (it != base.index.end() && base.files[it->second].ino != 0) {
-                const TableFile& bf = base.files[it->second];
-                const bool ok = lstat(pjoin(io.base_root, e.rel).c_str(), &bs) == 0 && S_ISREG(bs.st_mode) &&
-                                (uint64_t)bs.st_ino == bf.ino && (uint64_t)bs.st_size == bf.size &&
-                                (int64_t)bs.st_ctim.tv_sec * 1000000000ll + bs.st_ctim.tv_nsec == bf.ctime_ns;
-                if (ok) { s.base_rec = &bf; any_base = true; }
+                if (base_trusted[it->second]) { s.base_rec = &base.files[it->second]; any_base = true; }
                 else sst_snap.files_base_untrusted++;
             }
         }
@@ -728,7 +776,10 @@ int migrate_tree_body(CallScope& call, const char* src_dir, const char* dst_dir,
         if (group.size() == 64) flush_group();
     }
     flush_group();
-    if (any_base) io.skipped.assign(man.n_blocks, 0);
+    // skip mode whenever the base can supply a block, also when no source path has a same-path record (a layer whose
+    // files were all moved): without it the submitter streams every block back with its hash (DESIGN.md §3)
+    const bool skip_mode = has_prior || any_base || !io.bidx.empty();
+    if (any_base || !io.bidx.empty()) io.skipped.assign(man.n_blocks, 0);
     st.ns_plan = now_ns() - t0;
 
     // VMIG_F_PRUNE runs first: what it removes is by definition not in the source, a directory sitting where the source
@@ -744,7 +795,7 @@ int migrate_tree_body(CallScope& call, const char* src_dir, const char* dst_dir,
     if (!hash_only) { rc = make_dirs(dst, man); if (rc) return rc; }
 
     t0 = now_ns();
-    rc = run_blocks(blocks, &io, has_prior || any_base, hash_only, o, hashes.data(), &st, ctl, false, expect.empty() ? nullptr : expect.data());
+    rc = run_blocks(blocks, &io, skip_mode, hash_only, o, hashes.data(), &st, ctl, false, expect.empty() ? nullptr : expect.data());
     st.ns_data = now_ns() - t0;
     if (rc) { std::string keep = last_error_cstr(); io.close_all(man.files.size()); set_last_error_str(keep); return rc; }
 

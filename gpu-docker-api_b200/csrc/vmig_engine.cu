@@ -711,7 +711,7 @@ int run_lane(Pipe* pipe, const std::vector<BlockRef>& blocks, BlockIO* io, bool 
             if (expect && expect[r.table_idx] != h_hash[i])
                 return fail(VMIG_ECORRUPT, "%s hashes %016llx, its block table says %016llx", io->block_name(r).c_str(),
                             (unsigned long long)h_hash[i], (unsigned long long)expect[r.table_idx]);
-            if (has_prior && !h_changed[i]) { b->survive[i] = 0; skipped++; }
+            if (has_prior && (!h_changed[i] || (!hash_only && io->reusable(r, h_hash[i])))) { b->survive[i] = 0; skipped++; }
         }
         if (dev_dst) {
             for (uint32_t i = 0; i < n; i++) if (b->survive[i]) d2h += blocks[b->b0 + i].len;      // drained by the writers straight from HBM

@@ -40,6 +40,10 @@ public:
     // true: block_done of this block, if skipped, may do file-sized work (vmig_snapshot_tree links or backfills the file
     // when its last block passes); it then runs on a writer thread under the block's write key, not on the d2h-waiter
     virtual bool done_on_writer(const BlockRef&) { return false; }
+    // skip mode (has_prior): asked in the hash-waiter, before any D2H, for each block K1 found changed against its prior
+    // hash.  true: the backend has these bytes elsewhere (vmig_snapshot_tree: a base block with the same hash and
+    // length); the block is then skipped like an unchanged one -- no D2H, no write, block_done(b, false)
+    virtual bool reusable(const BlockRef&, uint64_t /*hash*/) { return false; }
     // writes with the same key are issued by one writer thread, in order (a file takes writes from one
     // thread at a time anyway); backends without such a constraint spread the keys
     virtual uint32_t write_key(const BlockRef& b) { return b.file; }

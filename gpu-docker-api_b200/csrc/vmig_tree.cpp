@@ -273,6 +273,12 @@ int unlink_if_exists(const std::string& path, bool* was_dir)
 int copy_range(int in_fd, int out_fd, uint64_t off, uint64_t len, bool out_direct, bool rw_only, const std::string& what,
                const std::atomic<int>* cancel)
 {
+    return copy_range_at(in_fd, off, out_fd, off, len, out_direct, rw_only, what, cancel);
+}
+
+int copy_range_at(int in_fd, uint64_t off, int out_fd, uint64_t out_off, uint64_t len, bool out_direct, bool rw_only,
+                  const std::string& what, const std::atomic<int>* cancel)
+{
     auto cancelled = [&](uint64_t at) {
         return fail(VMIG_ECANCELED, "cancelled while copying %s from the base, at byte %llu of %llu", what.c_str(),
                     (unsigned long long)at, (unsigned long long)(off + len));
@@ -284,7 +290,7 @@ int copy_range(int in_fd, int out_fd, uint64_t off, uint64_t len, bool out_direc
             if (cancel && cancel->load()) return cancelled(off + done);
             const uint64_t end = std::min<uint64_t>(len, done + kCopyChunk);
             while (done < end) {
-                loff_t a = (loff_t)(off + done), b = a;
+                loff_t a = (loff_t)(off + done), b = (loff_t)(out_off + done);
                 const ssize_t n = copy_file_range(in_fd, &a, out_fd, &b, (size_t)(end - done), 0);
                 if (n > 0) { done += (uint64_t)n; continue; }
                 if (n == 0) return fail(VMIG_ESRCCHANGED, "%s ends at %llu, before %llu", what.c_str(), (unsigned long long)(off + done), (unsigned long long)(off + len));
@@ -318,7 +324,7 @@ int copy_range(int in_fd, int out_fd, uint64_t off, uint64_t len, bool out_direc
         if (!rc) memset(buf + want, 0, out_len - want);
         size_t put = 0;
         while (put < out_len && !rc) {
-            const ssize_t w = pwrite(out_fd, buf + put, out_len - put, (off_t)(off + done + put));
+            const ssize_t w = pwrite(out_fd, buf + put, out_len - put, (off_t)(out_off + done + put));
             if (w < 0 && errno == EINTR) continue;
             if (w < 0) rc = fail(VMIG_EIO, "pwrite (copy of %s): %s", what.c_str(), errno_str(errno).c_str());
             else if (w == 0) rc = fail(VMIG_EIO, "pwrite (copy of %s): wrote 0 bytes", what.c_str());

@@ -94,5 +94,9 @@ int unlink_if_exists(const std::string& path, bool* was_dir);
 static constexpr uint64_t kCopyChunk = 64ull << 20;
 int copy_range(int in_fd, int out_fd, uint64_t off, uint64_t len, bool out_direct, bool rw_only, const std::string& what,
                const std::atomic<int>* cancel = nullptr);
+// The same copy from [in_off, in_off + len) of in_fd to [out_off, out_off + len) of out_fd (a block that sits at another
+// offset, or in another file, of the base snapshot).  out_direct: out_off must be a multiple of 4096.
+int copy_range_at(int in_fd, uint64_t in_off, int out_fd, uint64_t out_off, uint64_t len, bool out_direct, bool rw_only,
+                  const std::string& what, const std::atomic<int>* cancel = nullptr);
 
 }  // namespace vmig

@@ -100,7 +100,8 @@ def baseVersion(ctrVersionName: str) -> Optional[str]:
 
 def SnapshotVersionIncremental(ctrVersionName: str) -> dict:
     """N1, as setToMergeMap calls it: SnapshotVersion that shares unchanged files and blocks with the newest earlier
-    snapshot of the ReplicaSet (a full SnapshotDirVerified when there is none).  That version's blocks.vmig may have
+    snapshot of the ReplicaSet, wherever that snapshot holds them (a file renamed or moved since is still shared), and
+    a full SnapshotDirVerified when there is none.  That version's blocks.vmig may have
     been written last by HandoffCopy for the container's layer, not for diff/ (a snapshot of it that failed part
     way): the identities it records then name no file under diff/, the engine trusts none of them, and the result is
     a plain verified copy."""

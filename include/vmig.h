@@ -205,20 +205,31 @@ typedef struct vmig_snapshot_stats {
  *     inside it, or contains it (compared by real path).  VMIG_F_VERIFY, VMIG_F_PRUNE, VMIG_F_DIRECT_IO,
  *     lanes_per_gpu and gpu_mask act as in a migration.
  *   - base_table loads like a prior table (formats 01 and 02); its block_bytes must equal the call's (VMIG_ETABLE).
- * A source regular file is a base candidate when dst_dir and base_dir are on one device, the base table records the
- * path with an inode, and the base file is still that regular file with that inode, ctime and size (its link count
- * may exceed 1: base files are shared with older snapshots).  A candidate's blocks are compared on the GPU with the
- * base table's hashes, exactly as the in-place diff path compares with a prior table; unchanged blocks are neither
- * copied back from HBM nor written.  When the file's last block has passed:
- *   - link: the new path becomes a hard link to the base file if no block was written, the sizes are equal, the
- *     source file has no hard-link partner in src_dir, no other path of this call was linked to that base inode, and
- *     the base inode already carries the owner, mode and mtime the copy would get.  A linked inode's metadata is
- *     never changed (that would change older snapshots too);
- *   - backfill: otherwise the file is written new: changed blocks from the ring, unchanged ones copied from the base
- *     file at the same offsets (copy_file_range, or pread/pwrite where that is refused), then its metadata applied.
- * Before it links or copies from a base file the call re-checks its inode and ctime; a base file that changed during
- * the call fails it with VMIG_ESRCCHANGED naming the path (a retry copies that file in full).  Files that are not
- * candidates are copied as by vmig_migrate_tree; where the base table named the path, files_base_untrusted counts it.
+ * A base file is trusted when dst_dir and base_dir are on one device, the base table records it with an inode, and it
+ * is still that regular file with that inode, ctime and size (its link count may exceed 1: base files are shared with
+ * older snapshots).  Unchanged content is found in the trusted base files by block, wherever it sits there:
+ *   - a source file whose path a trusted base file has is compared on the GPU with that file's hashes, block by block,
+ *     exactly as the in-place diff path compares with a prior table;
+ *   - every other block -- a changed one, or one of a file the base holds under another path -- is looked up by its
+ *     (XXH64, length) among all blocks of all trusted base files.
+ * A block found either way is neither copied back from HBM nor written.  When the file's last block has passed:
+ *   - link: the new path becomes a hard link to a base file if no block was written, the base file has the source
+ *     file's size and every block hash at the same index, the source file has no hard-link partner in src_dir, no
+ *     other path of this call was linked to that base inode, and the base inode already carries the owner, mode and
+ *     mtime the copy would get.  The same-path base file is tried first, then the others in table order, so a file
+ *     moved or renamed with its mtime kept is linked.  A linked inode's metadata is never changed (that would change
+ *     older snapshots too);
+ *   - backfill: otherwise the file is written new: changed blocks from the ring, the others copied from the base --
+ *     the same-path block when it matches, else the block that continues the previous block's base run, else the
+ *     first base block with that hash and length -- in runs contiguous in one base file (copy_file_range, or
+ *     pread/pwrite where that is refused), then its metadata applied.  Matches are whole blocks at block offsets.
+ * Before it links or copies from a base file the call re-checks its inode and ctime (the ctime it recorded, or the one
+ * this call's own link to it left); a base file that changed during the call fails it with VMIG_ESRCCHANGED naming the
+ * path (a retry copies that file in full).  A reused block trusts (XXH64, length) equality as the positional skip does:
+ * with n changed source blocks and m base blocks, a chance collision has probability at most n*m/2^64 (about 5e-8 for
+ * 1e6 x 1e6); VMIG_F_VERIFY re-reads linked and backfilled files.  Files none of whose blocks the base holds are copied
+ * as by vmig_migrate_tree; where the base table named the path but the file is not trusted, files_base_untrusted counts
+ * it.
  * Empty files are never linked.  out_table records the inode and ctime of every file as this call leaves it, linked
  * and hard-linked files included (vmig_migrate_tree records a hard-linked file before its links are made), so that the
  * next snapshot can use each one as a base.

@@ -103,8 +103,9 @@ func RestoreDirDiffVerifiedContext(ctx context.Context, snap, snapTable, dest, p
 }
 
 // SnapshotDirIncrementalVerified is SnapshotDirVerified that shares what did not change with the previous snapshot
-// baseDir, taken with baseTable (vmig_snapshot_tree): an unchanged file becomes a hard link to the base's, a changed
-// file takes its unchanged blocks from the base file.  The re-read (VMIG_F_VERIFY) covers linked files too, so a base
+// baseDir, taken with baseTable (vmig_snapshot_tree): an unchanged file becomes a hard link to the base's, also when it
+// was renamed or moved since, and a changed or copied file takes every block the base holds from the base file that
+// holds it, found by block hash.  The re-read (VMIG_F_VERIFY) covers linked files too, so a base
 // that rotted without moving its ctime is caught when the snapshot is taken.
 func SnapshotDirIncrementalVerified(src, dest, baseDir, baseTable, outTable string) error {
 	return SnapshotDirIncrementalVerifiedContext(context.Background(), src, dest, baseDir, baseTable, outTable)

@@ -47,8 +47,9 @@ EXPORTS = [
     "vmig_resident_set_len", "vmig_resident_upload", "vmig_resident_download", "vmig_resident_flip",
     "vmig_resident_set_prior", "vmig_resident_pass", "vmig_resident_results", "vmig_table_info_read",
     "vmig_table_hashes", "vmig_dir_size", "vmig_to_bytes", "vmig_datagen_files", "vmig_manifest", "vmig_link_probe", "vmig_thread_plan",
-    "vmig_ctl_open", "vmig_ctl_cancel", "vmig_ctl_progress", "vmig_ctl_close",
+    "vmig_ctl_open", "vmig_ctl_cancel", "vmig_ctl_progress", "vmig_ctl_close", "vmig_scrub_store",
 ]
+SCRUB_KINDS = ("missing", "extra", "resized", "block", "hardlink", "unreadable", "table", "dir")
 
 
 class Opts(C.Structure):
@@ -77,6 +78,14 @@ class Stats(C.Structure):
 class SnapshotStats(C.Structure):
     _fields_ = [(n, C.c_uint64) for n in ("files_linked", "bytes_linked", "files_backfilled", "bytes_backfilled",
                                           "files_base_untrusted")] + [("reserved", C.c_uint64 * 3)]
+
+    def as_dict(self) -> dict:
+        return {n: getattr(self, n) for n, _ in self._fields_ if n != "reserved"}
+
+
+class ScrubStats(C.Structure):
+    _fields_ = [(n, C.c_uint64) for n in ("versions", "versions_damaged", "bytes_referenced", "bytes_unique", "files_damaged",
+                                          "blocks_damaged", "files_unreadable")] + [("reserved", C.c_uint64 * 4)]
 
     def as_dict(self) -> dict:
         return {n: getattr(self, n) for n, _ in self._fields_ if n != "reserved"}
@@ -131,6 +140,8 @@ _sig = {
     "vmig_thread_plan": (C.c_int, [C.c_uint32, C.c_uint32, C.c_uint32, C.c_int, C.POINTER(C.c_uint32), C.POINTER(C.c_uint32)]),
     "vmig_ctl_open": (C.c_int, [C.POINTER(C.c_uint32)]), "vmig_ctl_cancel": (C.c_int, [C.c_uint32]),
     "vmig_ctl_progress": (C.c_int, [C.c_uint32, C.POINTER(Progress)]), "vmig_ctl_close": (C.c_int, [C.c_uint32]),
+    "vmig_scrub_store": (C.c_int, [C.c_uint32, C.POINTER(C.c_char_p), C.POINTER(C.c_char_p), C.c_char_p, C.POINTER(C.c_int32),
+                                   C.POINTER(Opts), C.POINTER(Stats), C.POINTER(ScrubStats)]),
 }
 for _n, (_r, _a) in _sig.items():
     _f = getattr(_lib, _n)
@@ -316,6 +327,73 @@ def snapshot_tree(src, dst, base=None, base_table=None, out_table=None, *, flags
     _check(_lib.vmig_snapshot_tree(_b(src), _b(dst), _b(base), _b(base_table), _b(out_table), C.byref(o), C.byref(st),
                                    C.byref(ss)), f"vmig_snapshot_tree({src} -> {dst}, base {base})")
     return {**st.as_dict(), **ss.as_dict()}
+
+
+def unescape_report_path(s: str) -> bytes:
+    """The inverse of the report's path escaping (include/vmig.h, vmig_scrub_store): "\\\\", "\\t", "\\n", "\\xHH"."""
+    raw, out, i = os.fsencode(s), bytearray(), 0
+    while i < len(raw):
+        c = raw[i]
+        if c != 0x5C:
+            out.append(c)
+            i += 1
+            continue
+        e = raw[i + 1:i + 2]
+        if e == b"\\":
+            out.append(0x5C)
+        elif e == b"t":
+            out.append(0x09)
+        elif e == b"n":
+            out.append(0x0A)
+        elif e == b"x":
+            out.append(int(raw[i + 2:i + 4], 16))
+            i += 2
+        else:
+            raise ValueError(f"bad escape in report path {s!r}")
+        i += 2
+    return bytes(out)
+
+
+def parse_scrub_report(path) -> list:
+    """The findings of a vmig_scrub_store report: dicts with version, kind, path (str, os.fsdecode of the raw name),
+    block, got and want (None where the report has "-")."""
+    out = []
+    with open(path, "rb") as f:
+        for line in f.read().split(b"\n"):
+            if not line:
+                continue
+            v, kind, p, blk, got, want = os.fsdecode(line).split("\t")
+            out.append({"version": int(v), "kind": kind, "path": os.fsdecode(unescape_report_path(p)),
+                        "block": None if blk == "-" else int(blk), "got": None if got == "-" else int(got, 16),
+                        "want": None if want == "-" else int(want, 16)})
+    return out
+
+
+def scrub_store(pairs, report=None, *, flags: int = 0, gpu_mask: int = 0, lanes_per_gpu: int = 0, block_bytes: int = 0,
+                ctl: Optional[Ctl] = None) -> dict:
+    """Check every version of a snapshot store, pairs = [(snap_dir, snap_table), ...], in one pass that reads each shared
+    inode once.  Returns {"verdicts": [VMIG_* per version], "findings": [...], "stats": the data pass's counters} plus
+    the vmig_scrub_stats fields.  A damaged version is a verdict, not an exception.  report: where the report file is
+    written (the findings are parsed from it); None: a temporary file that is removed afterwards."""
+    import tempfile
+    pairs = list(pairs)
+    n = len(pairs)
+    dirs = (C.c_char_p * max(n, 1))(*[_b(d) for d, _ in pairs])
+    tabs = (C.c_char_p * max(n, 1))(*[_b(t) for _, t in pairs])
+    verdicts = (C.c_int32 * max(n, 1))()
+    o = Opts(gpu_mask=gpu_mask, block_bytes=block_bytes, flags=flags, lanes_per_gpu=lanes_per_gpu, ctl=_ctl_id(ctl))
+    st, ss = Stats(), ScrubStats()
+    tmpdir = tempfile.mkdtemp(prefix="vmig_scrub_") if report is None else None
+    rpath = Path(tmpdir) / "scrub.txt" if tmpdir else Path(report)
+    try:
+        _check(_lib.vmig_scrub_store(n, dirs, tabs, _b(rpath), verdicts, C.byref(o), C.byref(st), C.byref(ss)),
+               f"vmig_scrub_store({n} versions)")
+        findings = parse_scrub_report(rpath)
+    finally:
+        if tmpdir:
+            import shutil
+            shutil.rmtree(tmpdir, ignore_errors=True)
+    return {"verdicts": list(verdicts[:n]), "findings": findings, "stats": st.as_dict(), **ss.as_dict()}
 
 
 def hash_tree(src, out_table, *, gpu_mask: int = 0, block_bytes: int = 0) -> dict:

@@ -9,6 +9,7 @@
 #include "vmig_table.h"
 #include "vmig_cufile.h"
 #include "vmig_reuse.h"
+#include "vmig_scrub.h"
 
 #include <fcntl.h>
 #include <unistd.h>
@@ -953,6 +954,157 @@ int check_snapshot_paths(const char* dst_dir, const char* base_dir)
     return VMIG_OK;
 }
 
+// ---------------------------------------------------------------------------------------------
+// vmig_scrub_store: the block pipeline reads each distinct inode of the store through a ScrubReader (vmig_scrub.h), in
+// hash-only mode; block b of inode u is BlockRef{file = u, table_idx = its index in the scrub's hash array}
+class ScrubIO : public BlockIO {
+public:
+    ScrubReader* r = nullptr;
+    uint32_t block_bytes = 4u << 20;
+    int read_block(const BlockRef& b, uint8_t* dst) override { return r->read(b.file, b.file_off, b.len, dst); }
+    int write_block(const BlockRef&, const uint8_t*) override { return fail(VMIG_EINVAL, "a scrub writes nothing"); }
+    uint32_t slot_align() override { return r->direct ? ScrubReader::kSector : 512; }
+    std::string block_name(const BlockRef& b) override {
+        const ScrubInode& I = (*r->inodes)[b.file];
+        return I.rel + " (version " + std::to_string(I.version) + ") block " + std::to_string(b.file_off / block_bytes);
+    }
+};
+
+int scrub_body(CallScope& call, uint32_t n, const char* const* dirs, const char* const* tables, const char* report_path,
+               int32_t* verdicts_out, const vmig_opts& o, vmig_stats* stats_out, vmig_scrub_stats* ss_out)
+{
+    CallCtl* ctl = call.ctl;
+    const std::atomic<int>* cancel = call.cancel();
+    vmig_stats st; memset(&st, 0, sizeof st);
+    vmig_scrub_stats ss; memset(&ss, 0, sizeof ss);
+    const uint64_t t_begin = now_ns();
+    if (cancel->load()) return fail(VMIG_ECANCELED, "the control was cancelled before the call started");
+    std::vector<DeviceInfo> devs;                    // no CPU fallback: the GPU is there before anything is read
+    int rc = ctx_select(o.gpu_mask, &devs);
+    if (rc) return rc;
+
+    // ---- walk every version, load its table, merge the two (every difference recorded)
+    call.phase(VMIG_PHASE_WALK);
+    uint64_t t0 = now_ns();
+    std::vector<Manifest> man(n);
+    std::vector<BlockTable> tab(n);
+    std::vector<const Manifest*> walked(n, nullptr);
+    std::vector<std::vector<int64_t>> tab_of(n);
+    std::vector<int32_t> verdict(n, VMIG_OK);
+    std::vector<ScrubFinding> findings;
+    auto whole = [&](uint32_t v, ScrubKind k, const char* path) {
+        ScrubFinding f; f.version = v; f.kind = k; f.path = path; findings.push_back(f);
+    };
+    for (uint32_t v = 0; v < n; v++) {
+        struct stat sb;
+        if (stat(dirs[v], &sb) != 0 || !S_ISDIR(sb.st_mode)) { verdict[v] = VMIG_ENOTDIR; whole(v, kScrubDir, "."); continue; }
+        rc = walk_tree(dirs[v], o.block_bytes, (o.flags & VMIG_F_SKIP_HIDDEN_TOPDIRS) != 0, &man[v], cancel);
+        if (rc == VMIG_ECANCELED || rc == VMIG_ESRCCHANGED || rc == VMIG_ENOMEM) return rc;
+        if (rc) { verdict[v] = VMIG_ECORRUPT; whole(v, kScrubUnreadable, "."); continue; }      // a directory that cannot be read
+        ss.bytes_referenced += man[v].bytes_total;
+        if (table_load(tables[v], &tab[v]) != VMIG_OK || tab[v].block_bytes != o.block_bytes) { verdict[v] = VMIG_ETABLE; whole(v, kScrubTable, "."); continue; }
+        if (scrub_merge_table(v, man[v], tab[v], &tab_of[v], &findings)) verdict[v] = VMIG_ECORRUPT;
+        walked[v] = &man[v];
+    }
+    st.ns_walk = now_ns() - t0;
+
+    // ---- one block list over the distinct inodes
+    t0 = now_ns();
+    std::vector<ScrubInode> inodes;
+    std::vector<std::vector<uint32_t>> inode_of;
+    rc = scrub_group_inodes(walked, tab_of, o.block_bytes, &inodes, &inode_of);
+    if (rc) return rc;
+    uint64_t n_blocks = 0;
+    for (const ScrubInode& I : inodes) { ss.bytes_unique += I.size; n_blocks += I.n_blocks; }
+    ctl->bytes_total.store(ss.bytes_unique); ctl->blocks_total.store(n_blocks);
+    std::vector<int> root_fds(n, -1);
+    auto close_roots = [&] { for (int& fd : root_fds) if (fd >= 0) { close(fd); fd = -1; } };
+    for (const ScrubInode& I : inodes)
+        if (root_fds[I.version] < 0) {
+            root_fds[I.version] = open(dirs[I.version], O_RDONLY | O_DIRECTORY | O_CLOEXEC);
+            if (root_fds[I.version] < 0) { const int e = errno; close_roots(); return fail(VMIG_ESRCCHANGED, "open %s: %s", dirs[I.version], errno_str(e).c_str()); }
+        }
+    ScrubReader reader;
+    reader.root_fds = root_fds; reader.inodes = &inodes; reader.direct = (o.flags & VMIG_F_DIRECT_IO) != 0;
+    reader.init();
+    ScrubIO io; io.r = &reader; io.block_bytes = o.block_bytes;
+    // inodes in groups of 64 (bounds open descriptors), blocks round-robin across a group's inodes: as a migration does
+    std::vector<BlockRef> blocks; blocks.reserve(n_blocks);
+    for (size_t g = 0; g < inodes.size(); g += 64) {
+        const size_t g1 = std::min(inodes.size(), g + 64);
+        uint64_t maxb = 0;
+        for (size_t u = g; u < g1; u++) maxb = std::max(maxb, inodes[u].n_blocks);
+        for (uint64_t r = 0; r < maxb; r++)
+            for (size_t u = g; u < g1; u++) {
+                const ScrubInode& I = inodes[u];
+                if (r >= I.n_blocks) continue;
+                BlockRef b; b.file = (uint32_t)u; b.file_off = r * (uint64_t)o.block_bytes;
+                b.len = (uint32_t)std::min<uint64_t>(o.block_bytes, I.size - b.file_off);
+                b.table_idx = I.first_block + r; b.prior_hash = 0; b.prior_valid = 0;
+                blocks.push_back(b);
+            }
+    }
+    st.ns_plan = now_ns() - t0;
+
+    // ---- the data pass: K1 over every distinct block, once
+    call.phase(VMIG_PHASE_DATA);
+    if (cancel->load()) { close_roots(); return fail(VMIG_ECANCELED, "before the data pass"); }
+    t0 = now_ns();
+    std::vector<uint64_t> hashes(n_blocks, 0);
+    rc = run_blocks(blocks, &io, false, true, o, hashes.data(), &st, ctl, false);
+    reader.close_all();
+    close_roots();
+    st.ns_data = now_ns() - t0;
+    if (rc) return rc;
+
+    // ---- compare every table record with the hashes of the inode it names
+    t0 = now_ns();
+    std::unordered_set<uint64_t> bad_blocks;
+    for (uint32_t v = 0; v < n; v++) {
+        if (!walked[v]) continue;
+        const Manifest& m = man[v];
+        for (size_t f = 0; f < m.files.size(); f++) {
+            const uint32_t u = inode_of[v][f];
+            if (u == kNoInode) continue;
+            const Entry& e = m.files[f];
+            const ScrubInode& I = inodes[u];
+            if (reader.unreadable(u)) { verdict[v] = VMIG_ECORRUPT; whole(v, kScrubUnreadable, e.rel.c_str()); continue; }
+            const TableFile& tf = tab[v].files[(size_t)tab_of[v][f]];
+            for (uint64_t r = 0; r < e.n_blocks; r++) {
+                const uint64_t got = hashes[I.first_block + r], want = tab[v].hashes[tf.first_block + r];
+                if (got == want) continue;
+                ScrubFinding x; x.version = v; x.kind = e.hardlink_of >= 0 ? kScrubHardlink : kScrubBlock; x.path = e.rel;
+                x.block = (int64_t)r; x.has_hashes = true; x.got = got; x.want = want;
+                findings.push_back(x);
+                bad_blocks.insert(I.first_block + r);
+                verdict[v] = VMIG_ECORRUPT;
+            }
+        }
+    }
+    for (uint32_t u = 0; u < inodes.size(); u++) ss.files_unreadable += reader.unreadable(u);
+    scrub_sort(&findings);
+    for (size_t i = 0; i < findings.size(); i++) {
+        const ScrubFinding& f = findings[i];
+        if (f.kind == kScrubTable || f.kind == kScrubDir || (f.kind == kScrubUnreadable && f.path == ".")) continue;
+        if (i && findings[i - 1].version == f.version && findings[i - 1].path == f.path) continue;   // sorted: one count per path
+        ss.files_damaged++;
+    }
+    ss.versions = n; ss.blocks_damaged = bad_blocks.size();
+    for (int32_t x : verdict) ss.versions_damaged += x != VMIG_OK;
+    if (report_path && *report_path) {
+        rc = scrub_report_store(report_path, findings, cancel);
+        if (rc) return rc;
+    }
+    st.ns_table = now_ns() - t0;
+    st.files_direct = reader.n_direct.load();
+    st.bytes_total = ss.bytes_unique; st.blocks_total = n_blocks; st.files = inodes.size();
+    st.ns_total = now_ns() - t_begin;
+    if (verdicts_out) std::copy(verdict.begin(), verdict.end(), verdicts_out);
+    if (stats_out) *stats_out = st;
+    if (ss_out) *ss_out = ss;
+    return VMIG_OK;
+}
+
 }  // namespace
 
 // =============================================================================================
@@ -1070,6 +1222,23 @@ int vmig_snapshot_tree(const char* src_dir, const char* dst_dir, const char* bas
     if (snap_stats) memset(snap_stats, 0, sizeof *snap_stats);
     const SnapshotArgs sa{has_dir ? base_dir : nullptr, has_table ? base_table : nullptr, snap_stats};
     return migrate_tree_impl(src_dir, dst_dir, nullptr, out_table, opts, stats, nullptr, &sa);
+}
+int vmig_scrub_store(uint32_t n, const char* const* snap_dirs, const char* const* snap_tables, const char* report_path,
+                     int32_t* verdicts, const vmig_opts* opts, vmig_stats* stats, vmig_scrub_stats* scrub_stats)
+{
+    if (n == 0) return fail(VMIG_EINVAL, "n == 0: no version to scrub");
+    if (!snap_dirs || !snap_tables) return fail(VMIG_EINVAL, "snap_dirs / snap_tables is NULL");
+    for (uint32_t i = 0; i < n; i++)
+        if (!snap_dirs[i] || !*snap_dirs[i] || !snap_tables[i] || !*snap_tables[i]) return fail(VMIG_EINVAL, "version %u: snap_dir or snap_table is NULL/empty", i);
+    const vmig_opts o = norm_opts(opts);                     // VMIG_CUFILE=1 in the environment is refused too
+    const uint32_t allowed = VMIG_F_DIRECT_IO | VMIG_F_SKIP_HIDDEN_TOPDIRS;
+    if (o.flags & ~allowed) return fail(VMIG_EINVAL, "flags 0x%x: a scrub takes only VMIG_F_DIRECT_IO and VMIG_F_SKIP_HIDDEN_TOPDIRS", o.flags & ~allowed);
+    if (o.block_bytes & 4095u) return fail(VMIG_EINVAL, "block_bytes %u is not a multiple of 4096", o.block_bytes);
+    if (o.block_bytes > pipe_slot_bytes()) return fail(VMIG_EINVAL, "block_bytes %u exceeds the staging slot (%u)", o.block_bytes, pipe_slot_bytes());
+    CallScope call;
+    const int rc = call.attach(o.ctl);
+    if (rc) return rc;
+    return call.finish(scrub_body(call, n, snap_dirs, snap_tables, report_path, verdicts, o, stats, scrub_stats));
 }
 int vmig_copy_dir(const char* src_dir, const char* dst_dir) { return migrate_tree_impl(src_dir, dst_dir, nullptr, nullptr, nullptr, nullptr); }
 int vmig_move_dir(const char* src_dir, const char* dst_dir)

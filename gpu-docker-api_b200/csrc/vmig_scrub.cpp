@@ -1,0 +1,248 @@
+// vmig_scrub.cpp -- the host side of vmig_scrub_store (see vmig_scrub.h).
+#include "vmig_scrub.h"
+#include "vmig_common.h"
+
+#include <fcntl.h>
+#include <unistd.h>
+#include <sys/stat.h>
+#include <sys/syscall.h>
+#include <algorithm>
+#include <cctype>
+#include <cstdlib>
+#include <map>
+#include <tuple>
+#include <utility>
+
+namespace vmig {
+
+const char* scrub_kind_name(ScrubKind k)
+{
+    static const char* const names[] = {"missing", "extra", "resized", "block", "hardlink", "unreadable", "table", "dir"};
+    return k <= kScrubDir ? names[k] : "?";
+}
+
+size_t scrub_merge_table(uint32_t version, const Manifest& man, const BlockTable& t, std::vector<int64_t>* tab_of,
+                         std::vector<ScrubFinding>* out)
+{
+    tab_of->assign(man.files.size(), -1);
+    size_t i = 0, j = 0, n = 0;
+    auto add = [&](ScrubKind k, const std::string& rel) {
+        ScrubFinding f; f.version = version; f.kind = k; f.path = rel;
+        out->push_back(std::move(f)); n++;
+    };
+    while (i < man.files.size() || j < t.files.size()) {
+        if (j == t.files.size() || (i < man.files.size() && man.files[i].rel < t.files[j].rel)) { add(kScrubExtra, man.files[i].rel); i++; continue; }
+        if (i == man.files.size() || t.files[j].rel < man.files[i].rel) { add(kScrubMissing, t.files[j].rel); j++; continue; }
+        if (man.files[i].size != t.files[j].size) add(kScrubResized, man.files[i].rel);
+        else (*tab_of)[i] = (int64_t)j;
+        i++; j++;
+    }
+    return n;
+}
+
+int scrub_group_inodes(const std::vector<const Manifest*>& mans, const std::vector<std::vector<int64_t>>& tab_of,
+                       uint32_t block_bytes, std::vector<ScrubInode>* inodes, std::vector<std::vector<uint32_t>>* inode_of)
+{
+    inodes->clear();
+    inode_of->assign(mans.size(), {});
+    std::map<std::pair<uint64_t, uint64_t>, uint32_t> seen;
+    uint64_t fb = 0;
+    for (size_t v = 0; v < mans.size(); v++) {
+        if (!mans[v]) continue;
+        const Manifest& m = *mans[v];
+        (*inode_of)[v].assign(m.files.size(), kNoInode);
+        for (size_t f = 0; f < m.files.size() && f < tab_of[v].size(); f++) {
+            const Entry& e = m.files[f];
+            if (tab_of[v][f] < 0 || e.size == 0) continue;
+            auto it = seen.find({e.dev, e.ino});
+            uint32_t u;
+            if (it == seen.end()) {
+                u = (uint32_t)inodes->size();
+                const uint64_t nb = (e.size + block_bytes - 1) / block_bytes;
+                inodes->push_back({e.dev, e.ino, e.size, fb, nb, (uint32_t)v, e.rel});
+                fb += nb;
+                seen.emplace(std::make_pair(e.dev, e.ino), u);
+            } else {
+                u = it->second;
+                const ScrubInode& I = (*inodes)[u];
+                if (I.size != e.size)
+                    return fail(VMIG_ESRCCHANGED, "inode %llu is %llu bytes as version %u's %s and %llu bytes as version %zu's %s: the store changed during the scrub",
+                                (unsigned long long)e.ino, (unsigned long long)I.size, I.version, I.rel.c_str(), (unsigned long long)e.size, v, e.rel.c_str());
+            }
+            (*inode_of)[v][f] = u;
+        }
+    }
+    return VMIG_OK;
+}
+
+std::string scrub_escape(const std::string& s)
+{
+    std::string o;
+    o.reserve(s.size());
+    for (unsigned char c : s) {
+        if (c == '\\') o += "\\\\";
+        else if (c == '\t') o += "\\t";
+        else if (c == '\n') o += "\\n";
+        else if (c < 0x20) { char b[8]; snprintf(b, sizeof b, "\\x%02x", c); o += b; }
+        else o += (char)c;
+    }
+    return o;
+}
+
+bool scrub_unescape(const std::string& s, std::string* out)
+{
+    out->clear();
+    for (size_t i = 0; i < s.size(); i++) {
+        if (s[i] != '\\') { *out += s[i]; continue; }
+        if (++i == s.size()) return false;
+        if (s[i] == '\\') *out += '\\';
+        else if (s[i] == 't') *out += '\t';
+        else if (s[i] == 'n') *out += '\n';
+        else if (s[i] == 'x' && i + 2 < s.size() && isxdigit((unsigned char)s[i + 1]) && isxdigit((unsigned char)s[i + 2])) {
+            *out += (char)strtoul(s.substr(i + 1, 2).c_str(), nullptr, 16);
+            i += 2;
+        } else return false;
+    }
+    return true;
+}
+
+std::string scrub_format(const ScrubFinding& f)
+{
+    char b[96];
+    std::string line = std::to_string(f.version) + "\t" + scrub_kind_name(f.kind) + "\t" + scrub_escape(f.path) + "\t";
+    line += f.block >= 0 ? std::to_string(f.block) : "-";
+    if (f.has_hashes) { snprintf(b, sizeof b, "\t%016llx\t%016llx\n", (unsigned long long)f.got, (unsigned long long)f.want); line += b; }
+    else line += "\t-\t-\n";
+    return line;
+}
+
+void scrub_sort(std::vector<ScrubFinding>* v)
+{
+    std::stable_sort(v->begin(), v->end(), [](const ScrubFinding& a, const ScrubFinding& b) {
+        return std::tie(a.version, a.path, a.block) < std::tie(b.version, b.path, b.block);
+    });
+}
+
+int scrub_report_store(const std::string& path, const std::vector<ScrubFinding>& v, const std::atomic<int>* cancel)
+{
+    if (cancel && cancel->load()) return fail(VMIG_ECANCELED, "cancelled before the scrub report %s was written", path.c_str());
+    std::string raw;
+    for (const ScrubFinding& f : v) raw += scrub_format(f);
+    const std::string tmp = path + ".tmp." + std::to_string((long)getpid()) + "." + std::to_string((long)syscall(SYS_gettid));
+    int fd = open(tmp.c_str(), O_WRONLY | O_CREAT | O_TRUNC | O_CLOEXEC, 0644);
+    if (fd < 0) return fail(VMIG_EIO, "create %s: %s", tmp.c_str(), errno_str(errno).c_str());
+    size_t put = 0;
+    while (put < raw.size()) {
+        ssize_t w = write(fd, raw.data() + put, raw.size() - put);
+        if (w <= 0) { const int e = errno; close(fd); unlink(tmp.c_str()); return fail(VMIG_EIO, "write %s: %s", tmp.c_str(), errno_str(e).c_str()); }
+        put += (size_t)w;
+    }
+    if (fsync(fd) != 0) { const int e = errno; close(fd); unlink(tmp.c_str()); return fail(VMIG_EIO, "fsync %s: %s", tmp.c_str(), errno_str(e).c_str()); }
+    close(fd);
+    if (cancel && cancel->load()) { unlink(tmp.c_str()); return fail(VMIG_ECANCELED, "cancelled before the scrub report %s was renamed into place", path.c_str()); }
+    if (rename(tmp.c_str(), path.c_str()) != 0) { const int e = errno; unlink(tmp.c_str()); return fail(VMIG_EIO, "rename %s: %s", path.c_str(), errno_str(e).c_str()); }
+    return VMIG_OK;
+}
+
+// ---------------------------------------------------------------------------------------------
+void ScrubReader::init()
+{
+    n_st = inodes->size();
+    st.reset(new State[n_st ? n_st : 1]);
+    for (size_t u = 0; u < n_st; u++) st[u].reads_left.store((uint32_t)(*inodes)[u].n_blocks);
+}
+
+void ScrubReader::adopt(uint32_t u, int fd, bool is_direct)
+{
+    st[u].s_direct = is_direct;
+    st[u].fd.store(fd, std::memory_order_release);
+}
+
+std::string ScrubReader::why(uint32_t u)
+{
+    std::lock_guard<std::mutex> lk(stripes[u & 63]);
+    return st[u].why;
+}
+
+void ScrubReader::mark_bad(uint32_t u, const std::string& why)
+{
+    std::lock_guard<std::mutex> lk(stripes[u & 63]);
+    if (!st[u].bad.load()) st[u].why = why;
+    st[u].bad.store(true);
+}
+
+void ScrubReader::done_one(uint32_t u)
+{
+    if (st[u].reads_left.fetch_sub(1) != 1) return;
+    const int fd = st[u].fd.exchange(-1);
+    if (fd >= 0) close(fd);
+}
+
+void ScrubReader::close_all()
+{
+    for (size_t u = 0; u < n_st; u++) {
+        const int fd = st[u].fd.exchange(-1);
+        if (fd >= 0) close(fd);
+    }
+}
+
+// VMIG_OK with *out; VMIG_ESRCCHANGED: not the walked inode any more; any other code: the inode cannot be opened
+int ScrubReader::open_inode(uint32_t u, int* out)
+{
+    State& s = st[u];
+    int fd = s.fd.load(std::memory_order_acquire);
+    if (fd >= 0) { *out = fd; return VMIG_OK; }
+    std::lock_guard<std::mutex> lk(stripes[u & 63]);
+    fd = s.fd.load(std::memory_order_acquire);
+    if (fd >= 0) { *out = fd; return VMIG_OK; }
+    const ScrubInode& I = (*inodes)[u];
+    const int root = root_fds[I.version];
+    int rc = VMIG_EIO;
+    if (direct) { rc = open_beneath(root, I.rel, O_RDONLY | O_NONBLOCK | O_DIRECT, &fd); s.s_direct = rc == VMIG_OK; }
+    if (rc) rc = open_beneath(root, I.rel, O_RDONLY | O_NONBLOCK, &fd);        // the filesystem may refuse O_DIRECT
+    if (rc) return rc;
+    struct stat sb;
+    if (fstat(fd, &sb) != 0) { const int e = errno; close(fd); return fail(VMIG_EIO, "fstat %s: %s", I.rel.c_str(), errno_str(e).c_str()); }
+    if (!S_ISREG(sb.st_mode) || (uint64_t)sb.st_dev != I.dev || (uint64_t)sb.st_ino != I.ino || (uint64_t)sb.st_size != I.size) {
+        close(fd);
+        return fail(VMIG_ESRCCHANGED, "%s (version %u) is no longer the %llu-byte regular file the walk saw: the store changed during the scrub",
+                    I.rel.c_str(), I.version, (unsigned long long)I.size);
+    }
+    if (s.s_direct) n_direct++;
+    s.fd.store(fd, std::memory_order_release);
+    *out = fd;
+    return VMIG_OK;
+}
+
+int ScrubReader::read(uint32_t u, uint64_t off, uint32_t len, uint8_t* dst)
+{
+    State& s = st[u];
+    if (s.bad.load()) { done_one(u); return VMIG_OK; }             // the rest of an unreadable inode is not read
+    int fd;
+    int rc = open_inode(u, &fd);
+    if (rc == VMIG_ESRCCHANGED) return rc;
+    if (rc) { mark_bad(u, last_error_cstr()); done_one(u); return VMIG_OK; }
+    const ScrubInode& I = (*inodes)[u];
+    // O_DIRECT: buffer, offset and length in whole sectors (the pipeline's slot layout leaves the room), as FileIO reads
+    const size_t want = s.s_direct ? (size_t)align_up(len, kSector) : len;
+    size_t got = 0;
+    while (got < len) {
+        const size_t pos = s.s_direct ? (got & ~(size_t)(kSector - 1)) : got;
+        const ssize_t r = pread(fd, dst + pos, want - pos, (off_t)(off + pos));
+        if (r < 0) {
+            if (errno == EINTR) continue;
+            char b[64]; snprintf(b, sizeof b, " at offset %llu: ", (unsigned long long)(off + pos));
+            mark_bad(u, "pread " + I.rel + b + errno_str(errno));
+            done_one(u);
+            return VMIG_OK;
+        }
+        if (r == 0 || pos + (size_t)r <= got)
+            return fail(VMIG_ESRCCHANGED, "%s (version %u) shrank during the scrub (wanted %u bytes at %llu, got %zu)", I.rel.c_str(), I.version,
+                        len, (unsigned long long)off, got);
+        got = pos + (size_t)r;
+    }
+    done_one(u);
+    return VMIG_OK;
+}
+
+}  // namespace vmig

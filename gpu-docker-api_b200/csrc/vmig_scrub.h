@@ -1,0 +1,101 @@
+// vmig_scrub.h -- the host side of vmig_scrub_store: check every version of a snapshot store against its block table,
+// reading each inode the versions share once (DESIGN.md §6).
+//
+// The per-byte work is K1's, through the block pipeline in hash-only mode, exactly as a checked restore reads.  What is
+// here is the plan around it: the table merge that lists every difference instead of stopping at the first, the grouping
+// of all versions' regular files by (st_dev, st_ino), the reader that turns an unreadable inode into a finding instead
+// of a call failure, and the report.  No CUDA header is needed (tests/scrub_unit.cpp builds it with g++ alone).
+#pragma once
+#include <stdint.h>
+#include <atomic>
+#include <memory>
+#include <mutex>
+#include <string>
+#include <vector>
+#include "vmig_table.h"
+#include "vmig_tree.h"
+
+namespace vmig {
+
+enum ScrubKind : uint8_t { kScrubMissing, kScrubExtra, kScrubResized, kScrubBlock, kScrubHardlink, kScrubUnreadable, kScrubTable, kScrubDir };
+const char* scrub_kind_name(ScrubKind k);
+
+// One line of the report.  block < 0: the finding is about the whole path ("-"); has_hashes: got / want are printed.
+struct ScrubFinding {
+    uint32_t version = 0;
+    ScrubKind kind = kScrubBlock;
+    std::string path;
+    int64_t block = -1;
+    bool has_hashes = false;
+    uint64_t got = 0, want = 0;
+};
+
+// The merge of restore's plan-time check (the walked regular-file paths must be the table's, each with the table's
+// size), recording every difference: a path only in the walk is `extra`, only in the table `missing`, in both with other
+// sizes `resized`.  (*tab_of)[f] is the table index of manifest file f when both name it with one size, else -1.
+// Returns the number of findings appended.
+size_t scrub_merge_table(uint32_t version, const Manifest& man, const BlockTable& t, std::vector<int64_t>* tab_of,
+                         std::vector<ScrubFinding>* out);
+
+// One distinct inode of the store: read once, its blocks at [first_block, first_block + n_blocks) of the scrub's hash
+// array.  (version, rel) is the first path that names it; it is opened there.
+struct ScrubInode { uint64_t dev, ino, size, first_block, n_blocks; uint32_t version; std::string rel; };
+static constexpr uint32_t kNoInode = 0xFFFFFFFFu;
+
+// Group the matched, non-empty regular files of every version (tab_of[v][f] >= 0; mans[v] may be null for a version
+// that was not walked) by (dev, ino).  (*inode_of)[v][f] is the inode's index, kNoInode where the path is not read.
+// Two paths of one inode with different sizes mean the store changed between the walks: VMIG_ESRCCHANGED.
+int scrub_group_inodes(const std::vector<const Manifest*>& mans, const std::vector<std::vector<int64_t>>& tab_of,
+                       uint32_t block_bytes, std::vector<ScrubInode>* inodes, std::vector<std::vector<uint32_t>>* inode_of);
+
+// Report paths: '\' -> "\\", tab -> "\t", newline -> "\n", any other byte below 0x20 -> "\xHH" (two lower-case hex
+// digits).  scrub_unescape is the inverse; false on a malformed escape.
+std::string scrub_escape(const std::string& s);
+bool scrub_unescape(const std::string& s, std::string* out);
+// "<version>\t<kind>\t<path>\t<block|->\t<got|->\t<want|->\n", hashes as 16 lower-case hex digits
+std::string scrub_format(const ScrubFinding& f);
+// by version, then path (bytewise), then block ("-" first)
+void scrub_sort(std::vector<ScrubFinding>* v);
+// Atomic, like a block table: path.tmp.<pid>.<tid>, fsync, rename.  A non-zero *cancel before the rename removes the
+// .tmp and returns VMIG_ECANCELED; any failure leaves no .tmp.
+int scrub_report_store(const std::string& path, const std::vector<ScrubFinding>& v, const std::atomic<int>* cancel);
+
+// The scrub's source of block bytes.  An inode is opened lazily beneath the root of the version that names it first
+// (open_beneath: no symlink followed), O_RDONLY, O_DIRECT when asked and the filesystem allows it.  An inode that is no
+// longer the walked one (other dev/ino, not a regular file, other size, shorter than its blocks, or its path gone) is
+// VMIG_ESRCCHANGED, a call failure as everywhere else.  Any other open or read error does NOT fail: the inode is marked
+// unreadable, its remaining blocks are not read, and read() returns VMIG_OK so the pipeline's first-error latch stays
+// clear.  Thread-safe; the descriptor is closed after the inode's last block.
+class ScrubReader {
+public:
+    std::vector<int> root_fds;                 // per version; -1 for a version that is not read (not owned)
+    const std::vector<ScrubInode>* inodes = nullptr;
+    bool direct = false;                       // VMIG_F_DIRECT_IO
+    static constexpr uint32_t kSector = 4096;
+    std::atomic<uint64_t> n_direct{0};         // descriptors really opened O_DIRECT
+
+    void init();                               // after inodes is set: one reads_left per block
+    int read(uint32_t u, uint64_t off, uint32_t len, uint8_t* dst);
+    void adopt(uint32_t u, int fd, bool is_direct);   // use this open descriptor for inode u (tests/scrub_unit.cpp)
+    bool unreadable(uint32_t u) const { return st[u].bad.load(); }
+    std::string why(uint32_t u);               // the error that made u unreadable
+    void close_all();
+    ~ScrubReader() { close_all(); }
+
+private:
+    struct State {
+        std::atomic<int> fd{-1};
+        std::atomic<uint32_t> reads_left{0};
+        std::atomic<bool> bad{false};
+        bool s_direct = false;
+        std::string why;                       // under the inode's stripe
+    };
+    std::unique_ptr<State[]> st;
+    size_t n_st = 0;
+    std::mutex stripes[64];
+    int open_inode(uint32_t u, int* out);
+    void mark_bad(uint32_t u, const std::string& why);
+    void done_one(uint32_t u);
+};
+
+}  // namespace vmig

@@ -115,6 +115,7 @@ static int walk_dir(int dfd, const std::string& rel, uint32_t block_bytes, bool 
         case S_IFREG: {
             e.type = kFile; e.size = (uint64_t)st.st_size;
             e.n_blocks = (e.size + block_bytes - 1) / block_bytes;
+            e.dev = (uint64_t)st.st_dev; e.ino = (uint64_t)st.st_ino;
             if (st.st_nlink > 1) {                   // group key (device:inode); resolved to an index after sorting
                 char key[48]; snprintf(key, sizeof key, "%llx:%llx", (unsigned long long)st.st_dev, (unsigned long long)st.st_ino);
                 e.target = key;

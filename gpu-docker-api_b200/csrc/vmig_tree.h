@@ -32,6 +32,7 @@ struct Entry {
     int64_t     hardlink_of = -1;   // files: index (in Manifest::files) of the first path to the same inode
     uint64_t    first_block = 0;    // files: index of this file's first hash in the block table
     uint64_t    n_blocks = 0;
+    uint64_t    dev = 0, ino = 0;   // files: st_dev / st_ino as the walk saw them (vmig_scrub_store groups paths by inode)
 };
 
 struct Manifest {

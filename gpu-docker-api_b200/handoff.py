@@ -22,7 +22,7 @@ from typing import Callable, Optional
 import threading
 
 from . import (F_PRUNE, F_VERIFY, VMIG_ECANCELED, Ctl, GetContainerMergedLayer, GetVolumeMountPoint, VmigError, manifest,
-               migrate_tree, restore_tree, snapshot_tree)
+               migrate_tree, restore_tree, scrub_store, snapshot_tree)
 
 log = logging.getLogger("vmig.handoff")
 _root: dict = {"cwd": None}
@@ -113,6 +113,28 @@ def SnapshotVersionIncremental(ctrVersionName: str) -> dict:
         return SnapshotDirVerified(upper, data, table)
     baseData, baseTable = snapshotPaths(base)
     return SnapshotDirIncrementalVerified(upper, data, baseData, baseTable, table)
+
+
+def ScrubReplicaSet(rs: str) -> dict:
+    """N1: check every snapshot of the ReplicaSet against its block table in one pass (vmig_scrub_store) that reads each
+    inode the versions share once.  The versions are the merges/<rs>/<rs>-<k> that hold diff/ (the rule of baseVersion;
+    a missing blocks.vmig is that version's VMIG_ETABLE).  Returns {"verdicts": {version name: VMIG_* verdict},
+    "report": merges/<rs>/scrub.txt}, the report listing every damaged path and block."""
+    parent = versionDir(rs + "-0").parent
+    found = []
+    for d in (parent.iterdir() if parent.is_dir() else ()):
+        k = d.name[len(rs) + 1:]
+        if not d.name.startswith(rs + "-") or not k.isdigit():
+            continue
+        if (d / "diff").is_dir():
+            found.append((int(k), d.name))
+    found.sort()
+    names = [name for _, name in found]
+    report = parent / "scrub.txt"
+    if not names:
+        return {"verdicts": {}, "report": None}
+    out = scrub_store([snapshotPaths(name) for name in names], report)
+    return {"verdicts": dict(zip(names, out["verdicts"])), "report": report}
 
 
 def RollbackFromSnapshot(targetCtrVersionName: str, newContainer: str, seedTable=None) -> dict:

@@ -242,6 +242,58 @@ int vmig_snapshot_tree(const char* src_dir, const char* dst_dir,
                        const char* out_table, const vmig_opts* opts /*nullable*/,
                        vmig_stats* stats /*nullable*/, vmig_snapshot_stats* snap_stats /*nullable*/);
 
+/* Scrub of a snapshot store: what vmig_scrub_store read and found. */
+typedef struct vmig_scrub_stats {
+    uint64_t versions, versions_damaged;   /* versions whose verdict is not VMIG_OK                                  */
+    uint64_t bytes_referenced;             /* sum of regular-file sizes over all versions' walks (per path)          */
+    uint64_t bytes_unique;                 /* bytes of distinct inodes read and hashed: what the scrub cost          */
+    uint64_t files_damaged;                /* (version, path) pairs with at least one finding                        */
+    uint64_t blocks_damaged;               /* (inode, block) pairs whose hash differs from some table naming it      */
+    uint64_t files_unreadable;             /* distinct inodes that failed to read (every naming version damaged)     */
+    uint64_t reserved[4];
+} vmig_scrub_stats;
+
+/* Check the n versions of a snapshot store -- snap_dirs[i] written together with its block table snap_tables[i] by
+ * vmig_snapshot_tree -- in one pass that reads each distinct inode once, however many versions hard-link it.  Nothing
+ * is written under any snap_dir and no table is touched: inode ctimes stay as they were, so the identities the next
+ * incremental snapshot trusts stay valid.
+ *   - verdicts[i] (nullable; n entries, written on success) is what vmig_restore_tree(snap_dirs[i], snap_tables[i],
+ *     NULL, NULL, NULL, {VMIG_F_HASH_ONLY}) returns for that version, with two differences: a snapshot directory that
+ *     is missing or not a directory is VMIG_ENOTDIR (restore: VMIG_EIO when missing), and a file that cannot be read
+ *     (or a directory of the version that cannot be walked) is VMIG_ECORRUPT (restore: VMIG_EIO):
+ *       VMIG_OK        the version matches its table;
+ *       VMIG_ECORRUPT  a path is missing, extra or resized, a block's XXH64 differs from the table's, a hard-linked
+ *                      path's table hashes differ from what its primary holds, or a file could not be read;
+ *       VMIG_ETABLE    the table is missing, cannot be loaded, or its block_bytes differs from the call's;
+ *       VMIG_ENOTDIR   the snapshot directory is missing or is not a directory.
+ *   - A damaged version is a result, not a failure: the call returns VMIG_OK when it ran to the end.  It fails with
+ *     VMIG_EINVAL (n == 0, a NULL array or entry, flags other than VMIG_F_DIRECT_IO | VMIG_F_SKIP_HIDDEN_TOPDIRS, bad
+ *     block_bytes), VMIG_ENOGPU (checked before anything is read), VMIG_ECANCELED, VMIG_ECUDA, VMIG_ENOMEM,
+ *     VMIG_ESRCCHANGED (an inode is no longer the one the walk saw -- other inode, type or size, or shorter than its
+ *     blocks: the store was modified during the scrub) or VMIG_EIO (writing the report).  A failed call writes no
+ *     verdicts and leaves report_path as it was, with no .tmp beside it.
+ *   - Plan: every version is walked as restore walks it, its table merged against the walk (every difference recorded),
+ *     and the matched regular files of all versions grouped by (st_dev, st_ino).  Each distinct inode is read once
+ *     through the block pipeline in hash-only mode -- lanes, GPUs and VMIG_F_DIRECT_IO as in a checked restore; with
+ *     VMIG_F_DIRECT_IO what is checked is what the device holds -- and each block hash is then compared on the host with
+ *     every table record that names that inode.  An inode that fails to open or read is not a call failure: it is
+ *     reported `unreadable` for every version that names it, and its remaining blocks are not read.
+ *   - report_path (nullable): one line per finding, sorted by version, then path (bytewise), then block:
+ *       <version index>\t<kind>\t<path>\t<block|->\t<got|->\t<want|->\n
+ *     kind: missing, extra, resized, block (a primary path's block), hardlink (a hard-linked path's block), unreadable,
+ *     table, dir (the last two with path "."); got / want: 16 lower-case hex digits (block and hardlink only).  In paths
+ *     '\' is "\\", tab "\t", newline "\n" and any other byte below 0x20 "\xHH".  Written like a table: tmp, fsync,
+ *     rename; an empty file when nothing was found.
+ *   - Control: vmig_opts.ctl as for the tree calls; phases WALK, DATA, DONE; bytes_total is bytes_unique and
+ *     bytes_hashed counts unique bytes.  stats (nullable): the vmig_stats of the data pass (bytes_h2d == bytes_unique,
+ *     bytes_total / blocks_total / files: the distinct inodes).
+ * Directories, symlinks, specials and metadata are not in the tables and are not checked, as for restore.  The walk flag
+ * VMIG_F_SKIP_HIDDEN_TOPDIRS must be the one the snapshots were taken with. */
+int vmig_scrub_store(uint32_t n, const char* const* snap_dirs, const char* const* snap_tables,
+                     const char* report_path /*nullable*/, int32_t* verdicts /*n, nullable*/,
+                     const vmig_opts* opts /*nullable*/, vmig_stats* stats /*nullable*/,
+                     vmig_scrub_stats* scrub_stats /*nullable*/);
+
 /* utils.CopyDir(src, dest) (reference utils/copy.go:21-27) == vmig_migrate_tree with defaults. */
 int vmig_copy_dir(const char* src_dir, const char* dst_dir);
 
@@ -264,7 +316,7 @@ void vmig_host_free(void* p);
 
 /* ---- cancellation and progress ------------------------------------------------------------------
  * A control is a numeric id (cgo passes it in vmig_opts.ctl without any pointer rules).  It serves the entry points
- * that take vmig_opts: vmig_migrate_tree, vmig_restore_tree, vmig_snapshot_tree and vmig_migrate_buffer (a caller that
+ * that take vmig_opts: vmig_migrate_tree, vmig_restore_tree, vmig_snapshot_tree, vmig_scrub_store and vmig_migrate_buffer (a caller that
  * wants to cancel a copy or a move calls vmig_migrate_tree with the flags vmig_copy_dir / vmig_move_dir use).  One
  * control serves one call at a time: attaching it to a second concurrent call fails with VMIG_EINVAL.  The engine has
  * no deadline of its own; a deadline is the caller's timer calling vmig_ctl_cancel.

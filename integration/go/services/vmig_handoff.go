@@ -21,6 +21,7 @@ import (
 	"os"
 	"path/filepath"
 	"runtime"
+	"sort"
 	"strconv"
 	"strings"
 	"time"
@@ -111,6 +112,48 @@ func SnapshotVersionIncremental(ctrVersionName string) error {
 	baseData, baseTable := snapshotPaths(base)
 	return errors.WithMessagef(utils.SnapshotDirIncrementalVerified(upper, data, baseData, baseTable, table),
 		"snapshot of %s against %s failed", ctrVersionName, base)
+}
+
+// N1 -- ScrubReplicaSet checks every snapshot of the ReplicaSet against its block table in one pass that reads each
+// inode the versions share once.  The versions are the merges/<rs>/<rs>-<k> that hold diff/ (the rule of baseVersion;
+// a missing blocks.vmig is that version's VMIG_ETABLE).  It returns each version's verdict by name and the report,
+// merges/<rs>/scrub.txt, which lists every damaged path and block.
+func ScrubReplicaSet(rs string) (map[string]int, string, error) {
+	parent := filepath.Dir(versionDir(rs + "-0"))
+	entries, _ := os.ReadDir(parent)
+	type version struct {
+		k    int
+		name string
+	}
+	var found []version
+	for _, e := range entries {
+		k, err := strconv.Atoi(strings.TrimPrefix(e.Name(), rs+"-"))
+		if !strings.HasPrefix(e.Name(), rs+"-") || err != nil || k < 0 {
+			continue
+		}
+		if st, err := os.Stat(filepath.Join(parent, e.Name(), "diff")); err != nil || !st.IsDir() {
+			continue
+		}
+		found = append(found, version{k, e.Name()})
+	}
+	sort.Slice(found, func(i, j int) bool { return found[i].k < found[j].k })
+	report := filepath.Join(parent, "scrub.txt")
+	if len(found) == 0 {
+		return map[string]int{}, "", nil
+	}
+	dirs, tables := make([]string, len(found)), make([]string, len(found))
+	for i, v := range found {
+		dirs[i], tables[i] = snapshotPaths(v.name)
+	}
+	verdicts, err := utils.ScrubSnapshots(dirs, tables, report)
+	if err != nil {
+		return nil, "", errors.WithMessagef(err, "scrub of %s failed", rs)
+	}
+	out := make(map[string]int, len(found))
+	for i, v := range found {
+		out[v.name] = verdicts[i]
+	}
+	return out, report, nil
 }
 
 // N1 -- RollbackFromSnapshot fills newContainer's layer with version `target` of the ReplicaSet.  The new

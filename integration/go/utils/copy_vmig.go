@@ -123,6 +123,68 @@ func SnapshotDirIncrementalVerifiedContext(ctx context.Context, src, dest, baseD
 		})
 }
 
+// ScrubSnapshots checks every snapshot snapDirs[i] against its block table snapTables[i] in one pass that reads each
+// inode the snapshots share once (vmig_scrub_store), and writes every finding to report.  verdicts[i] is the VMIG_*
+// code a hash-only restore of that snapshot would return (VMIG_OK, VMIG_ECORRUPT, VMIG_ETABLE, VMIG_ENOTDIR); a
+// damaged snapshot is a verdict, not an error.  Nothing is written under any snapshot.
+func ScrubSnapshots(snapDirs, snapTables []string, report string) ([]int, error) {
+	return ScrubSnapshotsContext(context.Background(), snapDirs, snapTables, report)
+}
+
+// ScrubSnapshotsContext is ScrubSnapshots that stops when ctx is done (see CopyDirDiffContext); no report is written then.
+func ScrubSnapshotsContext(ctx context.Context, snapDirs, snapTables []string, report string) ([]int, error) {
+	n := len(snapDirs)
+	if n == 0 || len(snapTables) != n {
+		return nil, errors.Errorf("ScrubSnapshots: %d directories, %d tables", n, len(snapTables))
+	}
+	ptrSize := C.size_t(unsafe.Sizeof((*C.char)(nil)))
+	cdirs := (*[1 << 28]*C.char)(C.malloc(C.size_t(n) * ptrSize))[:n:n] // C memory: cgo forbids Go pointers to Go pointers
+	ctabs := (*[1 << 28]*C.char)(C.malloc(C.size_t(n) * ptrSize))[:n:n]
+	defer C.free(unsafe.Pointer(&cdirs[0]))
+	defer C.free(unsafe.Pointer(&ctabs[0]))
+	for i := 0; i < n; i++ {
+		cdirs[i], ctabs[i] = C.CString(snapDirs[i]), C.CString(snapTables[i])
+		defer C.free(unsafe.Pointer(cdirs[i]))
+		defer C.free(unsafe.Pointer(ctabs[i]))
+	}
+	var cr *C.char
+	if report != "" {
+		cr = C.CString(report)
+		defer C.free(unsafe.Pointer(cr))
+	}
+	verdicts := make([]C.int32_t, n)
+	var st C.vmig_stats
+	var ss C.vmig_scrub_stats
+	var o C.vmig_opts
+	var id C.uint32_t
+	if err := lockedCall("vmig_ctl_open", func() C.int { return C.vmig_ctl_open(&id) }); err != nil {
+		return nil, err
+	}
+	defer C.vmig_ctl_close(id)
+	stop := context.AfterFunc(ctx, func() { C.vmig_ctl_cancel(id) })
+	defer stop()
+	o.ctl = id
+	var rc C.int
+	err := lockedCall("vmig_scrub_store", func() C.int {
+		rc = C.vmig_scrub_store(C.uint32_t(n), &cdirs[0], &ctabs[0], cr, &verdicts[0], &o, &st, &ss)
+		return rc
+	})
+	if rc == C.VMIG_ECANCELED && ctx.Err() != nil {
+		return nil, fmt.Errorf("%w: %v", ctx.Err(), err)
+	}
+	if err != nil {
+		return nil, err
+	}
+	log.Infof("vmig: scrubbed %d snapshots, %d damaged: %d bytes read for %d referenced, %d paths and %d blocks damaged, %d files unreadable",
+		uint64(ss.versions), uint64(ss.versions_damaged), uint64(ss.bytes_unique), uint64(ss.bytes_referenced),
+		uint64(ss.files_damaged), uint64(ss.blocks_damaged), uint64(ss.files_unreadable))
+	out := make([]int, n)
+	for i, v := range verdicts {
+		out[i] = int(v)
+	}
+	return out, nil
+}
+
 func copyDirDiff(ctx context.Context, src, dest, priorTable, outTable string, flags C.uint32_t) error {
 	return runDiff(ctx, "vmig_migrate_tree", src, dest, priorTable, outTable, flags,
 		func(cs, cd, cp, co *C.char, o *C.vmig_opts, st *C.vmig_stats, _ *C.vmig_snapshot_stats) C.int {

@@ -214,9 +214,7 @@ public:
                 std::lock_guard<std::mutex> lk(link_mu);
                 if (linked_inos.count(bf.ino)) { close(bfd); continue; }
                 const std::string bp = pjoin(base_root, bf.rel);
-                bool was_dir = false;
-                rc = unlink_if_exists(p, &was_dir);
-                if (!rc && was_dir) rc = fail(VMIG_EIO, "%s: a directory is in the way of a regular file", p.c_str());
+                rc = clear_path(p, "a regular file");
                 if (!rc && linkat(AT_FDCWD, bp.c_str(), AT_FDCWD, p.c_str(), 0) != 0) rc = fail(VMIG_EIO, "link %s -> %s: %s", p.c_str(), bp.c_str(), errno_str(errno).c_str());
                 struct stat ls;
                 if (!rc && (lstat(p.c_str(), &ls) != 0 || ls.st_ino != bs.st_ino)) {      // the base path was replaced after the fstat
@@ -308,12 +306,16 @@ public:
                 const int dflag = direct && corrupt_block < 0 ? O_DIRECT : 0;
                 if (s.inplace) {
                     fd = open(p.c_str(), O_WRONLY | O_CLOEXEC | O_NOFOLLOW | dflag);
+                    // an ordinary user's own read-only file (tar would replace it): made writable for the patch; its mode no
+                    // longer matches the source's, so block_done puts the source's back whether a block was written or not
+                    struct stat ws;
+                    if (fd < 0 && errno == EACCES && lstat(p.c_str(), &ws) == 0 && S_ISREG(ws.st_mode) &&
+                        chmod(p.c_str(), (ws.st_mode & 07777) | S_IWUSR) == 0)
+                        fd = open(p.c_str(), O_WRONLY | O_CLOEXEC | O_NOFOLLOW | dflag);
                     if (fd < 0 && dflag && errno == EINVAL) fd = open(p.c_str(), O_WRONLY | O_CLOEXEC | O_NOFOLLOW); else s.d_direct = dflag != 0 && fd >= 0;
                 } else {
-                    bool was_dir = false;
-                    int rc = unlink_if_exists(p, &was_dir);     // tar replaces what is there
+                    int rc = clear_path(p, "a regular file");     // tar replaces what is there
                     if (rc) return rc;
-                    if (was_dir) return fail(VMIG_EIO, "%s: a directory is in the way of a regular file", p.c_str());
                     fd = open(p.c_str(), O_WRONLY | O_CREAT | O_EXCL | O_CLOEXEC | O_NOFOLLOW | dflag, 0600);
                     if (fd < 0 && dflag && errno == EINVAL) fd = open(p.c_str(), O_WRONLY | O_CREAT | O_CLOEXEC | O_NOFOLLOW, 0600); else s.d_direct = dflag != 0 && fd >= 0;
                 }
@@ -822,9 +824,7 @@ int migrate_tree_body(CallScope& call, const char* src_dir, const char* dst_dir,
             if (e.hardlink_of >= 0 || e.n_blocks) continue;
             if (steps++ % kMetaCheckEvery == 0 && cancel->load()) return fail(VMIG_ECANCELED, "before creating %s", e.rel.c_str());
             const std::string p = pjoin(dst, e.rel);
-            bool was_dir = false;
-            rc = unlink_if_exists(p, &was_dir); if (rc) return rc;
-            if (was_dir) return fail(VMIG_EIO, "%s: a directory is in the way of a regular file", p.c_str());
+            rc = clear_path(p, "an empty regular file"); if (rc) return rc;
             int fd = open(p.c_str(), O_WRONLY | O_CREAT | O_EXCL | O_CLOEXEC | O_NOFOLLOW, 0600);
             if (fd < 0) return fail(VMIG_EIO, "create %s: %s", p.c_str(), errno_str(errno).c_str());
             rc = apply_file_meta(fd, p, e, io.pol);

@@ -257,15 +257,18 @@ static inline void fill_times(const Entry& e, const MetaPolicy& pol, struct time
     if (!pol.mtime_ns) ts[1].tv_nsec = 0;   // tar's gnu format stores whole seconds
 }
 
-int unlink_if_exists(const std::string& path, bool* was_dir)
+int clear_path(const std::string& path, const char* what)
 {
     struct stat st;
-    if (was_dir) *was_dir = false;
     if (lstat(path.c_str(), &st) != 0) {
         if (errno == ENOENT) return VMIG_OK;
         return fail(VMIG_EIO, "lstat %s: %s", path.c_str(), errno_str(errno).c_str());
     }
-    if (S_ISDIR(st.st_mode)) { if (was_dir) *was_dir = true; return VMIG_OK; }
+    if (S_ISDIR(st.st_mode)) {
+        if (rmdir(path.c_str()) == 0 || errno == ENOENT) return VMIG_OK;
+        if (errno == ENOTEMPTY || errno == EEXIST) return fail(VMIG_EIO, "%s: a non-empty directory is in the way of %s", path.c_str(), what);
+        return fail(VMIG_EIO, "rmdir %s (in the way of %s): %s", path.c_str(), what, errno_str(errno).c_str());
+    }
     if (unlink(path.c_str()) != 0 && errno != ENOENT)
         return fail(VMIG_EIO, "unlink %s: %s", path.c_str(), errno_str(errno).c_str());
     return VMIG_OK;
@@ -394,10 +397,8 @@ int replay_metadata(const std::string& dst_root, const Manifest& m, const MetaPo
     for (const auto& e : m.symlinks) {
         if (int rc = stop(e.rel)) return rc;
         const std::string p = join(dst_root, e.rel);
-        bool was_dir = false;
-        int rc = unlink_if_exists(p, &was_dir);
+        int rc = clear_path(p, "a symlink");
         if (rc) return rc;
-        if (was_dir && rmdir(p.c_str()) != 0) return fail(VMIG_EIO, "rmdir %s (symlink over directory): %s", p.c_str(), errno_str(errno).c_str());
         if (symlink(e.target.c_str(), p.c_str()) != 0) return fail(VMIG_EIO, "symlink %s: %s", p.c_str(), errno_str(errno).c_str());
         if (!pol.no_metadata) {
             if (pol.is_root && lchown(p.c_str(), e.uid, e.gid) != 0) return fail(VMIG_EIO, "lchown %s: %s", p.c_str(), errno_str(errno).c_str());
@@ -409,10 +410,8 @@ int replay_metadata(const std::string& dst_root, const Manifest& m, const MetaPo
     for (const auto& e : m.specials) {
         if (int rc = stop(e.rel)) return rc;
         const std::string p = join(dst_root, e.rel);
-        bool was_dir = false;
-        int rc = unlink_if_exists(p, &was_dir);
+        int rc = clear_path(p, "a special file");
         if (rc) return rc;
-        if (was_dir && rmdir(p.c_str()) != 0) return fail(VMIG_EIO, "rmdir %s: %s", p.c_str(), errno_str(errno).c_str());
         if (mknod(p.c_str(), (e.mode & S_IFMT) | 0600, e.rdev) != 0) return fail(VMIG_EIO, "mknod %s: %s", p.c_str(), errno_str(errno).c_str());
         rc = apply_file_meta(-1, p, e, pol);
         if (rc) return rc;
@@ -423,10 +422,8 @@ int replay_metadata(const std::string& dst_root, const Manifest& m, const MetaPo
         if (int rc = stop(e.rel)) return rc;
         const std::string p = join(dst_root, e.rel);
         const std::string prim = join(dst_root, m.files[(size_t)e.hardlink_of].rel);
-        bool was_dir = false;
-        int rc = unlink_if_exists(p, &was_dir);
+        int rc = clear_path(p, "a hard link");
         if (rc) return rc;
-        if (was_dir) return fail(VMIG_EIO, "%s: directory in the way of a hard link", p.c_str());
         if (link(prim.c_str(), p.c_str()) != 0) return fail(VMIG_EIO, "link %s -> %s: %s", p.c_str(), prim.c_str(), errno_str(errno).c_str());
         if (n_hardlinks) (*n_hardlinks)++;
     }

@@ -84,8 +84,10 @@ int remove_source(const std::string& src_root, const Manifest& m);
 // handled by descriptor, symlinks are never followed.  dry_run only counts them (the verify pass uses that).
 int prune_extras(const std::string& dst_root, const Manifest& m, bool dry_run, uint64_t* n_extras,
                  const std::atomic<int>* cancel = nullptr);
-// Remove whatever non-directory sits at path (tar replaces existing entries).  ENOENT is fine.
-int unlink_if_exists(const std::string& path, bool* was_dir);
+// Remove whatever sits at path so that `what` (named in the error) can be created there: a non-directory or an EMPTY
+// directory goes, as GNU tar replaces them; a non-empty directory is VMIG_EIO, as tar fails with "Cannot open: File
+// exists".  ENOENT is fine.  Every non-directory the engine creates goes through this.
+int clear_path(const std::string& path, const char* what);
 // Copy bytes [off, off + len) of in_fd to the same offsets of out_fd (a snapshot file's unchanged blocks, taken from
 // the base snapshot's file).  copy_file_range, which may share extents on filesystems that reflink; pread/pwrite where
 // the kernel or filesystem refuses it (ENOSYS, EXDEV, EINVAL, EOPNOTSUPP) or rw_only is set.  out_direct: out_fd was

@@ -10,6 +10,7 @@
 #include "vmig_cufile.h"
 #include "vmig_reuse.h"
 #include "vmig_scrub.h"
+#include "vmig_plan.h"
 
 #include <fcntl.h>
 #include <unistd.h>
@@ -35,8 +36,6 @@ void vmig::CallCtl::cancel()
 }
 
 namespace {
-
-inline std::string pjoin(const std::string& a, const std::string& b) { return b == "." ? a : a + "/" + b; }
 
 // ---------------------------------------------------------------------------------------------
 // controls (vmig_ctl_*) and the calls in flight (vmig_shutdown cancels them and waits for them)
@@ -114,28 +113,26 @@ struct LatchLink {
 // file-backed BlockIO
 class FileIO : public BlockIO {
 public:
+    // the call's mutable state of one file; what was decided about it before the data pass is in plan->files
     struct FS {
         std::atomic<int> sfd{-1}, dfd{-1};
         std::atomic<uint32_t> reads_left{0}, blocks_left{0};
-        bool inplace = false;            // diff path: destination file is the prior version, patched in place
-        uint64_t dst_old_size = 0;
         uint64_t id_ino = 0; int64_t id_ctime_ns = 0;   // identity of the file the table will speak for (vmig_table.h)
         bool s_direct = false, d_direct = false;         // this file's descriptor was opened with O_DIRECT
         std::atomic<void*> s_cfh{nullptr}, d_cfh{nullptr};   // cuFile handles of sfd / dfd (VMIG_F_CUFILE)
         std::atomic<bool> wrote{false};                  // at least one block of the file was written in this call
-        const TableFile* base_rec = nullptr;             // vmig_snapshot_tree: the base file still is this record
         std::atomic<bool> reused{false};                 // vmig_snapshot_tree: a changed block was found elsewhere in the base
-        bool solo = true;                                // no other source path is a hard link to this file
+        void identify(const struct stat& st) { id_ino = (uint64_t)st.st_ino; id_ctime_ns = ctime_ns(st); }
     };
     std::string src_root, dst_root;
     int src_root_fd = -1;                // source files are opened beneath this descriptor, never by absolute path
     const Manifest* m = nullptr;
+    const TreePlan* plan = nullptr;
     MetaPolicy pol;
     bool hash_only = false;
     bool direct = false;                 // VMIG_F_DIRECT_IO: O_DIRECT into / out of the pinned rings
     bool cufile = false;                 // VMIG_F_CUFILE: file <-> HBM slot through libcufile (GPUDirect Storage)
     std::atomic<uint64_t> n_direct{0};   // descriptors that really were opened O_DIRECT
-    static constexpr uint32_t kSector = 4096;
     uint32_t slot_align() override { return direct || cufile ? kSector : 512; }
     bool device_reads() override { return cufile; }
     bool device_writes() override { return cufile && !hash_only; }
@@ -146,6 +143,16 @@ public:
     }
     std::unique_ptr<FS[]> fs;
     std::mutex stripes[64];
+    // one FS per manifest file; a file's blocks count down to the close of its source and to its finalization
+    void init_files(const Manifest& man, const TreePlan& p) {
+        m = &man; plan = &p;
+        fs.reset(new FS[man.files.size() ? man.files.size() : 1]);
+        for (uint32_t f = 0; f < man.files.size(); f++) {
+            const Entry& e = man.files[f];
+            if (e.hardlink_of >= 0 || e.n_blocks == 0) continue;
+            fs[f].reads_left.store((uint32_t)e.n_blocks); fs[f].blocks_left.store((uint32_t)e.n_blocks);
+        }
+    }
 
     // vmig_snapshot_tree: the base snapshot whose files supply the blocks K1 found unchanged, at the same path and offset
     // or anywhere else in the base (bidx: every block of every trusted base file, by hash and length)
@@ -159,7 +166,7 @@ public:
     std::atomic<uint64_t> n_linked{0}, b_linked{0}, n_backfilled{0}, b_backfilled{0};
     const std::atomic<int>* cancel = nullptr;              // the call's cancel flag: checked per backfill chunk
     static constexpr size_t kLinkTries = 16;               // base files of equal content tried as a link target, per file
-    bool done_on_writer(const BlockRef& b) override { return fs[b.file].base_rec != nullptr || fs[b.file].reused.load(); }
+    bool done_on_writer(const BlockRef& b) override { return plan->files[b.file].base_rec != nullptr || fs[b.file].reused.load(); }
     bool reusable(const BlockRef& b, uint64_t hash) override {
         if (bidx.empty() || !bidx.contains(hash, b.len)) return false;
         skipped[b.table_idx] = 1;
@@ -175,7 +182,7 @@ public:
         const int bfd = open(bp.c_str(), O_RDONLY | O_NOFOLLOW | O_CLOEXEC);
         bool same = bfd >= 0 && fstat(bfd, bs) == 0 && S_ISREG(bs->st_mode) && (uint64_t)bs->st_ino == bf.ino;
         if (same) {
-            const int64_t ct = (int64_t)bs->st_ctim.tv_sec * 1000000000ll + bs->st_ctim.tv_nsec;
+            const int64_t ct = ctime_ns(*bs);
             std::lock_guard<std::mutex> lk(link_mu);     // a link in flight holds it from before linkat until linked_inos has its ctime
             auto it = linked_inos.find(bf.ino);
             same = ct == bf.ctime_ns || (it != linked_inos.end() && it->second == ct);
@@ -198,10 +205,11 @@ public:
         bool any_skipped = false;
         for (uint64_t r = 0; r < e.n_blocks && !any_skipped; r++) any_skipped = skipped[e.first_block + r] != 0;
         if (!any_skipped) return VMIG_OK;
-        const int same = s.base_rec ? (int)(s.base_rec - bidx.t->files.data()) : -1;
+        const FilePlan& fp = plan->files[f];
+        const int same = fp.base_rec ? (int)(fp.base_rec - bidx.t->files.data()) : -1;
         const uint64_t* h = hashes + e.first_block;
         const std::string p = pjoin(dst_root, e.rel);
-        if (!s.wrote.load() && s.solo) {
+        if (!s.wrote.load() && fp.solo) {
             std::vector<uint32_t> cands;
             link_candidates(bidx, same, e.size, block_bytes, h, &cands, kLinkTries);
             for (uint32_t g : cands) {
@@ -223,7 +231,7 @@ public:
                 }
                 close(bfd);
                 if (rc) return rc;
-                linked_inos[bf.ino] = (int64_t)ls.st_ctim.tv_sec * 1000000000ll + ls.st_ctim.tv_nsec;
+                linked_inos[bf.ino] = ctime_ns(ls);
                 linked_files.push_back(f);
                 n_linked++; b_linked += e.size;
                 *linked = true;
@@ -256,10 +264,16 @@ public:
 
     // libcufile refuses descriptors whose open flags include O_NOFOLLOW / O_NONBLOCK ("unsupported file open flags"),
     // which is exactly how the safe opens below are made, and F_SETFL cannot clear O_NOFOLLOW.  The descriptor already
-    // refers to the checked regular file, so it is re-opened through /proc/self/fd with plain flags.
-    static int reopen_plain(int fd, int flags) {
-        char p[64]; snprintf(p, sizeof p, "/proc/self/fd/%d", fd);
-        return open(p, flags | O_CLOEXEC);
+    // refers to the checked regular file, so it is re-opened through /proc/self/fd with plain flags and registered.
+    // *fd is replaced by the new descriptor, or closed on failure.
+    static int attach_cufile(int* fd, int flags, const char* what, void** handle) {
+        char p[64]; snprintf(p, sizeof p, "/proc/self/fd/%d", *fd);
+        const int nfd = open(p, flags | O_CLOEXEC);
+        if (nfd < 0) { const int e = errno; close(*fd); return fail(VMIG_EIO, "reopen %s for cuFile: %s", what, errno_str(e).c_str()); }
+        close(*fd); *fd = nfd;
+        const int rc = cufile_handle_open(nfd, handle);
+        if (rc) close(nfd);
+        return rc;
     }
     int open_src(uint32_t f, int* out) {
         FS& s = fs[f];
@@ -279,15 +293,12 @@ public:
                     close(fd);
                     return fail(VMIG_ESRCCHANGED, "%s is not a regular file any more", m->files[f].rel.c_str());
                 }
-                if (hash_only && st.st_nlink == 1) { s.id_ino = (uint64_t)st.st_ino; s.id_ctime_ns = (int64_t)st.st_ctim.tv_sec * 1000000000ll + st.st_ctim.tv_nsec; }
+                if (hash_only && st.st_nlink == 1) s.identify(st);
                 if (s.s_direct) n_direct++;
                 if (cufile) {
-                    const int nfd = reopen_plain(fd, O_RDONLY | (s.s_direct ? O_DIRECT : 0));
-                    if (nfd < 0) { const int e = errno; close(fd); return fail(VMIG_EIO, "reopen %s for cuFile: %s", m->files[f].rel.c_str(), errno_str(e).c_str()); }
-                    close(fd); fd = nfd;
                     void* h = nullptr;
-                    rc = cufile_handle_open(fd, &h);
-                    if (rc) { close(fd); return rc; }
+                    rc = attach_cufile(&fd, O_RDONLY | (s.s_direct ? O_DIRECT : 0), m->files[f].rel.c_str(), &h);
+                    if (rc) return rc;
                     s.s_cfh.store(h, std::memory_order_release);
                 }
                 s.sfd.store(fd, std::memory_order_release);
@@ -304,7 +315,7 @@ public:
             if (fd < 0) {
                 const std::string p = pjoin(dst_root, m->files[f].rel);
                 const int dflag = direct && corrupt_block < 0 ? O_DIRECT : 0;
-                if (s.inplace) {
+                if (plan->files[f].prior_rec) {
                     fd = open(p.c_str(), O_WRONLY | O_CLOEXEC | O_NOFOLLOW | dflag);
                     // an ordinary user's own read-only file (tar would replace it): made writable for the patch; its mode no
                     // longer matches the source's, so block_done puts the source's back whether a block was written or not
@@ -322,12 +333,9 @@ public:
                 if (fd < 0) return fail(VMIG_EIO, "open %s for writing: %s", p.c_str(), errno_str(errno).c_str());
                 if (s.d_direct) n_direct++;
                 if (cufile && !hash_only) {
-                    const int nfd = reopen_plain(fd, O_WRONLY | (s.d_direct ? O_DIRECT : 0));
-                    if (nfd < 0) { const int e = errno; close(fd); return fail(VMIG_EIO, "reopen %s for cuFile: %s", p.c_str(), errno_str(e).c_str()); }
-                    close(fd); fd = nfd;
                     void* h = nullptr;
-                    int rc = cufile_handle_open(fd, &h);
-                    if (rc) { close(fd); return rc; }
+                    const int rc = attach_cufile(&fd, O_WRONLY | (s.d_direct ? O_DIRECT : 0), p.c_str(), &h);
+                    if (rc) return rc;
                     s.d_cfh.store(h, std::memory_order_release);
                 }
                 s.dfd.store(fd, std::memory_order_release);
@@ -339,19 +347,17 @@ public:
         int fd; int rc = open_src(b.file, &fd);
         if (rc) return rc;
         FS& s = fs[b.file];
-        // O_DIRECT: buffer, offset and length in whole sectors (the slot layout leaves the room; the device DMAs straight
-        // into the pinned ring); the file's last block is short, the read past EOF simply returns fewer bytes
-        const size_t want = s.s_direct ? (size_t)align_up(b.len, kSector) : b.len;
-        size_t got = 0;
-        while (got < b.len) {
-            const size_t pos = s.s_direct ? (got & ~(size_t)(kSector - 1)) : got;      // after a short direct read: back to a sector boundary
-            ssize_t r = pread(fd, dst + pos, want - pos, (off_t)(b.file_off + pos));
-            if (r < 0) { if (errno == EINTR) continue; return fail(VMIG_EIO, "pread %s: %s", m->files[b.file].rel.c_str(), errno_str(errno).c_str()); }
-            if (r == 0 || pos + (size_t)r <= got) return fail(VMIG_ESRCCHANGED, "%s shrank while being migrated (wanted %u bytes at %llu, got %zu)", m->files[b.file].rel.c_str(), b.len, (unsigned long long)b.file_off, got);
-            got = pos + (size_t)r;
-        }
+        // O_DIRECT: the device DMAs straight into the pinned ring; the file's last block is short, the read past EOF simply
+        // returns fewer bytes
+        size_t got;
+        rc = xfer_block(s.s_direct, true, b.len, &got, [&](size_t pos, size_t n) { return pread(fd, dst + pos, n, (off_t)(b.file_off + pos)); });
+        if (rc < 0) return fail(VMIG_EIO, "pread %s: %s", m->files[b.file].rel.c_str(), errno_str(errno).c_str());
+        if (rc) return shrank(b, got);
         if (s.reads_left.fetch_sub(1) == 1) { close_src(s, fd); }
         return VMIG_OK;
+    }
+    int shrank(const BlockRef& b, size_t got) {
+        return fail(VMIG_ESRCCHANGED, "%s shrank while being migrated (wanted %u bytes at %llu, got %zu)", m->files[b.file].rel.c_str(), b.len, (unsigned long long)b.file_off, got);
     }
     void close_src(FS& s, int fd) {
         void* h = s.s_cfh.exchange(nullptr);
@@ -364,15 +370,10 @@ public:
         if (rc) return rc;
         FS& s = fs[b.file];
         void* h = s.s_cfh.load(std::memory_order_acquire);
-        const size_t want = s.s_direct ? (size_t)align_up(b.len, kSector) : b.len;
-        size_t got = 0;
-        while (got < b.len) {
-            const size_t pos = s.s_direct ? (got & ~(size_t)(kSector - 1)) : got;
-            const ssize_t r = cufile_read(h, d_base, want - pos, (off_t)(b.file_off + pos), (off_t)(d_off + pos));
-            if (r < 0) return (int)r;
-            if (r == 0 || pos + (size_t)r <= got) return fail(VMIG_ESRCCHANGED, "%s shrank while being migrated (wanted %u bytes at %llu, got %zu)", m->files[b.file].rel.c_str(), b.len, (unsigned long long)b.file_off, got);
-            got = pos + (size_t)r;
-        }
+        size_t got;
+        rc = xfer_block(s.s_direct, false, b.len, &got, [&](size_t pos, size_t n) { return cufile_read(h, d_base, n, (off_t)(b.file_off + pos), (off_t)(d_off + pos)); });
+        if (rc < 0) return rc;
+        if (rc) return shrank(b, got);
         if (s.reads_left.fetch_sub(1) == 1) close_src(s, fd);
         return VMIG_OK;
     }
@@ -383,15 +384,10 @@ public:
         FS& s = fs[b.file];
         s.wrote.store(true, std::memory_order_relaxed);
         void* h = s.d_cfh.load(std::memory_order_acquire);
-        const size_t want = s.d_direct ? (size_t)align_up(b.len, kSector) : b.len;
-        size_t put = 0;
-        while (put < b.len) {
-            const size_t pos = s.d_direct ? (put & ~(size_t)(kSector - 1)) : put;
-            const ssize_t w = cufile_write(h, d_base, want - pos, (off_t)(b.file_off + pos), (off_t)(d_off + pos));
-            if (w < 0) return (int)w;
-            if (w == 0 || pos + (size_t)w <= put) return fail(VMIG_EIO, "cuFileWrite %s: wrote 0 bytes", m->files[b.file].rel.c_str());
-            put = pos + (size_t)w;
-        }
+        size_t put;
+        rc = xfer_block(s.d_direct, false, b.len, &put, [&](size_t pos, size_t n) { return cufile_write(h, d_base, n, (off_t)(b.file_off + pos), (off_t)(d_off + pos)); });
+        if (rc < 0) return rc;
+        if (rc) return fail(VMIG_EIO, "cuFileWrite %s: wrote 0 bytes", m->files[b.file].rel.c_str());
         return VMIG_OK;
     }
     int write_block(const BlockRef& b, const uint8_t* src) override {
@@ -408,25 +404,20 @@ public:
         }
         // O_DIRECT: whole sectors out of the pinned ring; a short last block is written padded (whatever follows it in the
         // slot) and block_done() cuts the file back to its size
-        const bool dio = fs[b.file].d_direct;
-        const size_t want = dio ? (size_t)align_up(b.len, kSector) : b.len;
-        size_t put = 0;
-        while (put < b.len) {
-            const size_t pos = dio ? (put & ~(size_t)(kSector - 1)) : put;
-            ssize_t w = pwrite(fd, src + pos, want - pos, (off_t)(b.file_off + pos));
-            if (w < 0) { if (errno == EINTR) continue; return fail(VMIG_EIO, "pwrite %s: %s", m->files[b.file].rel.c_str(), errno_str(errno).c_str()); }
-            if (w == 0 || pos + (size_t)w <= put) return fail(VMIG_EIO, "pwrite %s: wrote 0 bytes", m->files[b.file].rel.c_str());
-            put = pos + (size_t)w;
-        }
+        size_t put;
+        rc = xfer_block(fs[b.file].d_direct, true, b.len, &put, [&](size_t pos, size_t n) { return pwrite(fd, src + pos, n, (off_t)(b.file_off + pos)); });
+        if (rc < 0) return fail(VMIG_EIO, "pwrite %s: %s", m->files[b.file].rel.c_str(), errno_str(errno).c_str());
+        if (rc) return fail(VMIG_EIO, "pwrite %s: wrote 0 bytes", m->files[b.file].rel.c_str());
         return VMIG_OK;
     }
     int block_done(const BlockRef& b, bool written) override {
         FS& s = fs[b.file];
-        if (!written && s.base_rec) skipped[b.table_idx] = 1;          // (a reused block was marked by reusable())
+        const FilePlan& fp = plan->files[b.file];
+        if (!written && fp.base_rec) skipped[b.table_idx] = 1;          // (a reused block was marked by reusable())
         if (s.blocks_left.fetch_sub(1) != 1) return VMIG_OK;
         if (hash_only) return VMIG_OK;
         const Entry& e = m->files[b.file];
-        if (s.base_rec || s.reused.load()) {
+        if (fp.base_rec || s.reused.load()) {
             bool linked = false;
             int rc = finish_from_base(b.file, &linked);
             if (rc || linked) return rc;
@@ -434,15 +425,16 @@ public:
         int fd; int rc = open_dst(b.file, &fd);      // also covers "every block was skipped"
         if (rc) return rc;
         const std::string p = pjoin(dst_root, e.rel);
-        if (((s.inplace && s.dst_old_size != e.size) || (s.d_direct && (e.size & (kSector - 1)))) && ftruncate(fd, (off_t)e.size) != 0) {
+        const bool inplace = fp.prior_rec != nullptr;
+        if (((inplace && fp.prior_rec->size != e.size) || (s.d_direct && (e.size & (kSector - 1)))) && ftruncate(fd, (off_t)e.size) != 0) {
             close(fd); return fail(VMIG_EIO, "ftruncate %s: %s", p.c_str(), errno_str(errno).c_str());
         }
         // a patched-in-place file none of whose blocks changed and whose metadata is already right is not touched at all:
         // its ctime -- by which the block table knows it -- stays what the table recorded
-        const bool untouched = s.inplace && !s.wrote.load() && s.dst_old_size == e.size && file_meta_matches(fd, e, pol);
+        const bool untouched = inplace && !s.wrote.load() && fp.prior_rec->size == e.size && file_meta_matches(fd, e, pol);
         rc = untouched ? VMIG_OK : apply_file_meta(fd, p, e, pol);
         struct stat ids;                             // nothing touches the file after this point: its ctime is final
-        if (!rc && fstat(fd, &ids) == 0) { s.id_ino = (uint64_t)ids.st_ino; s.id_ctime_ns = (int64_t)ids.st_ctim.tv_sec * 1000000000ll + ids.st_ctim.tv_nsec; }
+        if (!rc && fstat(fd, &ids) == 0) s.identify(ids);
         { void* h = s.d_cfh.exchange(nullptr); if (h) cufile_handle_close(h); }
         if (close(fd) != 0 && !rc) rc = fail(VMIG_EIO, "close %s: %s", p.c_str(), errno_str(errno).c_str());
         s.dfd.store(-1);
@@ -573,25 +565,25 @@ int run_blocks(const std::vector<BlockRef>& blocks, BlockIO* io, bool has_prior,
 
 // Restore, plan time: the walked tree must be the one the snapshot's table describes -- the same regular-file paths
 // (hard-linked ones included) with the same sizes.  ino/ctime_ns are not compared: a snapshot copied elsewhere keeps
-// its bytes, not its inodes.  Both lists are sorted bytewise, so one merge finds the first difference.  On success
-// expect[] holds the table's hashes in the manifest's block order.
+// its bytes, not its inodes.  The first difference in merge order fails the call.  On success expect[] holds the
+// table's hashes in the manifest's block order.
 int match_table(const Manifest& man, const BlockTable& t, std::vector<uint64_t>* expect)
 {
-    size_t i = 0, j = 0;
-    while (i < man.files.size() || j < t.files.size()) {
-        if (j == t.files.size() || (i < man.files.size() && man.files[i].rel < t.files[j].rel))
-            return fail(VMIG_ECORRUPT, "%s is in the snapshot but not in its block table (extra)", man.files[i].rel.c_str());
-        if (i == man.files.size() || t.files[j].rel < man.files[i].rel)
-            return fail(VMIG_ECORRUPT, "%s is in the block table but not in the snapshot (missing)", t.files[j].rel.c_str());
-        if (man.files[i].size != t.files[j].size)
-            return fail(VMIG_ECORRUPT, "%s is %llu bytes in the snapshot, %llu in its block table (resized)", man.files[i].rel.c_str(),
-                        (unsigned long long)man.files[i].size, (unsigned long long)t.files[j].size);
-        i++; j++;
+    std::vector<int64_t> tab_of;
+    std::vector<ScrubFinding> diff;
+    if (scrub_merge_table(0, man, t, &tab_of, &diff)) {
+        const ScrubFinding& d = diff[0];
+        const char* p = d.path.c_str();
+        if (d.kind == kScrubExtra) return fail(VMIG_ECORRUPT, "%s is in the snapshot but not in its block table (extra)", p);
+        if (d.kind == kScrubMissing) return fail(VMIG_ECORRUPT, "%s is in the block table but not in the snapshot (missing)", p);
+        const Entry& e = *std::lower_bound(man.files.begin(), man.files.end(), d.path, [](const Entry& a, const std::string& rel) { return a.rel < rel; });
+        return fail(VMIG_ECORRUPT, "%s is %llu bytes in the snapshot, %llu in its block table (resized)", p, (unsigned long long)e.size,
+                    (unsigned long long)t.files[t.index.at(d.path)].size);
     }
     expect->assign(man.n_blocks, 0);
     for (size_t f = 0; f < man.files.size(); f++) {
         const Entry& e = man.files[f];
-        std::copy_n(t.hashes.begin() + (ptrdiff_t)t.files[f].first_block, e.n_blocks, expect->begin() + (ptrdiff_t)e.first_block);
+        std::copy_n(t.hashes.begin() + (ptrdiff_t)t.files[(size_t)tab_of[f]].first_block, e.n_blocks, expect->begin() + (ptrdiff_t)e.first_block);
     }
     return VMIG_OK;
 }
@@ -605,43 +597,163 @@ vmig_opts norm_opts(const vmig_opts* in) {
     return o;
 }
 
+int load_table(const char* path, const char* what, uint32_t block_bytes, BlockTable* t)
+{
+    const int rc = table_load(path, t);
+    if (rc) return rc;
+    if (t->block_bytes != block_bytes) return fail(VMIG_ETABLE, "%s table block size %u != %u", what, t->block_bytes, block_bytes);
+    return VMIG_OK;
+}
+
+int check_block_bytes(const vmig_opts& o)
+{
+    if (o.block_bytes & 4095u) return fail(VMIG_EINVAL, "block_bytes %u is not a multiple of 4096", o.block_bytes);
+    if (o.block_bytes > pipe_slot_bytes()) return fail(VMIG_EINVAL, "block_bytes %u exceeds the staging slot (%u)", o.block_bytes, pipe_slot_bytes());
+    return VMIG_OK;
+}
+
 struct SnapshotArgs {
     const char* base_dir;              // both NULL: a full snapshot
     const char* base_table;
     vmig_snapshot_stats* out;          // nullable
 };
 
+// After the data pass: hard-linked paths take their primary's hashes, empty regular files are created, then the rest of
+// the tree's metadata is replayed (vmig_tree.h replay_metadata).
+int meta_pass(CallScope& call, FileIO& io, const std::vector<uint64_t>& expect, std::vector<uint64_t>* hashes, vmig_stats* st)
+{
+    const Manifest& man = *io.m;
+    const std::atomic<int>* cancel = call.cancel();
+    std::vector<uint64_t>& h = *hashes;
+    if (cancel->load()) return fail(VMIG_ECANCELED, "after the data pass, before any metadata step");
+    for (auto& e : man.files)                      // hard-linked paths share their primary's hashes
+        if (e.hardlink_of >= 0) {
+            const Entry& p = man.files[(size_t)e.hardlink_of];
+            for (uint64_t r = 0; r < e.n_blocks; r++) {
+                h[e.first_block + r] = h[p.first_block + r];
+                // restore: the table hashed this path on its own; it must describe the bytes its primary now holds
+                // (checked before replay_metadata creates any link)
+                if (!expect.empty() && expect[e.first_block + r] != h[e.first_block + r])
+                    return fail(VMIG_ECORRUPT, "%s block %llu (a hard link to %s) hashes %016llx, its block table says %016llx",
+                                e.rel.c_str(), (unsigned long long)r, p.rel.c_str(), (unsigned long long)h[e.first_block + r],
+                                (unsigned long long)expect[e.first_block + r]);
+            }
+        }
+    if (io.hash_only) return VMIG_OK;
+    size_t steps = 0;
+    for (auto& e : man.files) {                    // empty regular files carry no blocks
+        if (e.hardlink_of >= 0 || e.n_blocks) continue;
+        if (steps++ % kMetaCheckEvery == 0 && cancel->load()) return fail(VMIG_ECANCELED, "before creating %s", e.rel.c_str());
+        const std::string p = pjoin(io.dst_root, e.rel);
+        int rc = clear_path(p, "an empty regular file"); if (rc) return rc;
+        int fd = open(p.c_str(), O_WRONLY | O_CREAT | O_EXCL | O_CLOEXEC | O_NOFOLLOW, 0600);
+        if (fd < 0) return fail(VMIG_EIO, "create %s: %s", p.c_str(), errno_str(errno).c_str());
+        rc = apply_file_meta(fd, p, e, io.pol);
+        struct stat ids;
+        if (!rc && fstat(fd, &ids) == 0) io.fs[&e - &man.files[0]].identify(ids);
+        close(fd);
+        if (rc) return rc;
+    }
+    return replay_metadata(io.dst_root, man, io.pol, &st->symlinks, &st->hardlinks, &st->specials, cancel);
+}
+
+// VMIG_F_VERIFY: read the destination back through the same GPU path (hash only) and compare block tables
+int verify_pass(CallScope& call, const vmig_opts& o, const FileIO& io, const std::vector<uint64_t>& hashes, vmig_stats* st)
+{
+    const Manifest& man = *io.m;
+    FileIO vio;
+    vio.src_root = io.dst_root; vio.dst_root = io.dst_root; vio.pol = io.pol; vio.hash_only = true;
+    vio.direct = io.direct;          // O_DIRECT re-read: what is verified is what the device holds, not the page cache
+    vio.cufile = io.cufile;
+    TreePlan blank;                  // nothing patched in place or taken from a base: every block is read back
+    blank.files.resize(man.files.size());
+    vio.init_files(man, blank);
+    int rc = vio.open_root(); if (rc) return rc;
+    std::vector<BlockRef> vblocks = io.plan->blocks;
+    for (auto& b : vblocks) { b.prior_hash = 0; b.prior_valid = 0; }
+    std::vector<uint64_t> vh(man.n_blocks, 0);
+    vmig_stats vst; memset(&vst, 0, sizeof vst);
+    rc = run_blocks(vblocks, &vio, false, true, o, vh.data(), &vst, call.ctl, true);
+    if (rc) { std::string keep = last_error_cstr(); vio.close_all(man.files.size()); set_last_error_str(keep); return rc; }
+    st->kernel_launches += vst.kernel_launches; st->ms_kernel += vst.ms_kernel; st->bytes_h2d += vst.bytes_h2d;
+    for (auto& b : vblocks)
+        if (vh[b.table_idx] != hashes[b.table_idx])
+            return fail(VMIG_EVERIFY, "verify: %s block %llu hashes %016llx in the destination, %016llx in the source",
+                        man.files[b.file].rel.c_str(), (unsigned long long)(b.file_off / o.block_bytes),
+                        (unsigned long long)vh[b.table_idx], (unsigned long long)hashes[b.table_idx]);
+    if (o.flags & VMIG_F_PRUNE) {               // the destination's entry set must now equal the source's
+        uint64_t extras = 0;
+        rc = prune_extras(io.dst_root, man, true, &extras, call.cancel()); if (rc) return rc;
+        if (extras) return fail(VMIG_EVERIFY, "verify: %llu destination entries are not in the source after pruning", (unsigned long long)extras);
+    }
+    return VMIG_OK;
+}
+
+// The table records each file as the call leaves it.  A snapshot's must let the next increment trust it: a linked
+// path's ctime moved with this call's link to the base inode, and a hard-linked file's with replay_metadata's link (both
+// after block_done recorded it), so they are read again.  Nothing later in the call touches these inodes.
+int write_table(FileIO& io, bool snapshot, const char* out_path, const std::vector<uint64_t>& hashes, const std::atomic<int>* cancel)
+{
+    const Manifest& man = *io.m;
+    if (snapshot) {
+        std::vector<uint32_t> refresh = io.linked_files;
+        for (uint32_t f = 0; f < man.files.size(); f++) if (!io.plan->files[f].solo && man.files[f].n_blocks) refresh.push_back(f);
+        for (uint32_t f : refresh) {
+            const std::string p = pjoin(io.dst_root, man.files[f].rel);
+            struct stat ls;
+            if (lstat(p.c_str(), &ls) != 0) return fail(VMIG_EIO, "lstat %s: %s", p.c_str(), errno_str(errno).c_str());
+            io.fs[f].identify(ls);
+        }
+    }
+    if (!out_path || !*out_path) return VMIG_OK;
+    BlockTable t; t.block_bytes = io.block_bytes; t.algo = 1;
+    t.files.reserve(man.files.size());
+    for (uint32_t f = 0; f < man.files.size(); f++) {
+        const Entry& e = man.files[f];
+        const bool own = e.hardlink_of < 0 && (e.n_blocks || !io.hash_only);      // hard-linked paths are never patched in place
+        t.files.push_back({e.rel, e.size, e.first_block, own ? io.fs[f].id_ino : 0, own ? io.fs[f].id_ctime_ns : 0});
+    }
+    t.hashes = hashes;
+    return table_store(out_path, t, cancel);
+}
+
+// VMIG_F_MOVE_SRC: the old volume's data is about to be unlinked, so deferred write-back errors (ENOSPC / EIO on delayed
+// allocation, network filesystems) must surface first: a no-op on tmpfs, one flush on a disk.  A cancelled call leaves
+// no table, also when the cancel comes after the table was renamed into place.
+int finish_move(CallScope& call, const std::string& src, const std::string& dst, const Manifest& man, const char* out_path)
+{
+    auto cancelled = [&](const char* when) {
+        if (out_path && *out_path) unlink(out_path);
+        return fail(VMIG_ECANCELED, "%s (source left in place)", when);
+    };
+    if (call.cancel()->load()) return cancelled("before the destination was flushed");
+    int dfd = open(dst.c_str(), O_RDONLY | O_DIRECTORY | O_CLOEXEC);
+    if (dfd < 0) return fail(VMIG_EIO, "open %s: %s", dst.c_str(), errno_str(errno).c_str());
+    const int sr = syncfs(dfd); const int se = errno;
+    close(dfd);
+    if (sr != 0) return fail(VMIG_EIO, "syncfs %s: %s (source left in place)", dst.c_str(), errno_str(se).c_str());
+    if (call.cancel()->load()) return cancelled("before the first unlink");
+    // the point of no return: a half-unlinked source is worse than a finished move, so a cancel is no longer honoured
+    call.phase(VMIG_PHASE_UNLINK);
+    return remove_source(src, man);
+}
+
 // snap_path non-null: vmig_restore_tree -- src_dir must match that block table (match_table before anything touches the
 // destination, every block's hash in the hash-waiter, hard-linked paths before metadata replay).
 // snapshot non-null: vmig_snapshot_tree -- unchanged files and blocks come from the base (FileIO::finish_from_base).
-int migrate_tree_body(CallScope& call, const char* src_dir, const char* dst_dir, const char* prior_path, const char* out_path,
-                      const vmig_opts& o, vmig_stats* stats_out, const char* snap_path, const SnapshotArgs* snapshot);
-
-int migrate_tree_impl(const char* src_dir, const char* dst_dir, const char* prior_path, const char* out_path,
-                      const vmig_opts* opts_in, vmig_stats* stats_out, const char* snap_path = nullptr,
-                      const SnapshotArgs* snapshot = nullptr)
-{
-    const vmig_opts o = norm_opts(opts_in);
-    CallScope call;
-    const int rc = call.attach(o.ctl);
-    if (rc) return rc;
-    return call.finish(migrate_tree_body(call, src_dir, dst_dir, prior_path, out_path, o, stats_out, snap_path, snapshot));
-}
-
 int migrate_tree_body(CallScope& call, const char* src_dir, const char* dst_dir, const char* prior_path, const char* out_path,
                       const vmig_opts& o, vmig_stats* stats_out, const char* snap_path, const SnapshotArgs* snapshot)
 {
     const char* base_dir = snapshot ? snapshot->base_dir : nullptr;
     const char* base_path = snapshot ? snapshot->base_table : nullptr;
-    CallCtl* ctl = call.ctl;
     const std::atomic<int>* cancel = call.cancel();
     vmig_stats st; memset(&st, 0, sizeof st);
     const uint64_t t_begin = now_ns();
     if (!src_dir || !*src_dir) return fail(VMIG_EINVAL, "src_dir is NULL/empty");
     const bool hash_only = (o.flags & VMIG_F_HASH_ONLY) != 0;
     if (!hash_only && (!dst_dir || !*dst_dir)) return fail(VMIG_EINVAL, "dst_dir is NULL/empty");
-    if (o.block_bytes & 4095u) return fail(VMIG_EINVAL, "block_bytes %u is not a multiple of 4096", o.block_bytes);
-    if (o.block_bytes > pipe_slot_bytes()) return fail(VMIG_EINVAL, "block_bytes %u exceeds the staging slot (%u)", o.block_bytes, pipe_slot_bytes());
+    int rc = check_block_bytes(o);
+    if (rc) return rc;
     const std::string src(src_dir), dst(dst_dir ? dst_dir : "");
     struct stat sst;
     if (stat(src.c_str(), &sst) != 0) return fail(VMIG_EIO, "stat %s: %s", src.c_str(), errno_str(errno).c_str());
@@ -653,7 +765,7 @@ int migrate_tree_body(CallScope& call, const char* src_dir, const char* dst_dir,
     if (cancel->load()) return fail(VMIG_ECANCELED, "the control was cancelled before the call started");
     // make sure a GPU is there before touching the destination: no CPU fallback
     std::vector<DeviceInfo> devs;
-    int rc = ctx_select(o.gpu_mask, &devs);
+    rc = ctx_select(o.gpu_mask, &devs);
     if (rc) return rc;
 
     Manifest man;
@@ -662,37 +774,29 @@ int migrate_tree_body(CallScope& call, const char* src_dir, const char* dst_dir,
     rc = walk_tree(src, o.block_bytes, (o.flags & VMIG_F_SKIP_HIDDEN_TOPDIRS) != 0, &man, cancel);
     if (rc) return rc;
     st.ns_walk = now_ns() - t0;
-    ctl->bytes_total.store(man.bytes_total); ctl->blocks_total.store(man.n_blocks);
+    call.ctl->bytes_total.store(man.bytes_total); call.ctl->blocks_total.store(man.n_blocks);
 
     t0 = now_ns();
     std::vector<uint64_t> expect;
     if (snap_path) {
         BlockTable snap;
-        rc = table_load(snap_path, &snap);
-        if (rc) return rc;
-        if (snap.block_bytes != o.block_bytes) return fail(VMIG_ETABLE, "snapshot table block size %u != %u", snap.block_bytes, o.block_bytes);
-        rc = match_table(man, snap, &expect);
+        rc = load_table(snap_path, "snapshot", o.block_bytes, &snap);
+        if (!rc) rc = match_table(man, snap, &expect);
         if (rc) return rc;
     }
-    BlockTable prior; bool has_prior = false;
-    if (prior_path && *prior_path && !hash_only) {
-        rc = table_load(prior_path, &prior);
-        if (rc) return rc;
-        if (prior.block_bytes != o.block_bytes) return fail(VMIG_ETABLE, "prior table block size %u != %u", prior.block_bytes, o.block_bytes);
-        has_prior = true;
-    }
+    BlockTable prior;
+    const bool has_prior = prior_path && *prior_path && !hash_only;
+    if (has_prior && (rc = load_table(prior_path, "prior", o.block_bytes, &prior))) return rc;
     BlockTable base; bool has_base = false;
-    vmig_snapshot_stats sst_snap; memset(&sst_snap, 0, sizeof sst_snap);
     if (base_path) {
-        rc = table_load(base_path, &base);
+        rc = load_table(base_path, "base", o.block_bytes, &base);
         if (rc) return rc;
-        if (base.block_bytes != o.block_bytes) return fail(VMIG_ETABLE, "base table block size %u != %u", base.block_bytes, o.block_bytes);
         // a hard link cannot cross devices, and a base on another filesystem shares nothing with the snapshot
         struct stat bst, dst_st;
         has_base = stat(base_dir, &bst) == 0 && stat(dst.c_str(), &dst_st) == 0 && bst.st_dev == dst_st.st_dev;
     }
     FileIO io;
-    io.src_root = src; io.dst_root = dst; io.m = &man; io.pol = default_meta_policy(o.flags); io.hash_only = hash_only;
+    io.src_root = src; io.dst_root = dst; io.pol = default_meta_policy(o.flags); io.hash_only = hash_only;
     io.block_bytes = o.block_bytes;
     io.corrupt_block = env_long("VMIG_CORRUPT_BLOCK", -1);
     io.direct = (o.flags & VMIG_F_DIRECT_IO) != 0;
@@ -700,89 +804,17 @@ int migrate_tree_body(CallScope& call, const char* src_dir, const char* dst_dir,
     io.cancel = cancel;
     if (io.cufile) { rc = cufile_open(); if (rc) return rc; }
     rc = io.open_root(); if (rc) return rc;
-    io.fs.reset(new FileIO::FS[man.files.size() ? man.files.size() : 1]);
+    TreePlan plan;
+    rc = plan_tree(man, o.block_bytes, dst, has_prior ? &prior : nullptr, has_base ? base_dir : "", has_base ? &base : nullptr, cancel, &plan);
+    if (rc) return rc;
+    st.files_untrusted = plan.files_untrusted;
+    io.init_files(man, plan);
     std::vector<uint64_t> hashes(man.n_blocks, 0);
-
-    // ---- per-file state + block list.  Files are taken in groups of 64 (bounds open fds) and
-    // blocks round-robin across the group's files so many destination files are written at once
-    // (a single tmpfs/xfs file takes writes one thread at a time: probe/hostio_probe.cu).
-    std::vector<BlockRef> blocks; blocks.reserve(man.n_blocks);
-    std::vector<uint32_t> group;
-    auto flush_group = [&]() {
-        uint64_t maxb = 0;
-        for (uint32_t f : group) maxb = std::max(maxb, man.files[f].n_blocks);
-        for (uint64_t r = 0; r < maxb; r++)
-            for (uint32_t f : group) {
-                const Entry& e = man.files[f];
-                if (r >= e.n_blocks) continue;
-                BlockRef b; b.file = f; b.file_off = r * (uint64_t)o.block_bytes;
-                b.len = (uint32_t)std::min<uint64_t>(o.block_bytes, e.size - b.file_off);
-                b.table_idx = e.first_block + r; b.prior_hash = 0; b.prior_valid = 0;
-                // the same rule for a file patched in place and for a snapshot file whose base is trusted
-                const BlockTable* pt = io.fs[f].inplace ? &prior : io.fs[f].base_rec ? &base : nullptr;
-                if (pt) {
-                    const TableFile& pf = io.fs[f].inplace ? prior.files[prior.index[e.rel]] : *io.fs[f].base_rec;
-                    const uint64_t plen = r < pt->blocks_of(pf) ? std::min<uint64_t>(o.block_bytes, pf.size - b.file_off) : 0;
-                    if (plen == b.len) { b.prior_hash = pt->hashes[pf.first_block + r]; b.prior_valid = 1; }
-                }
-                blocks.push_back(b);
-            }
-        group.clear();
-    };
-    bool any_base = false;
-    std::vector<uint8_t> base_trusted(base.files.size(), 0);
-    if (has_base) {
-        io.base_root = base_dir;
-        // take blocks from a base file only while it still IS the one the base table was written for (its link count may
-        // exceed 1: base files are shared with older snapshots).  Every record is checked, once: a source file may find
-        // its bytes in any base file, whatever its path.
-        for (size_t i = 0; i < base.files.size(); i++) {
-            const TableFile& bf = base.files[i];
-            if (i % kMetaCheckEvery == 0 && cancel->load()) return fail(VMIG_ECANCELED, "while checking the base's files");
-            struct stat bs;
-            base_trusted[i] = bf.ino != 0 && lstat(pjoin(io.base_root, bf.rel).c_str(), &bs) == 0 && S_ISREG(bs.st_mode) &&
-                              (uint64_t)bs.st_ino == bf.ino && (uint64_t)bs.st_size == bf.size &&
-                              (int64_t)bs.st_ctim.tv_sec * 1000000000ll + bs.st_ctim.tv_nsec == bf.ctime_ns;
-        }
-        io.bidx.build(base, base_trusted);
-        io.hashes = hashes.data();
-    }
-    for (auto& e : man.files) if (e.hardlink_of >= 0) io.fs[(size_t)e.hardlink_of].solo = false;
-    for (uint32_t f = 0; f < man.files.size(); f++) {
-        const Entry& e = man.files[f];
-        if (e.hardlink_of >= 0 || e.n_blocks == 0) continue;
-        FileIO::FS& s = io.fs[f];
-        s.reads_left.store((uint32_t)e.n_blocks); s.blocks_left.store((uint32_t)e.n_blocks);
-        if (has_base) {
-            auto it = base.index.find(e.rel);
-            if (it != base.index.end() && base.files[it->second].ino != 0) {
-                if (base_trusted[it->second]) { s.base_rec = &base.files[it->second]; any_base = true; }
-                else sst_snap.files_base_untrusted++;
-            }
-        }
-        if (has_prior) {
-            auto it = prior.index.find(e.rel);
-            struct stat ds;
-            // patch in place only a destination file that still IS the one the table was written for: same
-            // inode, same ctime (any write, truncate, chmod or replacement since then moved it), same size
-            if (it != prior.index.end() && lstat(pjoin(dst, e.rel).c_str(), &ds) == 0 && S_ISREG(ds.st_mode) && ds.st_nlink == 1) {
-                const TableFile& pf = prior.files[it->second];
-                const int64_t ct = (int64_t)ds.st_ctim.tv_sec * 1000000000ll + ds.st_ctim.tv_nsec;
-                if (pf.ino != 0 && (uint64_t)ds.st_ino == pf.ino && ct == pf.ctime_ns && (uint64_t)ds.st_size == pf.size) {
-                    s.inplace = true; s.dst_old_size = (uint64_t)ds.st_size;
-                } else if (pf.ino != 0) {
-                    st.files_untrusted++;
-                }
-            }
-        }
-        group.push_back(f);
-        if (group.size() == 64) flush_group();
-    }
-    flush_group();
+    if (has_base) { io.base_root = base_dir; io.bidx.build(base, plan.base_trusted); io.hashes = hashes.data(); }
     // skip mode whenever the base can supply a block, also when no source path has a same-path record (a layer whose
     // files were all moved): without it the submitter streams every block back with its hash (DESIGN.md §3)
-    const bool skip_mode = has_prior || any_base || !io.bidx.empty();
-    if (any_base || !io.bidx.empty()) io.skipped.assign(man.n_blocks, 0);
+    const bool skip_mode = has_prior || plan.any_base || !io.bidx.empty();
+    if (plan.any_base || !io.bidx.empty()) io.skipped.assign(man.n_blocks, 0);
     st.ns_plan = now_ns() - t0;
 
     // VMIG_F_PRUNE runs first: what it removes is by definition not in the source, a directory sitting where the source
@@ -798,129 +830,31 @@ int migrate_tree_body(CallScope& call, const char* src_dir, const char* dst_dir,
     if (!hash_only) { rc = make_dirs(dst, man); if (rc) return rc; }
 
     t0 = now_ns();
-    rc = run_blocks(blocks, &io, skip_mode, hash_only, o, hashes.data(), &st, ctl, false, expect.empty() ? nullptr : expect.data());
+    rc = run_blocks(plan.blocks, &io, skip_mode, hash_only, o, hashes.data(), &st, call.ctl, false, expect.empty() ? nullptr : expect.data());
     st.ns_data = now_ns() - t0;
     if (rc) { std::string keep = last_error_cstr(); io.close_all(man.files.size()); set_last_error_str(keep); return rc; }
 
     t0 = now_ns();
     call.phase(VMIG_PHASE_META);
-    if (cancel->load()) return fail(VMIG_ECANCELED, "after the data pass, before any metadata step");
-    for (auto& e : man.files)                      // hard-linked paths share their primary's hashes
-        if (e.hardlink_of >= 0) {
-            const Entry& p = man.files[(size_t)e.hardlink_of];
-            for (uint64_t r = 0; r < e.n_blocks; r++) {
-                hashes[e.first_block + r] = hashes[p.first_block + r];
-                // restore: the table hashed this path on its own; it must describe the bytes its primary now holds
-                // (checked before replay_metadata creates any link)
-                if (!expect.empty() && expect[e.first_block + r] != hashes[e.first_block + r])
-                    return fail(VMIG_ECORRUPT, "%s block %llu (a hard link to %s) hashes %016llx, its block table says %016llx",
-                                e.rel.c_str(), (unsigned long long)r, p.rel.c_str(), (unsigned long long)hashes[e.first_block + r],
-                                (unsigned long long)expect[e.first_block + r]);
-            }
-        }
-    if (!hash_only) {
-        size_t steps = 0;
-        for (auto& e : man.files) {                // empty regular files carry no blocks
-            if (e.hardlink_of >= 0 || e.n_blocks) continue;
-            if (steps++ % kMetaCheckEvery == 0 && cancel->load()) return fail(VMIG_ECANCELED, "before creating %s", e.rel.c_str());
-            const std::string p = pjoin(dst, e.rel);
-            rc = clear_path(p, "an empty regular file"); if (rc) return rc;
-            int fd = open(p.c_str(), O_WRONLY | O_CREAT | O_EXCL | O_CLOEXEC | O_NOFOLLOW, 0600);
-            if (fd < 0) return fail(VMIG_EIO, "create %s: %s", p.c_str(), errno_str(errno).c_str());
-            rc = apply_file_meta(fd, p, e, io.pol);
-            struct stat ids;
-            if (!rc && fstat(fd, &ids) == 0) {
-                FileIO::FS& s = io.fs[&e - &man.files[0]];
-                s.id_ino = (uint64_t)ids.st_ino; s.id_ctime_ns = (int64_t)ids.st_ctim.tv_sec * 1000000000ll + ids.st_ctim.tv_nsec;
-            }
-            close(fd);
-            if (rc) return rc;
-        }
-        rc = replay_metadata(dst, man, io.pol, &st.symlinks, &st.hardlinks, &st.specials, cancel);
-        if (rc) return rc;
-    }
+    rc = meta_pass(call, io, expect, &hashes, &st);
+    if (rc) return rc;
     st.ns_meta = now_ns() - t0;
 
     if ((o.flags & VMIG_F_VERIFY) && !hash_only) {
         call.phase(VMIG_PHASE_VERIFY);
-        // read the destination back through the same GPU path (hash only) and compare block tables
-        FileIO vio;
-        vio.src_root = dst; vio.dst_root = dst; vio.m = &man; vio.pol = io.pol; vio.hash_only = true;
-        vio.direct = io.direct;          // O_DIRECT re-read: what is verified is what the device holds, not the page cache
-        vio.cufile = io.cufile;
-        vio.fs.reset(new FileIO::FS[man.files.size() ? man.files.size() : 1]);
-        rc = vio.open_root(); if (rc) return rc;
-        for (uint32_t f = 0; f < man.files.size(); f++) {
-            const Entry& e = man.files[f];
-            if (e.hardlink_of >= 0 || e.n_blocks == 0) continue;
-            vio.fs[f].reads_left.store((uint32_t)e.n_blocks); vio.fs[f].blocks_left.store((uint32_t)e.n_blocks);
-        }
-        std::vector<BlockRef> vblocks = blocks;
-        for (auto& b : vblocks) { b.prior_hash = 0; b.prior_valid = 0; }
-        std::vector<uint64_t> vh(man.n_blocks, 0);
-        vmig_stats vst; memset(&vst, 0, sizeof vst);
-        rc = run_blocks(vblocks, &vio, false, true, o, vh.data(), &vst, ctl, true);
-        if (rc) { std::string keep = last_error_cstr(); vio.close_all(man.files.size()); set_last_error_str(keep); return rc; }
-        st.kernel_launches += vst.kernel_launches; st.ms_kernel += vst.ms_kernel; st.bytes_h2d += vst.bytes_h2d;
-        for (auto& b : vblocks)
-            if (vh[b.table_idx] != hashes[b.table_idx])
-                return fail(VMIG_EVERIFY, "verify: %s block %llu hashes %016llx in the destination, %016llx in the source",
-                            man.files[b.file].rel.c_str(), (unsigned long long)(b.file_off / o.block_bytes),
-                            (unsigned long long)vh[b.table_idx], (unsigned long long)hashes[b.table_idx]);
-        if (o.flags & VMIG_F_PRUNE) {               // the destination's entry set must now equal the source's
-            uint64_t extras = 0;
-            rc = prune_extras(dst, man, true, &extras, cancel); if (rc) return rc;
-            if (extras) return fail(VMIG_EVERIFY, "verify: %llu destination entries are not in the source after pruning", (unsigned long long)extras);
-        }
+        rc = verify_pass(call, o, io, hashes, &st);
+        if (rc) return rc;
     }
 
     t0 = now_ns();
     call.phase(VMIG_PHASE_TABLE);
-    // A snapshot's table records each file as the call leaves it, so that the next increment can trust it: a linked
-    // path's ctime moved with this call's link to the base inode, and a hard-linked file's with replay_metadata's link
-    // (both after block_done recorded it).  Nothing later in the call touches these inodes.
-    if (snapshot) {
-        std::vector<uint32_t> refresh = io.linked_files;
-        for (uint32_t f = 0; f < man.files.size(); f++) if (!io.fs[f].solo && man.files[f].n_blocks) refresh.push_back(f);
-        for (uint32_t f : refresh) {
-            const std::string p = pjoin(dst, man.files[f].rel);
-            struct stat ls;
-            if (lstat(p.c_str(), &ls) != 0) return fail(VMIG_EIO, "lstat %s: %s", p.c_str(), errno_str(errno).c_str());
-            io.fs[f].id_ino = (uint64_t)ls.st_ino; io.fs[f].id_ctime_ns = (int64_t)ls.st_ctim.tv_sec * 1000000000ll + ls.st_ctim.tv_nsec;
-        }
-    }
-    if (out_path && *out_path) {
-        BlockTable t; t.block_bytes = o.block_bytes; t.algo = 1;
-        t.files.reserve(man.files.size());
-        for (uint32_t f = 0; f < man.files.size(); f++) {
-            const Entry& e = man.files[f];
-            const bool own = e.hardlink_of < 0 && (e.n_blocks || !hash_only);         // hard-linked paths are never patched in place
-            t.files.push_back({e.rel, e.size, e.first_block, own ? io.fs[f].id_ino : 0, own ? io.fs[f].id_ctime_ns : 0});
-        }
-        t.hashes = hashes;
-        rc = table_store(out_path, t, cancel);
-        if (rc) return rc;
-    }
+    rc = write_table(io, snapshot != nullptr, out_path, hashes, cancel);
+    if (rc) return rc;
     st.ns_table = now_ns() - t0;
 
     if ((o.flags & VMIG_F_MOVE_SRC) && !hash_only) {
-        // the old volume's data is about to be unlinked: deferred write-back errors (ENOSPC / EIO on delayed
-        // allocation, network filesystems) must surface first.  A no-op on tmpfs; one flush on a disk.
-        // a cancelled call leaves no table, also when the cancel comes after the table was renamed into place
-        auto cancelled = [&](const char* when) {
-            if (out_path && *out_path) unlink(out_path);
-            return fail(VMIG_ECANCELED, "%s (source left in place)", when);
-        };
-        if (cancel->load()) return cancelled("before the destination was flushed");
-        int dfd = open(dst.c_str(), O_RDONLY | O_DIRECTORY | O_CLOEXEC);
-        if (dfd < 0) return fail(VMIG_EIO, "open %s: %s", dst.c_str(), errno_str(errno).c_str());
-        const int sr = syncfs(dfd); const int se = errno;
-        close(dfd);
-        if (sr != 0) return fail(VMIG_EIO, "syncfs %s: %s (source left in place)", dst.c_str(), errno_str(se).c_str());
-        if (cancel->load()) return cancelled("before the first unlink");
-        // the point of no return: a half-unlinked source is worse than a finished move, so a cancel is no longer honoured
-        call.phase(VMIG_PHASE_UNLINK);
-        rc = remove_source(src, man); if (rc) return rc;
+        rc = finish_move(call, src, dst, man, out_path);
+        if (rc) return rc;
     }
 
     st.files_direct = io.n_direct.load();
@@ -929,11 +863,24 @@ int migrate_tree_body(CallScope& call, const char* src_dir, const char* dst_dir,
     st.ns_total = now_ns() - t_begin;
     if (stats_out) *stats_out = st;
     if (snapshot && snapshot->out) {
-        sst_snap.files_linked = io.n_linked.load(); sst_snap.bytes_linked = io.b_linked.load();
-        sst_snap.files_backfilled = io.n_backfilled.load(); sst_snap.bytes_backfilled = io.b_backfilled.load();
-        *snapshot->out = sst_snap;
+        vmig_snapshot_stats ss; memset(&ss, 0, sizeof ss);
+        ss.files_base_untrusted = plan.files_base_untrusted;
+        ss.files_linked = io.n_linked.load(); ss.bytes_linked = io.b_linked.load();
+        ss.files_backfilled = io.n_backfilled.load(); ss.bytes_backfilled = io.b_backfilled.load();
+        *snapshot->out = ss;
     }
     return VMIG_OK;
+}
+
+int migrate_tree_impl(const char* src_dir, const char* dst_dir, const char* prior_path, const char* out_path,
+                      const vmig_opts* opts_in, vmig_stats* stats_out, const char* snap_path = nullptr,
+                      const SnapshotArgs* snapshot = nullptr)
+{
+    const vmig_opts o = norm_opts(opts_in);
+    CallScope call;
+    const int rc = call.attach(o.ctl);
+    if (rc) return rc;
+    return call.finish(migrate_tree_body(call, src_dir, dst_dir, prior_path, out_path, o, stats_out, snap_path, snapshot));
 }
 
 // vmig_snapshot_tree: a base directory equal to the destination, or either one inside the other, is refused -- a
@@ -963,7 +910,7 @@ public:
     uint32_t block_bytes = 4u << 20;
     int read_block(const BlockRef& b, uint8_t* dst) override { return r->read(b.file, b.file_off, b.len, dst); }
     int write_block(const BlockRef&, const uint8_t*) override { return fail(VMIG_EINVAL, "a scrub writes nothing"); }
-    uint32_t slot_align() override { return r->direct ? ScrubReader::kSector : 512; }
+    uint32_t slot_align() override { return r->direct ? kSector : 512; }
     std::string block_name(const BlockRef& b) override {
         const ScrubInode& I = (*r->inodes)[b.file];
         return I.rel + " (version " + std::to_string(I.version) + ") block " + std::to_string(b.file_off / block_bytes);
@@ -1028,22 +975,11 @@ int scrub_body(CallScope& call, uint32_t n, const char* const* dirs, const char*
     reader.root_fds = root_fds; reader.inodes = &inodes; reader.direct = (o.flags & VMIG_F_DIRECT_IO) != 0;
     reader.init();
     ScrubIO io; io.r = &reader; io.block_bytes = o.block_bytes;
-    // inodes in groups of 64 (bounds open descriptors), blocks round-robin across a group's inodes: as a migration does
+    // the block order of a migration
+    std::vector<BlockSpan> spans;
+    for (uint32_t u = 0; u < inodes.size(); u++) spans.push_back({u, inodes[u].size, inodes[u].first_block, inodes[u].n_blocks});
     std::vector<BlockRef> blocks; blocks.reserve(n_blocks);
-    for (size_t g = 0; g < inodes.size(); g += 64) {
-        const size_t g1 = std::min(inodes.size(), g + 64);
-        uint64_t maxb = 0;
-        for (size_t u = g; u < g1; u++) maxb = std::max(maxb, inodes[u].n_blocks);
-        for (uint64_t r = 0; r < maxb; r++)
-            for (size_t u = g; u < g1; u++) {
-                const ScrubInode& I = inodes[u];
-                if (r >= I.n_blocks) continue;
-                BlockRef b; b.file = (uint32_t)u; b.file_off = r * (uint64_t)o.block_bytes;
-                b.len = (uint32_t)std::min<uint64_t>(o.block_bytes, I.size - b.file_off);
-                b.table_idx = I.first_block + r; b.prior_hash = 0; b.prior_valid = 0;
-                blocks.push_back(b);
-            }
-    }
+    interleave_blocks(spans, o.block_bytes, &blocks);
     st.ns_plan = now_ns() - t0;
 
     // ---- the data pass: K1 over every distinct block, once
@@ -1233,10 +1169,10 @@ int vmig_scrub_store(uint32_t n, const char* const* snap_dirs, const char* const
     const vmig_opts o = norm_opts(opts);                     // VMIG_CUFILE=1 in the environment is refused too
     const uint32_t allowed = VMIG_F_DIRECT_IO | VMIG_F_SKIP_HIDDEN_TOPDIRS;
     if (o.flags & ~allowed) return fail(VMIG_EINVAL, "flags 0x%x: a scrub takes only VMIG_F_DIRECT_IO and VMIG_F_SKIP_HIDDEN_TOPDIRS", o.flags & ~allowed);
-    if (o.block_bytes & 4095u) return fail(VMIG_EINVAL, "block_bytes %u is not a multiple of 4096", o.block_bytes);
-    if (o.block_bytes > pipe_slot_bytes()) return fail(VMIG_EINVAL, "block_bytes %u exceeds the staging slot (%u)", o.block_bytes, pipe_slot_bytes());
+    int rc = check_block_bytes(o);
+    if (rc) return rc;
     CallScope call;
-    const int rc = call.attach(o.ctl);
+    rc = call.attach(o.ctl);
     if (rc) return rc;
     return call.finish(scrub_body(call, n, snap_dirs, snap_tables, report_path, verdicts, o, stats, scrub_stats));
 }
@@ -1273,9 +1209,9 @@ int vmig_migrate_buffer(const void* src, void* dst, uint64_t nbytes, const uint6
     vmig_opts o = norm_opts(opts);
     const bool hash_only = (o.flags & VMIG_F_HASH_ONLY) != 0;
     if (!src || (!dst && !hash_only)) return fail(VMIG_EINVAL, "null buffer");
-    if ((o.block_bytes & 4095u) || o.block_bytes > pipe_slot_bytes()) return fail(VMIG_EINVAL, "bad block_bytes %u", o.block_bytes);
+    int rc = check_block_bytes(o); if (rc) return rc;
     CallScope call;
-    int rc = call.attach(o.ctl); if (rc) return rc;
+    rc = call.attach(o.ctl); if (rc) return rc;
     if (call.cancel()->load()) return call.finish(fail(VMIG_ECANCELED, "the control was cancelled before the call started"));
     std::vector<DeviceInfo> devs; rc = ctx_select(o.gpu_mask, &devs); if (rc) return rc;
     const uint64_t nb = (nbytes + o.block_bytes - 1) / o.block_bytes;

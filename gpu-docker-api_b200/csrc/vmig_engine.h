@@ -9,7 +9,6 @@
 // One Pipe owns kSlots such slot triples on one GPU; a lane (one GPU's share of one call) checks
 // a Pipe out of the process-wide pool, runs its block list through it and returns it.
 #pragma once
-#include <cuda_runtime.h>
 #include <stdint.h>
 #include <atomic>
 #include <memory>

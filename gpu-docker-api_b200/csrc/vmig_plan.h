@@ -1,0 +1,43 @@
+// vmig_plan.h -- the plan of a tree call (migrate, move, restore, snapshot): which destination files are patched in
+// place, which base-snapshot files may supply blocks, and the block list in submission order.  No CUDA (tests/plan_unit.cpp).
+#pragma once
+#include <stdint.h>
+#include <atomic>
+#include <string>
+#include <vector>
+#include "vmig_engine.h"
+#include "vmig_table.h"
+#include "vmig_tree.h"
+
+namespace vmig {
+
+// The blocks of one file (or scrub inode): BlockRef.file = file, hashes [first_block, first_block + n_blocks)
+struct BlockSpan { uint32_t file; uint64_t size, first_block, n_blocks; };
+
+// Append the blocks of spans[]: files in groups of 64 (bounds open descriptors), blocks round-robin across a group so that
+// many destination files are written at once (one tmpfs/xfs file takes writes one thread at a time: probe/hostio_probe.cu)
+void interleave_blocks(const std::vector<BlockSpan>& spans, uint32_t block_bytes, std::vector<BlockRef>* out);
+
+struct FilePlan {
+    const TableFile* prior_rec = nullptr;   // patched in place: the destination file still is this prior-table record
+    const TableFile* base_rec = nullptr;    // vmig_snapshot_tree: the same-path base file still is this record
+    bool solo = true;                       // no other source path is a hard link to this file
+};
+
+struct TreePlan {
+    std::vector<FilePlan> files;            // per manifest file
+    std::vector<uint8_t> base_trusted;      // per base-table file: it still is the file its record was written for
+    bool any_base = false;                  // some file has a base_rec
+    uint64_t files_untrusted = 0;           // vmig_stats.files_untrusted
+    uint64_t files_base_untrusted = 0;      // vmig_snapshot_stats.files_base_untrusted
+    std::vector<BlockRef> blocks;           // interleave_blocks order; a block's prior hash is its prior_rec / base_rec one
+};
+
+// prior (nullable): a destination file under dst_root is patched in place while it still is its record and has one link.
+// base (nullable; only when base_root is on the destination's device): every record is checked once, as a source file
+// may find its bytes in any base file.  Both tables are at block_bytes.  VMIG_ECANCELED once *cancel (nullable) is set,
+// checked every kMetaCheckEvery base records.
+int plan_tree(const Manifest& man, uint32_t block_bytes, const std::string& dst_root, const BlockTable* prior,
+              const std::string& base_root, const BlockTable* base, const std::atomic<int>* cancel, TreePlan* out);
+
+}  // namespace vmig

@@ -224,22 +224,14 @@ int ScrubReader::read(uint32_t u, uint64_t off, uint32_t len, uint8_t* dst)
     if (rc) { mark_bad(u, last_error_cstr()); done_one(u); return VMIG_OK; }
     const ScrubInode& I = (*inodes)[u];
     // O_DIRECT: buffer, offset and length in whole sectors (the pipeline's slot layout leaves the room), as FileIO reads
-    const size_t want = s.s_direct ? (size_t)align_up(len, kSector) : len;
-    size_t got = 0;
-    while (got < len) {
-        const size_t pos = s.s_direct ? (got & ~(size_t)(kSector - 1)) : got;
-        const ssize_t r = pread(fd, dst + pos, want - pos, (off_t)(off + pos));
-        if (r < 0) {
-            if (errno == EINTR) continue;
-            char b[64]; snprintf(b, sizeof b, " at offset %llu: ", (unsigned long long)(off + pos));
-            mark_bad(u, "pread " + I.rel + b + errno_str(errno));
-            done_one(u);
-            return VMIG_OK;
-        }
-        if (r == 0 || pos + (size_t)r <= got)
-            return fail(VMIG_ESRCCHANGED, "%s (version %u) shrank during the scrub (wanted %u bytes at %llu, got %zu)", I.rel.c_str(), I.version,
-                        len, (unsigned long long)off, got);
-        got = pos + (size_t)r;
+    size_t got, at = 0;
+    rc = xfer_block(s.s_direct, true, len, &got, [&](size_t pos, size_t n) { at = pos; return pread(fd, dst + pos, n, (off_t)(off + pos)); });
+    if (rc < 0) {
+        char b[64]; snprintf(b, sizeof b, " at offset %llu: ", (unsigned long long)(off + at));
+        mark_bad(u, "pread " + I.rel + b + errno_str(errno));
+    } else if (rc > 0) {
+        return fail(VMIG_ESRCCHANGED, "%s (version %u) shrank during the scrub (wanted %u bytes at %llu, got %zu)", I.rel.c_str(), I.version,
+                    len, (unsigned long long)off, got);
     }
     done_one(u);
     return VMIG_OK;

@@ -71,7 +71,6 @@ public:
     std::vector<int> root_fds;                 // per version; -1 for a version that is not read (not owned)
     const std::vector<ScrubInode>* inodes = nullptr;
     bool direct = false;                       // VMIG_F_DIRECT_IO
-    static constexpr uint32_t kSector = 4096;
     std::atomic<uint64_t> n_direct{0};         // descriptors really opened O_DIRECT
 
     void init();                               // after inodes is set: one reads_left per block

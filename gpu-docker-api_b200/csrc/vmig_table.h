@@ -5,6 +5,7 @@
 // internal/version/merge.go:16 (ContainerMergeMap) records.
 #pragma once
 #include <stdint.h>
+#include <sys/stat.h>
 #include <atomic>
 #include <string>
 #include <vector>
@@ -17,6 +18,13 @@ namespace vmig {
 // paths).  The in-place diff path trusts a prior table for a destination file only while both still match
 // (ctime cannot be set from user space: any out-of-band write, truncate, chmod or rename-over bumps it).
 struct TableFile { std::string rel; uint64_t size; uint64_t first_block; uint64_t ino = 0; int64_t ctime_ns = 0; };
+
+inline int64_t ctime_ns(const struct stat& st) { return (int64_t)st.st_ctim.tv_sec * 1000000000ll + st.st_ctim.tv_nsec; }
+// st is the file rec was written for: a regular file with the recorded inode, size and ctime (rec.ino == 0: unknown)
+inline bool is_recorded_file(const struct stat& st, const TableFile& rec) {
+    return S_ISREG(st.st_mode) && rec.ino != 0 && (uint64_t)st.st_ino == rec.ino && (uint64_t)st.st_size == rec.size &&
+           ctime_ns(st) == rec.ctime_ns;
+}
 
 struct BlockTable {
     uint32_t block_bytes = 0;

@@ -20,11 +20,6 @@
 
 namespace vmig {
 
-static inline std::string join(const std::string& a, const std::string& b) {
-    if (b == ".") return a;
-    return a + "/" + b;
-}
-
 // The source may belong to a container that is still running (the first pass of a two-pass hand-off), so
 // nothing on the source side trusts a path twice: directories are entered with openat(O_NOFOLLOW) relative to
 // their parent's descriptor, and files are opened later with open_beneath() below.  A directory that a tenant
@@ -304,7 +299,7 @@ int copy_range_at(int in_fd, uint64_t off, int out_fd, uint64_t out_off, uint64_
             }
         }
     }
-    const size_t kSector = 4096, kChunk = 1u << 20;
+    const size_t kChunk = 1u << 20;
     void* mem = nullptr;
     if (done < len && posix_memalign(&mem, kSector, kChunk) != 0) return fail(VMIG_ENOMEM, "copy buffer for %s", what.c_str());
     uint8_t* buf = (uint8_t*)mem;
@@ -343,7 +338,7 @@ int copy_range_at(int in_fd, uint64_t off, int out_fd, uint64_t out_off, uint64_
 int make_dirs(const std::string& dst_root, const Manifest& m)
 {
     for (size_t i = 1; i < m.dirs.size(); i++) {
-        const std::string p = join(dst_root, m.dirs[i].rel);
+        const std::string p = pjoin(dst_root, m.dirs[i].rel);
         if (mkdir(p.c_str(), 0700) == 0) continue;
         if (errno != EEXIST) return fail(VMIG_EIO, "mkdir %s: %s", p.c_str(), errno_str(errno).c_str());
         struct stat st;
@@ -396,7 +391,7 @@ int replay_metadata(const std::string& dst_root, const Manifest& m, const MetaPo
     struct timespec ts[2];
     for (const auto& e : m.symlinks) {
         if (int rc = stop(e.rel)) return rc;
-        const std::string p = join(dst_root, e.rel);
+        const std::string p = pjoin(dst_root, e.rel);
         int rc = clear_path(p, "a symlink");
         if (rc) return rc;
         if (symlink(e.target.c_str(), p.c_str()) != 0) return fail(VMIG_EIO, "symlink %s: %s", p.c_str(), errno_str(errno).c_str());
@@ -409,7 +404,7 @@ int replay_metadata(const std::string& dst_root, const Manifest& m, const MetaPo
     }
     for (const auto& e : m.specials) {
         if (int rc = stop(e.rel)) return rc;
-        const std::string p = join(dst_root, e.rel);
+        const std::string p = pjoin(dst_root, e.rel);
         int rc = clear_path(p, "a special file");
         if (rc) return rc;
         if (mknod(p.c_str(), (e.mode & S_IFMT) | 0600, e.rdev) != 0) return fail(VMIG_EIO, "mknod %s: %s", p.c_str(), errno_str(errno).c_str());
@@ -420,8 +415,8 @@ int replay_metadata(const std::string& dst_root, const Manifest& m, const MetaPo
     for (const auto& e : m.files) {
         if (e.hardlink_of < 0) continue;
         if (int rc = stop(e.rel)) return rc;
-        const std::string p = join(dst_root, e.rel);
-        const std::string prim = join(dst_root, m.files[(size_t)e.hardlink_of].rel);
+        const std::string p = pjoin(dst_root, e.rel);
+        const std::string prim = pjoin(dst_root, m.files[(size_t)e.hardlink_of].rel);
         int rc = clear_path(p, "a hard link");
         if (rc) return rc;
         if (link(prim.c_str(), p.c_str()) != 0) return fail(VMIG_EIO, "link %s -> %s: %s", p.c_str(), prim.c_str(), errno_str(errno).c_str());
@@ -431,7 +426,7 @@ int replay_metadata(const std::string& dst_root, const Manifest& m, const MetaPo
         for (size_t i = m.dirs.size(); i-- > 0;) {     // children before parents
             const Entry& e = m.dirs[i];
             if (int rc = stop(e.rel)) return rc;
-            const std::string p = join(dst_root, e.rel);
+            const std::string p = pjoin(dst_root, e.rel);
             if (pol.is_root && chown(p.c_str(), e.uid, e.gid) != 0) return fail(VMIG_EIO, "chown %s: %s", p.c_str(), errno_str(errno).c_str());
             if (chmod(p.c_str(), eff_mode(e, pol)) != 0) return fail(VMIG_EIO, "chmod %s: %s", p.c_str(), errno_str(errno).c_str());
             fill_times(e, pol, ts);

@@ -16,6 +16,9 @@
 
 namespace vmig {
 
+// a manifest path under root ("." is the root itself)
+inline std::string pjoin(const std::string& root, const std::string& rel) { return rel == "." ? root : root + "/" + rel; }
+
 enum EntryType : uint8_t { kDir = 1, kFile, kSymlink, kSpecial /* chr, blk, fifo */ };
 
 struct Entry {

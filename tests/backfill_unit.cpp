@@ -4,10 +4,13 @@
 // of the output and nothing else; an O_DIRECT output takes whole sectors (the caller truncates); an input that ends
 // early is VMIG_ESRCCHANGED.
 //   usage: backfill_unit DIR [DIR2 ...]   (each DIR is tried; O_DIRECT runs where the filesystem allows it)
+//          backfill_unit --large DIR      (a sparse file of 2^32 + 9 MiB + 777 bytes: one run longer than 2^32 bytes and offsets
+//                                          above 2^32, through both paths; DIR needs about 5 GiB, best on tmpfs)
 #include "vmig_tree.h"
 #include "vmig_common.h"
 #include <fcntl.h>
 #include <unistd.h>
+#include <sys/stat.h>
 #include <algorithm>
 #include <cstdio>
 #include <cstdlib>
@@ -76,8 +79,83 @@ static int run(const std::string& dir) {
     return 0;
 }
 
+// ---------------------------------------------------------------------------------------------- past 4 GiB
+static const uint64_t kBig = (1ull << 32) + (9ull << 20) + 777, k4G = 1ull << 32, kMiB = 1ull << 20;
+
+// Island bytes name their own offset and file, so bytes that landed in the wrong place cannot pass for the right ones
+static void island(std::vector<uint8_t>* v, uint64_t off, uint64_t salt) {
+    for (size_t i = 0; i < v->size(); i++) {
+        const uint64_t o = off + i, w = (o / 8 + salt) * 0x9E3779B97F4A7C15ull;
+        (*v)[i] = (uint8_t)(w >> (8 * (o % 8))) ^ (uint8_t)(w >> 56);
+    }
+}
+static bool put_at(int fd, uint64_t off, const std::vector<uint8_t>& v) {
+    size_t put = 0;
+    while (put < v.size()) { const ssize_t w = pwrite(fd, v.data() + put, v.size() - put, (off_t)(off + put)); if (w <= 0) return false; put += (size_t)w; }
+    return true;
+}
+static bool get_at(int fd, uint64_t off, std::vector<uint8_t>* v) {
+    size_t got = 0;
+    while (got < v->size()) { const ssize_t r = pread(fd, v->data() + got, v->size() - got, (off_t)(off + got)); if (r <= 0) return false; got += (size_t)r; }
+    return true;
+}
+// [a, b) of the two files are equal
+static bool same_range(int fa, int fb, uint64_t a, uint64_t b) {
+    std::vector<uint8_t> x(4 * kMiB), y(4 * kMiB);
+    for (uint64_t o = a; o < b; o += x.size()) {
+        const size_t n = (size_t)std::min<uint64_t>(x.size(), b - o);
+        x.resize(n); y.resize(n);
+        if (!get_at(fa, o, &x) || !get_at(fb, o, &y) || x != y) { printf("differs in [%llu, %llu)\n", (unsigned long long)o, (unsigned long long)(o + n)); return false; }
+    }
+    return true;
+}
+
+static int run_large(const std::string& dir) {
+    // the input: holes, and islands in the first blocks, either side of 2^32, at 3 GiB and over the tail
+    const std::string in = dir + "/big_in.bin";
+    const int ifd = open(in.c_str(), O_RDWR | O_CREAT | O_TRUNC, 0600);
+    CHECK(ifd >= 0 && ftruncate(ifd, (off_t)kBig) == 0);
+    const uint64_t at[][2] = {{0, 6 * kMiB}, {k4G - 5 * kMiB, 10 * kMiB}, {3ull << 30, 2 * kMiB + 4096}, {kBig - 2 * kMiB - 777, 2 * kMiB + 777}};
+    for (const auto& a : at) { std::vector<uint8_t> v(a[1]); island(&v, a[0], 1); CHECK(put_at(ifd, a[0], v)); }
+    const uint64_t r0 = 4 * kMiB, r1 = kBig - 4096 - 777;               // the long run: [4 MiB, the file's last 4873 bytes)
+    CHECK(r1 - r0 > k4G);
+    for (int rw_only = 0; rw_only < 2; rw_only++) {
+        const std::string out = dir + "/big_out" + std::to_string(rw_only) + ".bin";
+        const int ofd = open(out.c_str(), O_RDWR | O_CREAT | O_TRUNC, 0600);
+        CHECK(ofd >= 0 && ftruncate(ofd, (off_t)kBig) == 0);
+        // what the output holds outside the run, and must keep
+        std::vector<uint8_t> head(r0), tail(kBig - r1);
+        island(&head, 0, 2); island(&tail, r1, 2);
+        CHECK(put_at(ofd, 0, head) && put_at(ofd, r1, tail));
+        CHECK(copy_range(ifd, ofd, r0, r1 - r0, false, rw_only != 0, in) == VMIG_OK);
+        struct stat so;
+        CHECK(fstat(ofd, &so) == 0 && (uint64_t)so.st_size == kBig);
+        std::vector<uint8_t> h2(head.size()), t2(tail.size());
+        CHECK(get_at(ofd, 0, &h2) && h2 == head && get_at(ofd, r1, &t2) && t2 == tail);
+        CHECK(same_range(ifd, ofd, r0, r1));
+        // separate offsets, both above 2^32: input [2^32 + 1 MiB, +2 MiB + 5) to output [2^32 + 5 MiB + 4096, ...)
+        const uint64_t so_off = k4G + kMiB, do_off = k4G + 5 * kMiB + 4096, n = 2 * kMiB + 5;
+        CHECK(copy_range_at(ifd, so_off, ofd, do_off, n, false, rw_only != 0, in) == VMIG_OK);
+        std::vector<uint8_t> want(n), got(n);
+        island(&want, so_off, 1);
+        CHECK(get_at(ofd, do_off, &got) && got == want);
+        CHECK(same_range(ifd, ofd, k4G - 5 * kMiB, do_off) && same_range(ifd, ofd, do_off + n, r1));      // and nothing around it
+        CHECK(get_at(ofd, 0, &h2) && h2 == head);
+        // a range that ends past the input's end, above 2^32
+        CHECK(copy_range(ifd, ofd, kBig - 100, 200, false, rw_only != 0, in) == VMIG_ESRCCHANGED);
+        CHECK(fstat(ofd, &so) == 0 && (uint64_t)so.st_size == kBig);
+        close(ofd);
+        CHECK(unlink(out.c_str()) == 0);
+    }
+    close(ifd);
+    CHECK(unlink(in.c_str()) == 0);
+    printf("backfill large ok\n");
+    return 0;
+}
+
 int main(int argc, char** argv) {
     if (argc < 2) return 2;
+    if (std::string(argv[1]) == "--large") return argc == 3 ? run_large(argv[2]) : 2;
     for (int i = 1; i < argc; i++) if (run(argv[i])) return 1;
     printf("backfill unit ok\n");
     return 0;

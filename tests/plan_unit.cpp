@@ -6,7 +6,8 @@
 //     makes it untrusted and counted; a second link, a missing file or a record without identity is neither;
 //   - a base record that is no longer its file is counted for a same-path source file, one without identity is not;
 //   - prior hashes come from the prior record or the base record, valid only where the block lengths agree;
-//   - a cancel during the base check is VMIG_ECANCELED.
+//   - a cancel during the base check is VMIG_ECANCELED;
+//   - a span longer than 2^32 bytes keeps 64-bit offsets: every block once, at r * block_bytes, the short last block last.
 //   usage: plan_unit DIR
 #include "vmig_plan.h"
 #include "vmig_common.h"
@@ -105,6 +106,44 @@ static int block_order(const std::string& dir) {
         const BlockSpan& s = spans[ws[k].file];
         CHECK(got[k].file == s.file && got[k].file_off == ws[k].r * kBB && got[k].table_idx == s.first_block + ws[k].r);
         CHECK(got[k].len == std::min<uint64_t>(kBB, s.size - got[k].file_off));
+    }
+    return 0;
+}
+
+// One file of 2^32 + 9 MiB + 777 bytes among small ones, at 4 MiB blocks and at 1 MiB + 4096 (one block straddles 2^32)
+static int large_spans() {
+    const uint64_t kBig = (1ull << 32) + (9ull << 20) + 777;
+    for (const uint32_t bb : {4u << 20, (1u << 20) + 4096}) {
+        const uint64_t sizes[] = {3ull * bb + 5, kBig, 1, 2ull * bb};
+        std::vector<BlockSpan> spans;
+        std::vector<std::pair<uint32_t, uint64_t>> ids;
+        uint64_t fb = 0;
+        for (uint32_t u = 0; u < 4; u++) {
+            const uint64_t nb = sizes[u] / bb + (sizes[u] % bb != 0);
+            spans.push_back({u, sizes[u], fb, nb});
+            ids.push_back({u, nb});
+            fb += nb;
+        }
+        std::vector<BlockRef> got;
+        interleave_blocks(spans, bb, &got);
+        const std::vector<Want> w = round_robin(ids);
+        CHECK(got.size() == w.size() && got.size() == fb);
+        uint64_t next_r = 0, above = 0, straddle = 0, big_bytes = 0;       // of the big span
+        for (size_t k = 0; k < w.size(); k++) {
+            const BlockSpan& s = spans[w[k].file];
+            const uint64_t off = w[k].r * (uint64_t)bb;
+            const uint64_t len = w[k].r + 1 < s.n_blocks ? bb : s.size - off;
+            CHECK(got[k].file == s.file && got[k].file_off == off && got[k].len == len && got[k].table_idx == s.first_block + w[k].r);
+            if (s.file != 1) continue;
+            CHECK(w[k].r == next_r++);                                      // in order, each exactly once
+            above += off >= (1ull << 32);
+            straddle += off < (1ull << 32) && off + len > (1ull << 32);
+            big_bytes += len;
+            if (w[k].r + 1 == s.n_blocks) CHECK(got[k].len == kBig % bb && got[k].file_off + got[k].len == kBig);
+        }
+        CHECK(next_r == spans[1].n_blocks && big_bytes == kBig);
+        CHECK(above == spans[1].n_blocks - ((1ull << 32) + bb - 1) / bb && above >= 3);
+        CHECK(straddle == ((1ull << 32) % bb != 0));
     }
     return 0;
 }
@@ -212,7 +251,7 @@ static int trust(const std::string& dir) {
 
 int main(int argc, char** argv) {
     if (argc < 2) return 2;
-    if (block_order(argv[1]) || trust(argv[1])) return 1;
+    if (block_order(argv[1]) || large_spans() || trust(argv[1])) return 1;
     printf("plan unit ok\n");
     return 0;
 }

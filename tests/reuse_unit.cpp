@@ -5,6 +5,7 @@
 //     base run, else the first index entry; runs contiguous in both files are coalesced;
 //   * a short last block only matches a base block of exactly its length;
 //   * untrusted base files are not in the index;
+//   * a file longer than 2^32 bytes: runs longer than 2^32 bytes, and source and destination offsets above 2^32;
 //   * link_candidates: same path first, then table order; equal size and every hash;
 //   * copy_range_at puts [in_off, +len) of the input at [out_off, +len) of the output and nothing else, through
 //     copy_file_range and through the forced pread/pwrite fallback, and whole sectors into an O_DIRECT output.
@@ -139,6 +140,57 @@ static int planning() {
     return 0;
 }
 
+// A new file of 2^32 + 9 MiB + 777 bytes at 4 MiB blocks.  Base file 0 holds the same blocks at the same indices, base file 1
+// holds them three blocks further on, behind three blocks of its own.
+static int planning_large() {
+    const uint32_t bb = 4u << 20;
+    const uint64_t kBig = (1ull << 32) + (9ull << 20) + 777, k4G = 1ull << 32;
+    const uint64_t nb = (kBig + bb - 1) / bb, last_len = kBig - (nb - 1) * bb;
+    CHECK(nb == 1027 && last_len == (1u << 20) + 777);
+    std::vector<uint64_t> h(nb);
+    for (uint64_t r = 0; r < nb; r++) h[r] = 0x1000 + r;
+    BlockTable t; t.block_bytes = bb;
+    t.files.push_back({"huge.bin", kBig, 0, 100, 1});
+    t.hashes = h;
+    t.files.push_back({"moved.bin", kBig + 3ull * bb, nb, 101, 1});
+    for (uint64_t x : {0x1, 0x2, 0x3}) t.hashes.push_back(x);
+    t.hashes.insert(t.hashes.end(), h.begin(), h.end());
+    t.index["huge.bin"] = 0; t.index["moved.bin"] = 1;
+    BaseIndex both, moved;
+    both.build(t, {1, 1});
+    moved.build(t, {0, 1});
+    CHECK(both.block_len(0, nb - 1) == last_len && both.block_len(1, nb + 2) == last_len && both.block_len(0, nb) == 0);
+    CHECK(both.block_len(0, 1024) == bb && both.block_len(0, 1023) == bb);
+
+    std::vector<ReuseRun> runs;
+    std::vector<uint8_t> sk(nb, 1);
+    // only the last block was written: one run of more than 2^32 bytes from the same path
+    std::vector<uint64_t> nh = h;
+    nh[nb - 1] = 0x99; sk[nb - 1] = 0;
+    CHECK(plan_backfill(both, 0, kBig, bb, nh.data(), sk.data(), "huge.bin", &runs) == VMIG_OK);
+    CHECK(runs.size() == 1 && run_is(runs[0], 0, 0, 0, kBig - last_len) && runs[0].len > k4G);
+    // only the first block was written: the run starts at one block and ends at the file's size
+    nh = h; sk.assign(nb, 1);
+    nh[0] = 0x99; sk[0] = 0;
+    CHECK(plan_backfill(both, 0, kBig, bb, nh.data(), sk.data(), "huge.bin", &runs) == VMIG_OK);
+    CHECK(runs.size() == 1 && run_is(runs[0], 0, bb, bb, kBig - bb) && runs[0].dst_off + runs[0].len == kBig);
+    // no same-path record; the block after the one that starts at 2^32 was written: the content is found in the other
+    // file three blocks further on, and the second run has both offsets above 2^32
+    nh = h; sk.assign(nb, 1);
+    nh[1025] = 0x99; sk[1025] = 0;
+    CHECK(plan_backfill(moved, -1, kBig, bb, nh.data(), sk.data(), "renamed.bin", &runs) == VMIG_OK);
+    CHECK(runs.size() == 2 && run_is(runs[0], 1, 3ull * bb, 0, 1025ull * bb));
+    CHECK(run_is(runs[1], 1, 1029ull * bb, 1026ull * bb, kBig - 1026ull * bb));
+    CHECK(runs[1].src_off > k4G && runs[1].dst_off > k4G && runs[1].src_off != runs[1].dst_off && runs[0].len > k4G);
+    // the whole file elsewhere is a link candidate only at its own size
+    std::vector<uint32_t> c;
+    link_candidates(both, -1, kBig, bb, h.data(), &c, 16);
+    CHECK(c == std::vector<uint32_t>({0}));
+    link_candidates(both, -1, kBig - k4G, bb, h.data(), &c, 16);       // the size a 32-bit length would see
+    CHECK(c.empty());
+    return 0;
+}
+
 static std::vector<uint8_t> pattern(size_t n, uint32_t seed) {
     std::vector<uint8_t> v(n);
     uint32_t x = seed;
@@ -194,7 +246,7 @@ static int copies(const std::string& dir) {
 
 int main(int argc, char** argv) {
     if (argc < 2) return 2;
-    if (planning()) return 1;
+    if (planning() || planning_large()) return 1;
     for (int i = 1; i < argc; i++) if (copies(argv[i])) return 1;
     printf("reuse unit ok\n");
     return 0;

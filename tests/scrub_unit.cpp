@@ -4,7 +4,8 @@
 //   - the inode grouping maps the paths of one inode, in any version, to one block range;
 //   - report path escaping round-trips awkward names, and the report is sorted and written atomically;
 //   - a reader fed a descriptor whose reads fail records the inode as unreadable and returns success to the pipeline;
-//     an inode replaced since the walk is VMIG_ESRCCHANGED.
+//     an inode replaced since the walk is VMIG_ESRCCHANGED;
+//   - the reader takes blocks either side of offset 2^32 of a sparse file longer than that, and its short last block.
 //   usage: scrub_unit DIR
 #include "vmig_scrub.h"
 #include "vmig_common.h"
@@ -157,9 +158,54 @@ static int reader(const std::string& dir) {
     return 0;
 }
 
+// A sparse inode of 2^32 + 9 MiB + 777 bytes whose words name their own offsets around 2^32 and in the tail
+static int reader_large(const std::string& dir) {
+    const uint64_t kBig = (1ull << 32) + (9ull << 20) + 777, k4G = 1ull << 32;
+    const uint32_t bb = 4096;
+    const std::string root = dir + "/bigroot", path = root + "/huge";
+    mkdir(root.c_str(), 0755);
+    const int wfd = open(path.c_str(), O_WRONLY | O_CREAT | O_TRUNC, 0600);
+    CHECK(wfd >= 0 && ftruncate(wfd, (off_t)kBig) == 0);
+    const uint64_t last_off = kBig / bb * bb;
+    auto words = [](uint64_t off, size_t n) {
+        std::vector<uint8_t> v(n);
+        for (size_t i = 0; i < n; i++) { const uint64_t o = off + i, w = (o / 8) * 0x9E3779B97F4A7C15ull + 1; v[i] = (uint8_t)(w >> (8 * (o % 8))); }
+        return v;
+    };
+    const std::vector<uint8_t> mid = words(k4G - 2 * bb, 4 * bb), tail = words(last_off, kBig - last_off);
+    CHECK(pwrite(wfd, mid.data(), mid.size(), (off_t)(k4G - 2 * bb)) == (ssize_t)mid.size());
+    CHECK(pwrite(wfd, tail.data(), tail.size(), (off_t)last_off) == (ssize_t)tail.size());
+    CHECK(close(wfd) == 0);
+    struct stat s;
+    CHECK(stat(path.c_str(), &s) == 0 && (uint64_t)s.st_size == kBig);
+    const uint64_t nb = (kBig + bb - 1) / bb;
+    std::vector<ScrubInode> inodes = {{(uint64_t)s.st_dev, (uint64_t)s.st_ino, kBig, 0, nb, 0, "huge"}};
+    const int rfd = open(root.c_str(), O_RDONLY | O_DIRECTORY);
+    CHECK(rfd >= 0);
+    ScrubReader r;
+    r.root_fds = {rfd}; r.inodes = &inodes;
+    r.init();
+    std::vector<uint8_t> slot(bb);
+    for (const uint64_t off : {k4G - 2 * bb, k4G - bb, k4G, k4G + bb}) {
+        CHECK(r.read(0, off, bb, slot.data()) == VMIG_OK);
+        CHECK(slot == words(off, bb));
+    }
+    CHECK(r.read(0, 0, bb, slot.data()) == VMIG_OK && slot == std::vector<uint8_t>(bb, 0));          // a hole: not 2^32's bytes
+    CHECK(r.read(0, 3ull << 30, bb, slot.data()) == VMIG_OK && slot == std::vector<uint8_t>(bb, 0));
+    CHECK(kBig - last_off == 777);
+    CHECK(r.read(0, last_off, 777, slot.data()) == VMIG_OK);
+    CHECK(std::equal(tail.begin(), tail.end(), slot.begin()));
+    CHECK(!r.unreadable(0));
+    CHECK(r.read(0, last_off, bb, slot.data()) == VMIG_ESRCCHANGED);                                   // a whole block there is past the end
+    r.close_all();
+    close(rfd);
+    CHECK(unlink(path.c_str()) == 0);
+    return 0;
+}
+
 int main(int argc, char** argv) {
     if (argc < 2) return 2;
-    if (merge_and_group() || escaping(argv[1]) || reader(argv[1])) return 1;
+    if (merge_and_group() || escaping(argv[1]) || reader(argv[1]) || reader_large(argv[1])) return 1;
     printf("scrub unit ok\n");
     return 0;
 }

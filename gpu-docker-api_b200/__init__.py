@@ -48,6 +48,7 @@ EXPORTS = [
     "vmig_resident_set_prior", "vmig_resident_pass", "vmig_resident_results", "vmig_table_info_read",
     "vmig_table_hashes", "vmig_dir_size", "vmig_to_bytes", "vmig_datagen_files", "vmig_manifest", "vmig_link_probe", "vmig_thread_plan",
     "vmig_ctl_open", "vmig_ctl_cancel", "vmig_ctl_progress", "vmig_ctl_close", "vmig_scrub_store",
+    "vmig_retire_versions",
 ]
 SCRUB_KINDS = ("missing", "extra", "resized", "block", "hardlink", "unreadable", "table", "dir")
 
@@ -86,6 +87,14 @@ class SnapshotStats(C.Structure):
 class ScrubStats(C.Structure):
     _fields_ = [(n, C.c_uint64) for n in ("versions", "versions_damaged", "bytes_referenced", "bytes_unique", "files_damaged",
                                           "blocks_damaged", "files_unreadable")] + [("reserved", C.c_uint64 * 4)]
+
+    def as_dict(self) -> dict:
+        return {n: getattr(self, n) for n, _ in self._fields_ if n != "reserved"}
+
+
+class RetireStats(C.Structure):
+    _fields_ = [(n, C.c_uint64) for n in ("versions_retired", "entries_removed", "files_freed", "bytes_freed", "records_stale",
+                                          "records_restamped", "bytes_rehashed", "tables_rewritten")] + [("reserved", C.c_uint64 * 4)]
 
     def as_dict(self) -> dict:
         return {n: getattr(self, n) for n, _ in self._fields_ if n != "reserved"}
@@ -142,6 +151,8 @@ _sig = {
     "vmig_ctl_progress": (C.c_int, [C.c_uint32, C.POINTER(Progress)]), "vmig_ctl_close": (C.c_int, [C.c_uint32]),
     "vmig_scrub_store": (C.c_int, [C.c_uint32, C.POINTER(C.c_char_p), C.POINTER(C.c_char_p), C.c_char_p, C.POINTER(C.c_int32),
                                    C.POINTER(Opts), C.POINTER(Stats), C.POINTER(ScrubStats)]),
+    "vmig_retire_versions": (C.c_int, [C.c_uint32, C.POINTER(C.c_char_p), C.POINTER(C.c_char_p), C.c_uint32, C.POINTER(C.c_char_p),
+                                       C.POINTER(C.c_char_p), C.POINTER(Opts), C.POINTER(Stats), C.POINTER(RetireStats)]),
 }
 for _n, (_r, _a) in _sig.items():
     _f = getattr(_lib, _n)
@@ -394,6 +405,23 @@ def scrub_store(pairs, report=None, *, flags: int = 0, gpu_mask: int = 0, lanes_
             import shutil
             shutil.rmtree(tmpdir, ignore_errors=True)
     return {"verdicts": list(verdicts[:n]), "findings": findings, "stats": st.as_dict(), **ss.as_dict()}
+
+
+def retire_versions(retire_pairs, keep_pairs, *, flags: int = 0, gpu_mask: int = 0, lanes_per_gpu: int = 0,
+                    block_bytes: int = 0, ctl: Optional[Ctl] = None) -> dict:
+    """Remove the versions retire_pairs = [(snap_dir, snap_table), ...] of a snapshot store, then re-verify on the GPU and
+    re-record the records of the kept versions keep_pairs whose ctime the removal moved, so that the next incremental
+    snapshot still trusts them.  Returns the vmig_retire_stats fields plus the data pass's counters ("stats")."""
+    retire_pairs, keep_pairs = list(retire_pairs), list(keep_pairs)
+
+    def arr(pairs, i):
+        return (C.c_char_p * max(len(pairs), 1))(*[_b(p[i]) for p in pairs])
+    o = Opts(gpu_mask=gpu_mask, block_bytes=block_bytes, flags=flags, lanes_per_gpu=lanes_per_gpu, ctl=_ctl_id(ctl))
+    st, rs = Stats(), RetireStats()
+    _check(_lib.vmig_retire_versions(len(retire_pairs), arr(retire_pairs, 0), arr(retire_pairs, 1), len(keep_pairs),
+                                     arr(keep_pairs, 0), arr(keep_pairs, 1), C.byref(o), C.byref(st), C.byref(rs)),
+           f"vmig_retire_versions({len(retire_pairs)} retired, {len(keep_pairs)} kept)")
+    return {"stats": st.as_dict(), **rs.as_dict()}
 
 
 def hash_tree(src, out_table, *, gpu_mask: int = 0, block_bytes: int = 0) -> dict:

@@ -10,6 +10,7 @@
 #include "vmig_cufile.h"
 #include "vmig_reuse.h"
 #include "vmig_scrub.h"
+#include "vmig_retire.h"
 #include "vmig_plan.h"
 
 #include <fcntl.h>
@@ -883,6 +884,12 @@ int migrate_tree_impl(const char* src_dir, const char* dst_dir, const char* prio
     return call.finish(migrate_tree_body(call, src_dir, dst_dir, prior_path, out_path, o, stats_out, snap_path, snapshot));
 }
 
+// a is root or lies beneath it (both real paths)
+bool path_inside(const std::string& a, const std::string& root)
+{
+    return a == root || (a.size() > root.size() && a.compare(0, root.size(), root) == 0 && (root == "/" || a[root.size()] == '/'));
+}
+
 // vmig_snapshot_tree: a base directory equal to the destination, or either one inside the other, is refused -- a
 // link or backfill would read what the same call is writing
 int check_snapshot_paths(const char* dst_dir, const char* base_dir)
@@ -893,10 +900,7 @@ int check_snapshot_paths(const char* dst_dir, const char* base_dir)
     if (!b) { const int e = errno; free(d); return fail(VMIG_EIO, "realpath %s: %s", base_dir, errno_str(e).c_str()); }
     const std::string ds(d), bs(b);
     free(d); free(b);
-    auto inside = [](const std::string& a, const std::string& root) {
-        return a == root || (a.size() > root.size() && a.compare(0, root.size(), root) == 0 && (root == "/" || a[root.size()] == '/'));
-    };
-    if (inside(ds, bs) || inside(bs, ds))
+    if (path_inside(ds, bs) || path_inside(bs, ds))
         return fail(VMIG_EINVAL, "base_dir %s and dst_dir %s are the same directory or one is inside the other", bs.c_str(), ds.c_str());
     return VMIG_OK;
 }
@@ -1041,6 +1045,169 @@ int scrub_body(CallScope& call, uint32_t n, const char* const* dirs, const char*
     return VMIG_OK;
 }
 
+// ---------------------------------------------------------------------------------------------
+// vmig_retire_versions: the removal and the re-stamp plan are vmig_retire.cpp's; the re-verify is the scrub's data pass
+// over the stale records' inodes
+// The real path of p without following its last component (it may be a symlink, or missing): realpath of the parent
+// plus the name.  A parent that does not exist leaves p as given (nothing can be removed beneath it).
+int real_parent_path(const char* p, std::string* out)
+{
+    std::string s(p);
+    while (s.size() > 1 && s.back() == '/') s.pop_back();
+    const size_t slash = s.rfind('/');
+    const std::string parent = slash == std::string::npos ? "." : slash == 0 ? "/" : s.substr(0, slash);
+    const std::string base = slash == std::string::npos ? s : s.substr(slash + 1);
+    if (base.empty() || base == "." || base == ".." || base == "/") return fail(VMIG_EINVAL, "%s names no directory entry", p);
+    char* r = realpath(parent.c_str(), nullptr);
+    if (!r) {
+        if (errno != ENOENT) return fail(VMIG_EIO, "realpath %s: %s", parent.c_str(), errno_str(errno).c_str());
+        *out = s;
+        return VMIG_OK;
+    }
+    *out = std::string(r) + (strcmp(r, "/") ? "/" : "") + base;
+    free(r);
+    return VMIG_OK;
+}
+
+struct RetireArgs {
+    std::vector<std::string> retire_dirs, retire_tables, keep_dirs, keep_tables;   // real paths
+};
+
+// the refusals that touch nothing, before the call is attached
+int check_retire_args(uint32_t n_retire, const char* const* retire_dirs, const char* const* retire_tables, uint32_t n_keep,
+                      const char* const* keep_dirs, const char* const* keep_tables, RetireArgs* a)
+{
+    for (uint32_t i = 0; i < n_retire; i++) {
+        std::string d, t;
+        int rc = real_parent_path(retire_dirs[i], &d);
+        if (!rc) rc = real_parent_path(retire_tables[i], &t);
+        if (rc) return rc;
+        struct stat st;
+        if (lstat(d.c_str(), &st) == 0 && !S_ISDIR(st.st_mode))
+            return fail(VMIG_ENOTDIR, "retired version %s is not a directory (a symlink is not followed)", retire_dirs[i]);
+        a->retire_dirs.push_back(d); a->retire_tables.push_back(t);
+    }
+    for (uint32_t i = 0; i < n_keep; i++) {
+        char* r = realpath(keep_dirs[i], nullptr);
+        struct stat st;
+        if (!r || stat(r, &st) != 0 || !S_ISDIR(st.st_mode)) { free(r); return fail(VMIG_ENOTDIR, "kept version %s is not a directory", keep_dirs[i]); }
+        a->keep_dirs.push_back(r);
+        free(r);
+        std::string t;
+        const int rc = real_parent_path(keep_tables[i], &t);
+        if (rc) return rc;
+        a->keep_tables.push_back(t);
+    }
+    std::vector<std::string> all(a->retire_dirs);
+    all.insert(all.end(), a->keep_dirs.begin(), a->keep_dirs.end());
+    for (size_t i = 0; i < all.size(); i++)
+        for (size_t j = i + 1; j < all.size(); j++)
+            if (path_inside(all[i], all[j]) || path_inside(all[j], all[i]))
+                return fail(VMIG_EINVAL, "%s and %s are the same directory or one is inside the other", all[i].c_str(), all[j].c_str());
+    for (const std::string& t : a->retire_tables)
+        for (size_t k = 0; k < n_keep; k++)
+            if (t == a->keep_tables[k] || path_inside(t, a->keep_dirs[k]))
+                return fail(VMIG_EINVAL, "retired table %s is kept version %s's table or lies inside it", t.c_str(), a->keep_dirs[k].c_str());
+    for (const std::string& t : a->keep_tables)
+        for (const std::string& d : a->retire_dirs)
+            if (path_inside(t, d)) return fail(VMIG_EINVAL, "kept table %s lies inside retired version %s", t.c_str(), d.c_str());
+    return VMIG_OK;
+}
+
+int retire_body(CallScope& call, const RetireArgs& a, const vmig_opts& o, vmig_stats* stats_out, vmig_retire_stats* rs_out)
+{
+    CallCtl* ctl = call.ctl;
+    const std::atomic<int>* cancel = call.cancel();
+    vmig_stats st; memset(&st, 0, sizeof st);
+    vmig_retire_stats rs; memset(&rs, 0, sizeof rs);
+    const uint64_t t_begin = now_ns();
+    if (cancel->load()) return fail(VMIG_ECANCELED, "the control was cancelled before the call started");
+    const size_t n_keep = a.keep_dirs.size();
+    std::vector<BlockTable> tab(n_keep);
+    for (size_t k = 0; k < n_keep; k++) {
+        const int rc = load_table(a.keep_tables[k].c_str(), "kept", o.block_bytes, &tab[k]);
+        if (rc) return rc;
+    }
+    std::vector<DeviceInfo> devs;                    // no CPU fallback: the GPU is there before anything is removed
+    int rc = ctx_select(o.gpu_mask, &devs);
+    if (rc) return rc;
+
+    // ---- remove the retired versions, table first
+    call.phase(VMIG_PHASE_UNLINK);
+    uint64_t t0 = now_ns();
+    RemoveCount removed;
+    for (size_t i = 0; i < a.retire_dirs.size(); i++) {
+        rc = retire_remove(a.retire_dirs[i], a.retire_tables[i], &removed, cancel);
+        if (rc) return rc;
+        rs.versions_retired++;
+    }
+    rs.entries_removed = removed.entries; rs.files_freed = removed.files_freed; rs.bytes_freed = removed.bytes_freed;
+
+    // ---- the kept records whose ctime moved, grouped by inode
+    call.phase(VMIG_PHASE_WALK);
+    std::vector<int> root_fds(n_keep, -1);
+    auto close_roots = [&] { for (int& fd : root_fds) if (fd >= 0) { close(fd); fd = -1; } };
+    for (size_t k = 0; k < n_keep; k++) {
+        root_fds[k] = open(a.keep_dirs[k].c_str(), O_RDONLY | O_DIRECTORY | O_CLOEXEC);
+        if (root_fds[k] < 0) { const int e = errno; close_roots(); return fail(VMIG_ESRCCHANGED, "open %s: %s", a.keep_dirs[k].c_str(), errno_str(e).c_str()); }
+    }
+    std::vector<const BlockTable*> tabs;
+    for (const BlockTable& t : tab) tabs.push_back(&t);
+    std::vector<StaleRecord> stale;
+    std::vector<ScrubInode> inodes;
+    std::vector<uint32_t> inode_of;
+    rc = retire_find_stale(root_fds, tabs, &stale, cancel);
+    if (!rc) rc = retire_group(stale, tabs, o.block_bytes, &inodes, &inode_of);
+    if (rc) { close_roots(); return rc; }
+    st.ns_walk = now_ns() - t0;
+    t0 = now_ns();
+    uint64_t n_blocks = 0;
+    for (const ScrubInode& I : inodes) { rs.bytes_rehashed += I.size; n_blocks += I.n_blocks; }
+    rs.records_stale = stale.size();
+    ctl->bytes_total.store(rs.bytes_rehashed); ctl->blocks_total.store(n_blocks);
+    ScrubReader reader;
+    reader.root_fds = root_fds; reader.inodes = &inodes; reader.direct = (o.flags & VMIG_F_DIRECT_IO) != 0;
+    reader.init();
+    ScrubIO io; io.r = &reader; io.block_bytes = o.block_bytes;
+    std::vector<BlockSpan> spans;
+    for (uint32_t u = 0; u < inodes.size(); u++) spans.push_back({u, inodes[u].size, inodes[u].first_block, inodes[u].n_blocks});
+    std::vector<BlockRef> blocks; blocks.reserve(n_blocks);
+    interleave_blocks(spans, o.block_bytes, &blocks);
+    st.ns_plan = now_ns() - t0;
+
+    // ---- re-verify each stale inode once: K1 in hash-only mode, compared on the host
+    call.phase(VMIG_PHASE_DATA);
+    if (cancel->load()) { close_roots(); return fail(VMIG_ECANCELED, "before the data pass"); }
+    t0 = now_ns();
+    std::vector<uint64_t> hashes(n_blocks, 0);
+    rc = run_blocks(blocks, &io, false, true, o, hashes.data(), &st, ctl, false);
+    reader.close_all();
+    st.ns_data = now_ns() - t0;
+    if (rc) { close_roots(); return rc; }
+    std::vector<bool> unreadable(inodes.size());
+    for (uint32_t u = 0; u < inodes.size(); u++) unreadable[u] = reader.unreadable(u);
+    const std::vector<size_t> chosen = retire_decide(root_fds, tabs, stale, inodes, inode_of, hashes, unreadable);
+    close_roots();
+    rs.records_restamped = chosen.size();
+
+    // ---- rewrite each kept table that gained a verified identity
+    call.phase(VMIG_PHASE_TABLE);
+    t0 = now_ns();
+    for (uint32_t k = 0; k < n_keep; k++) {
+        if (!retire_patch(k, stale, chosen, inodes, inode_of, &tab[k])) continue;
+        rc = table_store(a.keep_tables[k], tab[k], cancel);
+        if (rc) return rc;
+        rs.tables_rewritten++;
+    }
+    st.ns_table = now_ns() - t0;
+    st.files_direct = reader.n_direct.load();
+    st.bytes_total = rs.bytes_rehashed; st.blocks_total = n_blocks; st.files = inodes.size();
+    st.ns_total = now_ns() - t_begin;
+    if (stats_out) *stats_out = st;
+    if (rs_out) *rs_out = rs;
+    return VMIG_OK;
+}
+
 }  // namespace
 
 // =============================================================================================
@@ -1175,6 +1342,30 @@ int vmig_scrub_store(uint32_t n, const char* const* snap_dirs, const char* const
     rc = call.attach(o.ctl);
     if (rc) return rc;
     return call.finish(scrub_body(call, n, snap_dirs, snap_tables, report_path, verdicts, o, stats, scrub_stats));
+}
+int vmig_retire_versions(uint32_t n_retire, const char* const* retire_dirs, const char* const* retire_tables,
+                         uint32_t n_keep, const char* const* keep_dirs, const char* const* keep_tables,
+                         const vmig_opts* opts, vmig_stats* stats, vmig_retire_stats* retire_stats)
+{
+    if (n_retire + (uint64_t)n_keep == 0) return fail(VMIG_EINVAL, "n_retire + n_keep == 0: no version to retire or keep");
+    if ((n_retire && (!retire_dirs || !retire_tables)) || (n_keep && (!keep_dirs || !keep_tables)))
+        return fail(VMIG_EINVAL, "retire_dirs / retire_tables / keep_dirs / keep_tables is NULL");
+    for (uint32_t i = 0; i < n_retire; i++)
+        if (!retire_dirs[i] || !*retire_dirs[i] || !retire_tables[i] || !*retire_tables[i]) return fail(VMIG_EINVAL, "retired version %u: dir or table is NULL/empty", i);
+    for (uint32_t i = 0; i < n_keep; i++)
+        if (!keep_dirs[i] || !*keep_dirs[i] || !keep_tables[i] || !*keep_tables[i]) return fail(VMIG_EINVAL, "kept version %u: dir or table is NULL/empty", i);
+    const vmig_opts o = norm_opts(opts);                     // VMIG_CUFILE=1 in the environment is refused too
+    const uint32_t allowed = VMIG_F_DIRECT_IO | VMIG_F_SKIP_HIDDEN_TOPDIRS;
+    if (o.flags & ~allowed) return fail(VMIG_EINVAL, "flags 0x%x: a retire takes only VMIG_F_DIRECT_IO and VMIG_F_SKIP_HIDDEN_TOPDIRS", o.flags & ~allowed);
+    int rc = check_block_bytes(o);
+    if (rc) return rc;
+    RetireArgs a;
+    rc = check_retire_args(n_retire, retire_dirs, retire_tables, n_keep, keep_dirs, keep_tables, &a);
+    if (rc) return rc;
+    CallScope call;
+    rc = call.attach(o.ctl);
+    if (rc) return rc;
+    return call.finish(retire_body(call, a, o, stats, retire_stats));
 }
 int vmig_copy_dir(const char* src_dir, const char* dst_dir) { return migrate_tree_impl(src_dir, dst_dir, nullptr, nullptr, nullptr, nullptr); }
 int vmig_move_dir(const char* src_dir, const char* dst_dir)

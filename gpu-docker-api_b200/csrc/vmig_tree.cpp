@@ -486,23 +486,43 @@ static int prune_cancelled(const std::atomic<int>* cancel, const char* name)
     return fail(VMIG_ECANCELED, "cancelled during prune, before %s", name);
 }
 
+int remove_contents(int fd, const char* name, const char* what, RemoveCount* n, const std::atomic<int>* cancel)
+{
+    DIR* d = fdopendir(fd);
+    if (!d) { close(fd); return fail(VMIG_EIO, "%s: fdopendir %s: %s", what, name, errno_str(errno).c_str()); }
+    int rc = VMIG_OK;
+    while (struct dirent* de = readdir(d)) {
+        if (!strcmp(de->d_name, ".") || !strcmp(de->d_name, "..")) continue;
+        if (cancel && cancel->load()) { rc = fail(VMIG_ECANCELED, "cancelled during %s, before %s", what, de->d_name); break; }
+        struct stat st;
+        if (fstatat(fd, de->d_name, &st, AT_SYMLINK_NOFOLLOW) != 0) continue;
+        if (S_ISDIR(st.st_mode)) {
+            const int sub = openat(fd, de->d_name, O_RDONLY | O_DIRECTORY | O_NOFOLLOW | O_CLOEXEC);
+            if (sub < 0) { rc = fail(VMIG_EIO, "%s: open %s: %s", what, de->d_name, errno_str(errno).c_str()); break; }
+            if ((rc = remove_contents(sub, de->d_name, what, n, cancel))) break;
+            if (unlinkat(fd, de->d_name, AT_REMOVEDIR) != 0 && errno != ENOENT) { rc = fail(VMIG_EIO, "%s: rmdir %s: %s", what, de->d_name, errno_str(errno).c_str()); break; }
+            n->entries++;
+        } else if (unlinkat(fd, de->d_name, 0) == 0) {
+            n->entries++;
+            if (S_ISREG(st.st_mode) && st.st_nlink == 1) { n->files_freed++; n->bytes_freed += (uint64_t)st.st_size; }
+        } else if (errno == ENOENT) {
+            n->entries++;
+        } else {
+            rc = fail(VMIG_EIO, "%s: unlink %s: %s", what, de->d_name, errno_str(errno).c_str());
+            break;
+        }
+    }
+    closedir(d);
+    return rc;
+}
+
 static int rm_tree_at(int dfd, const char* name, uint64_t* n, const std::atomic<int>* cancel)
 {
     int fd = openat(dfd, name, O_RDONLY | O_DIRECTORY | O_NOFOLLOW | O_CLOEXEC);
     if (fd < 0) return fail(VMIG_EIO, "prune: open %s: %s", name, errno_str(errno).c_str());
-    DIR* d = fdopendir(fd);
-    if (!d) { close(fd); return fail(VMIG_EIO, "prune: fdopendir %s: %s", name, errno_str(errno).c_str()); }
-    int rc = VMIG_OK;
-    while (struct dirent* de = readdir(d)) {
-        if (!strcmp(de->d_name, ".") || !strcmp(de->d_name, "..")) continue;
-        if ((rc = prune_cancelled(cancel, de->d_name))) break;
-        struct stat st;
-        if (fstatat(fd, de->d_name, &st, AT_SYMLINK_NOFOLLOW) != 0) continue;
-        if (S_ISDIR(st.st_mode)) { rc = rm_tree_at(fd, de->d_name, n, cancel); if (rc) break; }
-        else if (unlinkat(fd, de->d_name, 0) != 0 && errno != ENOENT) { rc = fail(VMIG_EIO, "prune: unlink %s: %s", de->d_name, errno_str(errno).c_str()); break; }
-        else (*n)++;
-    }
-    closedir(d);
+    RemoveCount c;
+    const int rc = remove_contents(fd, name, "prune", &c, cancel);
+    *n += c.entries;
     if (rc) return rc;
     if (unlinkat(dfd, name, AT_REMOVEDIR) != 0 && errno != ENOENT) return fail(VMIG_EIO, "prune: rmdir %s: %s", name, errno_str(errno).c_str());
     (*n)++;

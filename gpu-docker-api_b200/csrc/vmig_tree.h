@@ -87,6 +87,13 @@ int remove_source(const std::string& src_root, const Manifest& m);
 // handled by descriptor, symlinks are never followed.  dry_run only counts them (the verify pass uses that).
 int prune_extras(const std::string& dst_root, const Manifest& m, bool dry_run, uint64_t* n_extras,
                  const std::atomic<int>* cancel = nullptr);
+// What remove_contents removed: entries unlinked or rmdir'ed, and the regular files among them whose link count was 1
+// just before the unlink (their space is freed unless a descriptor still holds them).
+struct RemoveCount { uint64_t entries = 0, files_freed = 0, bytes_freed = 0; };
+// Remove everything beneath the open directory fd (consumed; `name` and `what` only word the errors), children first,
+// each entry by its parent's descriptor, never following a symlink.  The cancel check is per entry.  VMIG_F_PRUNE and
+// vmig_retire_versions both remove trees this way.
+int remove_contents(int fd, const char* name, const char* what, RemoveCount* n, const std::atomic<int>* cancel = nullptr);
 // Remove whatever sits at path so that `what` (named in the error) can be created there: a non-directory or an EMPTY
 // directory goes, as GNU tar replaces them; a non-empty directory is VMIG_EIO, as tar fails with "Cannot open: File
 // exists".  ENOENT is fine.  Every non-directory the engine creates goes through this.

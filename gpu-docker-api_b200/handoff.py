@@ -22,7 +22,7 @@ from typing import Callable, Optional
 import threading
 
 from . import (F_PRUNE, F_VERIFY, VMIG_ECANCELED, Ctl, GetContainerMergedLayer, GetVolumeMountPoint, VmigError, manifest,
-               migrate_tree, restore_tree, scrub_store, snapshot_tree)
+               migrate_tree, restore_tree, retire_versions, scrub_store, snapshot_tree)
 
 log = logging.getLogger("vmig.handoff")
 _root: dict = {"cwd": None}
@@ -120,6 +120,17 @@ def ScrubReplicaSet(rs: str) -> dict:
     inode the versions share once.  The versions are the merges/<rs>/<rs>-<k> that hold diff/ (the rule of baseVersion;
     a missing blocks.vmig is that version's VMIG_ETABLE).  Returns {"verdicts": {version name: VMIG_* verdict},
     "report": merges/<rs>/scrub.txt}, the report listing every damaged path and block."""
+    names = snapshotVersions(rs)
+    report = versionDir(rs + "-0").parent / "scrub.txt"
+    if not names:
+        return {"verdicts": {}, "report": None}
+    out = scrub_store([snapshotPaths(name) for name in names], report)
+    return {"verdicts": dict(zip(names, out["verdicts"])), "report": report}
+
+
+def snapshotVersions(rs: str) -> list:
+    """The snapshot versions of the ReplicaSet, oldest first: every merges/<rs>/<rs>-<k> that holds diff/ (with or
+    without blocks.vmig).  A version directory without diff/ holds only the running container's table (HandoffCopy)."""
     parent = versionDir(rs + "-0").parent
     found = []
     for d in (parent.iterdir() if parent.is_dir() else ()):
@@ -129,12 +140,28 @@ def ScrubReplicaSet(rs: str) -> dict:
         if (d / "diff").is_dir():
             found.append((int(k), d.name))
     found.sort()
-    names = [name for _, name in found]
-    report = parent / "scrub.txt"
+    return [name for _, name in found]
+
+
+def RetireVersions(rs: str, keep: int) -> dict:
+    """N1: keep the newest `keep` snapshots of the ReplicaSet and remove the older ones (vmig_retire_versions), then remove
+    each emptied merges/<rs>/<rs>-<k>.  Unlike rm -rf, the kept versions' tables stay trusted: the records whose ctime
+    the removal moved are re-verified on the GPU and re-recorded, so the next SnapshotVersionIncremental still links
+    every unchanged file.  A version directory without diff/ is never touched.  Returns {"retired": [version names],
+    "kept": [version names]} plus the counters of retire_versions."""
+    if keep < 1:
+        raise ValueError(f"keep must be at least 1, not {keep}")
+    names = snapshotVersions(rs)
     if not names:
-        return {"verdicts": {}, "report": None}
-    out = scrub_store([snapshotPaths(name) for name in names], report)
-    return {"verdicts": dict(zip(names, out["verdicts"])), "report": report}
+        return {"retired": [], "kept": []}
+    retired, kept = names[:-keep], names[-keep:]
+    out = retire_versions([snapshotPaths(name) for name in retired], [snapshotPaths(name) for name in kept])
+    for name in retired:
+        try:
+            versionDir(name).rmdir()
+        except OSError:             # something else lives there too: the directory stays
+            pass
+    return {"retired": retired, "kept": kept, **out}
 
 
 def RollbackFromSnapshot(targetCtrVersionName: str, newContainer: str, seedTable=None) -> dict:

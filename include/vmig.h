@@ -294,6 +294,66 @@ int vmig_scrub_store(uint32_t n, const char* const* snap_dirs, const char* const
                      const vmig_opts* opts /*nullable*/, vmig_stats* stats /*nullable*/,
                      vmig_scrub_stats* scrub_stats /*nullable*/);
 
+/* Retirement of old versions of a snapshot store: what vmig_retire_versions removed and re-recorded. */
+typedef struct vmig_retire_stats {
+    uint64_t versions_retired;             /* retired snapshot directories gone at the end (already missing counts)   */
+    uint64_t entries_removed;              /* directory entries this call unlinked or rmdir'ed under them             */
+    uint64_t files_freed, bytes_freed;     /* regular files whose link count was 1 when this call unlinked them        */
+    uint64_t records_stale;                /* kept-table records found stale after the removal                        */
+    uint64_t records_restamped;            /* of those: re-verified on the GPU and re-recorded                        */
+    uint64_t bytes_rehashed;               /* distinct inodes read through the GPU to do so                           */
+    uint64_t tables_rewritten;
+    uint64_t reserved[4];
+} vmig_retire_stats;
+
+/* Remove the n_retire versions retire_dirs[i] (with their tables retire_tables[i]) of a snapshot store, and keep the
+ * n_keep versions keep_dirs[i] / keep_tables[i] usable as bases for the next incremental snapshot.
+ * Unlinking one hard link of an inode moves the inode's ctime, so removing a version by hand (rm -rf) leaves stale the
+ * kept tables' records of nearly every file it shared with them: the next vmig_snapshot_tree no longer trusts them and
+ * copies those files in full.  This call removes the versions, then re-verifies exactly the records whose identity went
+ * stale and re-records them.
+ *   - Refusals that touch nothing: VMIG_EINVAL for n_retire + n_keep == 0, a NULL array or entry, flags other than
+ *     VMIG_F_DIRECT_IO | VMIG_F_SKIP_HIDDEN_TOPDIRS, bad block_bytes, any two directories of the call that are the same
+ *     or one inside the other (compared by real path), a retired table that is a kept table or lies inside a kept
+ *     directory, and a kept table that lies inside a retired directory.  VMIG_ENOTDIR: a retired directory that exists
+ *     but is not a directory (a symlink included: it is never followed), or a kept directory that is missing or not a
+ *     directory.  A control cancelled before the call starts: VMIG_ECANCELED.  VMIG_ETABLE: a kept table that does not
+ *     load (formats 01 and 02) or whose block_bytes differs from the call's.  VMIG_ENOGPU, checked after the tables.
+ *   - Removal (phase UNLINK), one retired version at a time: first its table is unlinked, so a half-removed version is
+ *     never a base or a restore source again; then its tree, children first, each entry by its parent's descriptor,
+ *     never following a symlink (as VMIG_F_PRUNE removes); last the directory itself.  A missing table or directory is
+ *     not an error, so re-running a call that failed part way finishes the job.  files_freed / bytes_freed count the
+ *     regular files whose st_nlink was 1 just before this call unlinked them: a link held anywhere else keeps its
+ *     inode and is not counted.
+ *   - Stale records (phase WALK): every record of every kept table that carries an identity (ino != 0) is opened
+ *     beneath its version's directory (no symlink followed) and fstat'ed.  It is stale when the file is still a regular
+ *     file with the recorded inode and size but another ctime.  The rule does not depend on what this call unlinked: it
+ *     also covers a re-run after a failed or cancelled call, and records earlier snapshots' links had already left
+ *     stale.  Records of another inode or size, format-01 records and records without an identity are left alone.
+ *   - Re-verify (phase DATA): the stale records are grouped by (st_dev, st_ino) and each distinct inode is read once
+ *     through the block pipeline in hash-only mode, as vmig_scrub_store reads (lanes, GPUs and VMIG_F_DIRECT_IO as
+ *     there).  Then each inode is fstat'ed again.  A record is re-stamped with the identity seen before the read only
+ *     when every one of its blocks hashes as its table says and the ctime did not move during the read.  Any other
+ *     stale record stays exactly as it was (a mismatch, an unreadable inode, a ctime that moved): untrusted, which is
+ *     the state rm -rf leaves.  An inode that is no longer the one planned (other inode, type or size, or shorter than
+ *     its blocks) fails the call with VMIG_ESRCCHANGED.
+ *   - Tables (phase TABLE): each kept table with at least one re-stamped record is rewritten atomically (tmp, fsync,
+ *     rename).  Only the ino / ctime_ns fields of re-stamped records change; every other byte is identical.  No other
+ *     table is touched.
+ *   - Failure and cancel: a cancel is honoured in every phase (per removed entry, in the data pass, before each table
+ *     rename).  After any failure each kept table is byte-identical to what it was or already fully rewritten, never
+ *     half written, and never carries an identity that was not verified; a retired version is intact, gone, or half
+ *     removed with its table already gone.  The call never writes into a kept version's tree: nothing there moves
+ *     except the ctimes its own unlinks move.
+ *   - Control: phases UNLINK, WALK, DATA, TABLE, DONE; bytes_total is the stale bytes to re-hash.  stats (nullable):
+ *     the vmig_stats of the data pass.  retire_stats (nullable): the counters above, written on success.
+ * A snapshot that uses a kept version as its base must not run concurrently with a retire of the same store: if one
+ * does, it fails with VMIG_ESRCCHANGED or copies more than it needed to, but it is never wrong. */
+int vmig_retire_versions(uint32_t n_retire, const char* const* retire_dirs, const char* const* retire_tables,
+                         uint32_t n_keep, const char* const* keep_dirs, const char* const* keep_tables,
+                         const vmig_opts* opts /*nullable*/, vmig_stats* stats /*nullable*/,
+                         vmig_retire_stats* retire_stats /*nullable*/);
+
 /* utils.CopyDir(src, dest) (reference utils/copy.go:21-27) == vmig_migrate_tree with defaults. */
 int vmig_copy_dir(const char* src_dir, const char* dst_dir);
 
@@ -316,7 +376,7 @@ void vmig_host_free(void* p);
 
 /* ---- cancellation and progress ------------------------------------------------------------------
  * A control is a numeric id (cgo passes it in vmig_opts.ctl without any pointer rules).  It serves the entry points
- * that take vmig_opts: vmig_migrate_tree, vmig_restore_tree, vmig_snapshot_tree, vmig_scrub_store and vmig_migrate_buffer (a caller that
+ * that take vmig_opts: vmig_migrate_tree, vmig_restore_tree, vmig_snapshot_tree, vmig_scrub_store, vmig_retire_versions and vmig_migrate_buffer (a caller that
  * wants to cancel a copy or a move calls vmig_migrate_tree with the flags vmig_copy_dir / vmig_move_dir use).  One
  * control serves one call at a time: attaching it to a second concurrent call fails with VMIG_EINVAL.  The engine has
  * no deadline of its own; a deadline is the caller's timer calling vmig_ctl_cancel.
@@ -348,7 +408,8 @@ void vmig_host_free(void* p);
 #define VMIG_PHASE_META    4u   /* empty files, symlinks, specials, hard links, directory metadata          */
 #define VMIG_PHASE_PRUNE   5u   /* VMIG_F_PRUNE: removing destination entries the source does not have      */
 #define VMIG_PHASE_TABLE   6u   /* writing out_table                                                        */
-#define VMIG_PHASE_UNLINK  7u   /* VMIG_F_MOVE_SRC: unlinking the source; a cancel is no longer honoured    */
+#define VMIG_PHASE_UNLINK  7u   /* VMIG_F_MOVE_SRC: unlinking the source; a cancel is no longer honoured.
+                                   vmig_retire_versions: removing retired versions; a cancel is honoured   */
 #define VMIG_PHASE_DONE    8u   /* the call returned VMIG_OK                                                */
 
 typedef struct vmig_progress {

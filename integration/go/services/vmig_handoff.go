@@ -30,6 +30,7 @@ import (
 	"github.com/ngaut/log"
 	"github.com/pkg/errors"
 
+	vmap "github.com/mayooot/gpu-docker-api/internal/version"
 	"github.com/mayooot/gpu-docker-api/utils"
 )
 
@@ -119,6 +120,30 @@ func SnapshotVersionIncremental(ctrVersionName string) error {
 // a missing blocks.vmig is that version's VMIG_ETABLE).  It returns each version's verdict by name and the report,
 // merges/<rs>/scrub.txt, which lists every damaged path and block.
 func ScrubReplicaSet(rs string) (map[string]int, string, error) {
+	names := snapshotVersions(rs)
+	report := filepath.Join(filepath.Dir(versionDir(rs+"-0")), "scrub.txt")
+	if len(names) == 0 {
+		return map[string]int{}, "", nil
+	}
+	dirs, tables := make([]string, len(names)), make([]string, len(names))
+	for i, name := range names {
+		dirs[i], tables[i] = snapshotPaths(name)
+	}
+	verdicts, err := utils.ScrubSnapshots(dirs, tables, report)
+	if err != nil {
+		return nil, "", errors.WithMessagef(err, "scrub of %s failed", rs)
+	}
+	out := make(map[string]int, len(names))
+	for i, name := range names {
+		out[name] = verdicts[i]
+	}
+	return out, report, nil
+}
+
+// snapshotVersions lists the snapshot versions of the ReplicaSet, oldest first: every merges/<rs>/<rs>-<k> that holds
+// diff/ (with or without blocks.vmig).  A version directory without diff/ holds only the running container's table
+// (HandoffCopy).
+func snapshotVersions(rs string) []string {
 	parent := filepath.Dir(versionDir(rs + "-0"))
 	entries, _ := os.ReadDir(parent)
 	type version struct {
@@ -137,23 +162,49 @@ func ScrubReplicaSet(rs string) (map[string]int, string, error) {
 		found = append(found, version{k, e.Name()})
 	}
 	sort.Slice(found, func(i, j int) bool { return found[i].k < found[j].k })
-	report := filepath.Join(parent, "scrub.txt")
-	if len(found) == 0 {
-		return map[string]int{}, "", nil
-	}
-	dirs, tables := make([]string, len(found)), make([]string, len(found))
+	names := make([]string, len(found))
 	for i, v := range found {
-		dirs[i], tables[i] = snapshotPaths(v.name)
+		names[i] = v.name
 	}
-	verdicts, err := utils.ScrubSnapshots(dirs, tables, report)
-	if err != nil {
-		return nil, "", errors.WithMessagef(err, "scrub of %s failed", rs)
+	return names
+}
+
+// N1 -- RetireVersions keeps the newest `keep` snapshots of the ReplicaSet and removes the older ones
+// (utils.RetireSnapshots), then removes each emptied merges/<rs>/<rs>-<k> and drops it from ContainerMergeMap.  Unlike
+// rm -rf, the kept versions' tables stay trusted: the records whose ctime the removal moved are re-verified on the GPU
+// and re-recorded, so the next SnapshotVersionIncremental still links every unchanged file.  A version directory
+// without diff/ is never touched.  It returns the retired and the kept version names.
+func RetireVersions(rs string, keep int) (retired, kept []string, err error) {
+	if keep < 1 {
+		return nil, nil, errors.Errorf("RetireVersions: keep must be at least 1, not %d", keep)
 	}
-	out := make(map[string]int, len(found))
-	for i, v := range found {
-		out[v.name] = verdicts[i]
+	names := snapshotVersions(rs)
+	if len(names) == 0 {
+		return nil, nil, nil
 	}
-	return out, report, nil
+	cut := len(names) - keep
+	if cut < 0 {
+		cut = 0
+	}
+	retired, kept = names[:cut], names[cut:]
+	var rdirs, rtables, kdirs, ktables []string
+	for _, name := range retired {
+		d, t := snapshotPaths(name)
+		rdirs, rtables = append(rdirs, d), append(rtables, t)
+	}
+	for _, name := range kept {
+		d, t := snapshotPaths(name)
+		kdirs, ktables = append(kdirs, d), append(ktables, t)
+	}
+	if err := utils.RetireSnapshots(rdirs, rtables, kdirs, ktables); err != nil {
+		return nil, nil, errors.WithMessagef(err, "retire of %s failed", rs)
+	}
+	for _, name := range retired {
+		_ = os.Remove(versionDir(name)) // something else lives there too: the directory stays
+		k, _ := strconv.ParseInt(name[strings.LastIndex(name, "-")+1:], 10, 64)
+		vmap.ContainerMergeMap.Remove(k)
+	}
+	return retired, kept, nil
 }
 
 // N1 -- RollbackFromSnapshot fills newContainer's layer with version `target` of the ReplicaSet.  The new

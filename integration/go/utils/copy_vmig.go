@@ -185,6 +185,75 @@ func ScrubSnapshotsContext(ctx context.Context, snapDirs, snapTables []string, r
 	return out, nil
 }
 
+// RetireSnapshots removes the snapshots retireDirs[i] with their tables retireTables[i] and keeps keepDirs[i] /
+// keepTables[i] usable as bases (vmig_retire_versions): each retired table goes first, then its tree, never following
+// a symlink; then the kept tables' records whose ctime the removal moved are re-verified on the GPU and re-recorded.
+// Nothing is written under a kept snapshot.  A snapshot based on a kept one must not run at the same time.
+func RetireSnapshots(retireDirs, retireTables, keepDirs, keepTables []string) error {
+	return RetireSnapshotsContext(context.Background(), retireDirs, retireTables, keepDirs, keepTables)
+}
+
+// RetireSnapshotsContext is RetireSnapshots that stops when ctx is done (see CopyDirDiffContext).  A retired snapshot is
+// then intact, gone, or half removed without its table; each kept table is as it was or fully rewritten.
+func RetireSnapshotsContext(ctx context.Context, retireDirs, retireTables, keepDirs, keepTables []string) error {
+	nr, nk := len(retireDirs), len(keepDirs)
+	if nr+nk == 0 || len(retireTables) != nr || len(keepTables) != nk {
+		return errors.Errorf("RetireSnapshots: %d/%d retired directories/tables, %d/%d kept", nr, len(retireTables), nk, len(keepTables))
+	}
+	ptrSize := C.size_t(unsafe.Sizeof((*C.char)(nil)))
+	carr := func(v []string) **C.char { // C memory: cgo forbids Go pointers to Go pointers
+		if len(v) == 0 {
+			return nil
+		}
+		a := (*[1 << 28]*C.char)(C.malloc(C.size_t(len(v)) * ptrSize))[:len(v):len(v)]
+		for i, s := range v {
+			a[i] = C.CString(s)
+		}
+		return &a[0]
+	}
+	cfree := func(p **C.char, n int) {
+		if p == nil {
+			return
+		}
+		a := (*[1 << 28]*C.char)(unsafe.Pointer(p))[:n:n]
+		for i := range a {
+			C.free(unsafe.Pointer(a[i]))
+		}
+		C.free(unsafe.Pointer(p))
+	}
+	crd, crt, ckd, ckt := carr(retireDirs), carr(retireTables), carr(keepDirs), carr(keepTables)
+	defer cfree(crd, nr)
+	defer cfree(crt, nr)
+	defer cfree(ckd, nk)
+	defer cfree(ckt, nk)
+	var st C.vmig_stats
+	var rs C.vmig_retire_stats
+	var o C.vmig_opts
+	var id C.uint32_t
+	if err := lockedCall("vmig_ctl_open", func() C.int { return C.vmig_ctl_open(&id) }); err != nil {
+		return err
+	}
+	defer C.vmig_ctl_close(id)
+	stop := context.AfterFunc(ctx, func() { C.vmig_ctl_cancel(id) })
+	defer stop()
+	o.ctl = id
+	var rc C.int
+	err := lockedCall("vmig_retire_versions", func() C.int {
+		rc = C.vmig_retire_versions(C.uint32_t(nr), crd, crt, C.uint32_t(nk), ckd, ckt, &o, &st, &rs)
+		return rc
+	})
+	if rc == C.VMIG_ECANCELED && ctx.Err() != nil {
+		return fmt.Errorf("%w: %v", ctx.Err(), err)
+	}
+	if err != nil {
+		return err
+	}
+	log.Infof("vmig: retired %d snapshots (%d entries, %d bytes freed); %d kept records stale, %d re-stamped after re-hashing %d bytes, %d tables rewritten",
+		uint64(rs.versions_retired), uint64(rs.entries_removed), uint64(rs.bytes_freed), uint64(rs.records_stale),
+		uint64(rs.records_restamped), uint64(rs.bytes_rehashed), uint64(rs.tables_rewritten))
+	return nil
+}
+
 func copyDirDiff(ctx context.Context, src, dest, priorTable, outTable string, flags C.uint32_t) error {
 	return runDiff(ctx, "vmig_migrate_tree", src, dest, priorTable, outTable, flags,
 		func(cs, cd, cp, co *C.char, o *C.vmig_opts, st *C.vmig_stats, _ *C.vmig_snapshot_stats) C.int {

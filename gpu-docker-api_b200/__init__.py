@@ -48,7 +48,7 @@ EXPORTS = [
     "vmig_resident_set_prior", "vmig_resident_pass", "vmig_resident_results", "vmig_table_info_read",
     "vmig_table_hashes", "vmig_dir_size", "vmig_to_bytes", "vmig_datagen_files", "vmig_manifest", "vmig_link_probe", "vmig_thread_plan",
     "vmig_ctl_open", "vmig_ctl_cancel", "vmig_ctl_progress", "vmig_ctl_close", "vmig_scrub_store",
-    "vmig_retire_versions",
+    "vmig_retire_versions", "vmig_restore_paths",
 ]
 SCRUB_KINDS = ("missing", "extra", "resized", "block", "hardlink", "unreadable", "table", "dir")
 
@@ -153,6 +153,8 @@ _sig = {
                                    C.POINTER(Opts), C.POINTER(Stats), C.POINTER(ScrubStats)]),
     "vmig_retire_versions": (C.c_int, [C.c_uint32, C.POINTER(C.c_char_p), C.POINTER(C.c_char_p), C.c_uint32, C.POINTER(C.c_char_p),
                                        C.POINTER(C.c_char_p), C.POINTER(Opts), C.POINTER(Stats), C.POINTER(RetireStats)]),
+    "vmig_restore_paths": (C.c_int, [C.c_char_p, C.c_char_p, C.c_char_p, C.c_uint32, C.POINTER(C.c_char_p), C.c_char_p,
+                                     C.POINTER(Opts), C.POINTER(Stats)]),
 }
 for _n, (_r, _a) in _sig.items():
     _f = getattr(_lib, _n)
@@ -200,7 +202,7 @@ def _b(p) -> Optional[bytes]:
 
 
 class Ctl:
-    """A call control (vmig_ctl_*): pass it as ``ctl=`` to migrate_tree, restore_tree, snapshot_tree or migrate_buffer,
+    """A call control (vmig_ctl_*): pass it as ``ctl=`` to migrate_tree, restore_tree, restore_paths, snapshot_tree or migrate_buffer,
     then cancel() from any thread (the call raises VmigError(VMIG_ECANCELED)) or read progress() while it runs.  ctypes
     releases the GIL during the call.  One control serves one call at a time; a deadline is a threading.Timer."""
 
@@ -321,6 +323,21 @@ def restore_tree(snap, snap_table, dst, prior_table=None, out_table=None, *, gpu
     st = Stats()
     _check(_lib.vmig_restore_tree(_b(snap), _b(snap_table), _b(dst), _b(prior_table), _b(out_table), C.byref(o),
                                   C.byref(st)), f"vmig_restore_tree({snap} -> {dst})")
+    return st.as_dict()
+
+
+def restore_paths(snap, snap_table, dst, paths, prior_table=None, *, flags: int = 0, gpu_mask: int = 0,
+                  lanes_per_gpu: int = 0, block_bytes: int = 0, ctl: Optional[Ctl] = None) -> dict:
+    """Restore the chosen entries `paths` (str or bytes, relative to `snap`, named as the table names them) of a snapshot
+    into `dst`, each regular file checked against `snap_table` as restore_tree checks it; nothing in `dst` outside those
+    entries and their parent directories is touched.  prior_table: `dst`'s own table (unchanged blocks are not written);
+    no table is written.  Returns the migrate_tree counters of the selection."""
+    paths = list(paths)
+    arr = (C.c_char_p * max(len(paths), 1))(*[_b(p) for p in paths])
+    o = Opts(gpu_mask=gpu_mask, block_bytes=block_bytes, flags=flags, lanes_per_gpu=lanes_per_gpu, ctl=_ctl_id(ctl))
+    st = Stats()
+    _check(_lib.vmig_restore_paths(_b(snap), _b(snap_table), _b(dst), len(paths), arr, _b(prior_table), C.byref(o),
+                                   C.byref(st)), f"vmig_restore_paths({snap} -> {dst}, {len(paths)} paths)")
     return st.as_dict()
 
 

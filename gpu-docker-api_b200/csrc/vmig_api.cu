@@ -12,6 +12,7 @@
 #include "vmig_scrub.h"
 #include "vmig_retire.h"
 #include "vmig_plan.h"
+#include "vmig_select.h"
 
 #include <fcntl.h>
 #include <unistd.h>
@@ -621,7 +622,8 @@ struct SnapshotArgs {
 
 // After the data pass: hard-linked paths take their primary's hashes, empty regular files are created, then the rest of
 // the tree's metadata is replayed (vmig_tree.h replay_metadata).
-int meta_pass(CallScope& call, FileIO& io, const std::vector<uint64_t>& expect, std::vector<uint64_t>* hashes, vmig_stats* st)
+int meta_pass(CallScope& call, FileIO& io, const std::vector<uint64_t>& expect, std::vector<uint64_t>* hashes, vmig_stats* st,
+              size_t first_dir)
 {
     const Manifest& man = *io.m;
     const std::atomic<int>* cancel = call.cancel();
@@ -655,11 +657,12 @@ int meta_pass(CallScope& call, FileIO& io, const std::vector<uint64_t>& expect, 
         close(fd);
         if (rc) return rc;
     }
-    return replay_metadata(io.dst_root, man, io.pol, &st->symlinks, &st->hardlinks, &st->specials, cancel);
+    return replay_metadata(io.dst_root, man, io.pol, &st->symlinks, &st->hardlinks, &st->specials, cancel, first_dir);
 }
 
 // VMIG_F_VERIFY: read the destination back through the same GPU path (hash only) and compare block tables
-int verify_pass(CallScope& call, const vmig_opts& o, const FileIO& io, const std::vector<uint64_t>& hashes, vmig_stats* st)
+int verify_pass(CallScope& call, const vmig_opts& o, const FileIO& io, const std::vector<uint64_t>& hashes, vmig_stats* st,
+                const std::vector<std::string>* prune_scope)
 {
     const Manifest& man = *io.m;
     FileIO vio;
@@ -684,7 +687,7 @@ int verify_pass(CallScope& call, const vmig_opts& o, const FileIO& io, const std
                         (unsigned long long)vh[b.table_idx], (unsigned long long)hashes[b.table_idx]);
     if (o.flags & VMIG_F_PRUNE) {               // the destination's entry set must now equal the source's
         uint64_t extras = 0;
-        rc = prune_extras(io.dst_root, man, true, &extras, call.cancel()); if (rc) return rc;
+        rc = prune_extras(io.dst_root, man, true, &extras, call.cancel(), prune_scope); if (rc) return rc;
         if (extras) return fail(VMIG_EVERIFY, "verify: %llu destination entries are not in the source after pruning", (unsigned long long)extras);
     }
     return VMIG_OK;
@@ -739,14 +742,130 @@ int finish_move(CallScope& call, const std::string& src, const std::string& dst,
     return remove_source(src, man);
 }
 
-// snap_path non-null: vmig_restore_tree -- src_dir must match that block table (match_table before anything touches the
-// destination, every block's hash in the hash-waiter, hard-linked paths before metadata replay).
+// a is root or lies beneath it (both real paths)
+bool path_inside(const std::string& a, const std::string& root)
+{
+    return a == root || (a.size() > root.size() && a.compare(0, root.size(), root) == 0 && (root == "/" || a[root.size()] == '/'));
+}
+
+// The passes of a tree call after its manifest is walked and checked: plan, (prune), data, metadata, (verify), table,
+// (move).  expect: the snapshot table's hashes in the manifest's block order (a checked restore), else empty.
 // snapshot non-null: vmig_snapshot_tree -- unchanged files and blocks come from the base (FileIO::finish_from_base).
-int migrate_tree_body(CallScope& call, const char* src_dir, const char* dst_dir, const char* prior_path, const char* out_path,
-                      const vmig_opts& o, vmig_stats* stats_out, const char* snap_path, const SnapshotArgs* snapshot)
+// sel non-null: vmig_restore_paths -- the parent chains are made real directories before the plan looks at the
+// destination, the prune and its verify stay beneath the chosen directories, the destination root's metadata ("."
+// here stands for it) is not replayed, and no table is written.
+int tree_passes(CallScope& call, const std::string& src, const std::string& dst, Manifest& man, const std::vector<uint64_t>& expect,
+                const char* prior_path, const char* out_path, const vmig_opts& o, vmig_stats& st, const SnapshotArgs* snapshot,
+                Selection* sel, uint64_t t_begin, vmig_stats* stats_out)
 {
     const char* base_dir = snapshot ? snapshot->base_dir : nullptr;
     const char* base_path = snapshot ? snapshot->base_table : nullptr;
+    const std::atomic<int>* cancel = call.cancel();
+    const bool hash_only = (o.flags & VMIG_F_HASH_ONLY) != 0;
+    int rc;
+    uint64_t t0 = now_ns();
+    BlockTable prior;
+    const bool has_prior = prior_path && *prior_path && !hash_only;
+    if (has_prior && (rc = load_table(prior_path, "prior", o.block_bytes, &prior))) return rc;
+    BlockTable base; bool has_base = false;
+    if (base_path) {
+        rc = load_table(base_path, "base", o.block_bytes, &base);
+        if (rc) return rc;
+        // a hard link cannot cross devices, and a base on another filesystem shares nothing with the snapshot
+        struct stat bst, dst_st;
+        has_base = stat(base_dir, &bst) == 0 && stat(dst.c_str(), &dst_st) == 0 && bst.st_dev == dst_st.st_dev;
+    }
+    if (sel) {
+        if (cancel->load()) return fail(VMIG_ECANCELED, "before the destination's parent directories were made");
+        rc = prepare_parents(dst, sel, cancel);
+        if (rc) return rc;
+    }
+    FileIO io;
+    io.src_root = src; io.dst_root = dst; io.pol = default_meta_policy(o.flags); io.hash_only = hash_only;
+    io.block_bytes = o.block_bytes;
+    io.corrupt_block = env_long("VMIG_CORRUPT_BLOCK", -1);
+    io.direct = (o.flags & VMIG_F_DIRECT_IO) != 0;
+    io.cufile = (o.flags & VMIG_F_CUFILE) != 0;
+    io.cancel = cancel;
+    if (io.cufile) { rc = cufile_open(); if (rc) return rc; }
+    rc = io.open_root(); if (rc) return rc;
+    TreePlan plan;
+    rc = plan_tree(man, o.block_bytes, dst, has_prior ? &prior : nullptr, has_base ? base_dir : "", has_base ? &base : nullptr, cancel, &plan);
+    if (rc) return rc;
+    st.files_untrusted = plan.files_untrusted;
+    io.init_files(man, plan);
+    std::vector<uint64_t> hashes(man.n_blocks, 0);
+    if (has_base) { io.base_root = base_dir; io.bidx.build(base, plan.base_trusted); io.hashes = hashes.data(); }
+    // skip mode whenever the base can supply a block, also when no source path has a same-path record (a layer whose
+    // files were all moved): without it the submitter streams every block back with its hash (DESIGN.md §3)
+    const bool skip_mode = has_prior || plan.any_base || !io.bidx.empty();
+    if (plan.any_base || !io.bidx.empty()) io.skipped.assign(man.n_blocks, 0);
+    st.ns_plan += now_ns() - t0;
+    const std::vector<std::string>* prune_scope = sel ? &sel->chosen_dirs : nullptr;
+
+    // VMIG_F_PRUNE runs first: what it removes is by definition not in the source, a directory sitting where the source
+    // now has a file (or the reverse) is out of the way before anything is created, and the directory mtimes restored
+    // at the end are not disturbed by unlinks
+    if ((o.flags & VMIG_F_PRUNE) && !hash_only) {
+        call.phase(VMIG_PHASE_PRUNE);
+        rc = prune_extras(dst, man, false, &st.pruned, cancel, prune_scope);
+        if (rc) return rc;
+    }
+    call.phase(VMIG_PHASE_DATA);
+    if (cancel->load()) return fail(VMIG_ECANCELED, "before the destination's directories were made");
+    if (!hash_only) { rc = make_dirs(dst, man); if (rc) return rc; }
+
+    t0 = now_ns();
+    rc = run_blocks(plan.blocks, &io, skip_mode, hash_only, o, hashes.data(), &st, call.ctl, false, expect.empty() ? nullptr : expect.data());
+    st.ns_data = now_ns() - t0;
+    if (rc) { std::string keep = last_error_cstr(); io.close_all(man.files.size()); set_last_error_str(keep); return rc; }
+
+    t0 = now_ns();
+    call.phase(VMIG_PHASE_META);
+    rc = meta_pass(call, io, expect, &hashes, &st, sel ? 1 : 0);
+    if (rc) return rc;
+    st.ns_meta = now_ns() - t0;
+
+    if ((o.flags & VMIG_F_VERIFY) && !hash_only) {
+        call.phase(VMIG_PHASE_VERIFY);
+        rc = verify_pass(call, o, io, hashes, &st, prune_scope);
+        if (rc) return rc;
+    }
+
+    if (!sel) {
+        t0 = now_ns();
+        call.phase(VMIG_PHASE_TABLE);
+        rc = write_table(io, snapshot != nullptr, out_path, hashes, cancel);
+        if (rc) return rc;
+        st.ns_table = now_ns() - t0;
+    }
+
+    if ((o.flags & VMIG_F_MOVE_SRC) && !hash_only) {
+        rc = finish_move(call, src, dst, man, out_path);
+        if (rc) return rc;
+    }
+
+    st.files_direct = io.n_direct.load();
+    st.bytes_total = man.bytes_total; st.blocks_total = man.n_blocks;
+    st.files = man.files.size(); st.dirs = man.dirs.size() - (sel ? 1 : 0);
+    st.ns_total = now_ns() - t_begin;
+    if (stats_out) *stats_out = st;
+    if (snapshot && snapshot->out) {
+        vmig_snapshot_stats ss; memset(&ss, 0, sizeof ss);
+        ss.files_base_untrusted = plan.files_base_untrusted;
+        ss.files_linked = io.n_linked.load(); ss.bytes_linked = io.b_linked.load();
+        ss.files_backfilled = io.n_backfilled.load(); ss.bytes_backfilled = io.b_backfilled.load();
+        *snapshot->out = ss;
+    }
+    return VMIG_OK;
+}
+
+// snap_path non-null: vmig_restore_tree -- src_dir must match that block table (match_table before anything touches the
+// destination, every block's hash in the hash-waiter, hard-linked paths before metadata replay).
+// snapshot non-null: vmig_snapshot_tree (tree_passes).
+int migrate_tree_body(CallScope& call, const char* src_dir, const char* dst_dir, const char* prior_path, const char* out_path,
+                      const vmig_opts& o, vmig_stats* stats_out, const char* snap_path, const SnapshotArgs* snapshot)
+{
     const std::atomic<int>* cancel = call.cancel();
     vmig_stats st; memset(&st, 0, sizeof st);
     const uint64_t t_begin = now_ns();
@@ -785,91 +904,66 @@ int migrate_tree_body(CallScope& call, const char* src_dir, const char* dst_dir,
         if (!rc) rc = match_table(man, snap, &expect);
         if (rc) return rc;
     }
-    BlockTable prior;
-    const bool has_prior = prior_path && *prior_path && !hash_only;
-    if (has_prior && (rc = load_table(prior_path, "prior", o.block_bytes, &prior))) return rc;
-    BlockTable base; bool has_base = false;
-    if (base_path) {
-        rc = load_table(base_path, "base", o.block_bytes, &base);
-        if (rc) return rc;
-        // a hard link cannot cross devices, and a base on another filesystem shares nothing with the snapshot
-        struct stat bst, dst_st;
-        has_base = stat(base_dir, &bst) == 0 && stat(dst.c_str(), &dst_st) == 0 && bst.st_dev == dst_st.st_dev;
-    }
-    FileIO io;
-    io.src_root = src; io.dst_root = dst; io.pol = default_meta_policy(o.flags); io.hash_only = hash_only;
-    io.block_bytes = o.block_bytes;
-    io.corrupt_block = env_long("VMIG_CORRUPT_BLOCK", -1);
-    io.direct = (o.flags & VMIG_F_DIRECT_IO) != 0;
-    io.cufile = (o.flags & VMIG_F_CUFILE) != 0;
-    io.cancel = cancel;
-    if (io.cufile) { rc = cufile_open(); if (rc) return rc; }
-    rc = io.open_root(); if (rc) return rc;
-    TreePlan plan;
-    rc = plan_tree(man, o.block_bytes, dst, has_prior ? &prior : nullptr, has_base ? base_dir : "", has_base ? &base : nullptr, cancel, &plan);
-    if (rc) return rc;
-    st.files_untrusted = plan.files_untrusted;
-    io.init_files(man, plan);
-    std::vector<uint64_t> hashes(man.n_blocks, 0);
-    if (has_base) { io.base_root = base_dir; io.bidx.build(base, plan.base_trusted); io.hashes = hashes.data(); }
-    // skip mode whenever the base can supply a block, also when no source path has a same-path record (a layer whose
-    // files were all moved): without it the submitter streams every block back with its hash (DESIGN.md §3)
-    const bool skip_mode = has_prior || plan.any_base || !io.bidx.empty();
-    if (plan.any_base || !io.bidx.empty()) io.skipped.assign(man.n_blocks, 0);
     st.ns_plan = now_ns() - t0;
+    return tree_passes(call, src, dst, man, expect, prior_path, out_path, o, st, snapshot, nullptr, t_begin, stats_out);
+}
 
-    // VMIG_F_PRUNE runs first: what it removes is by definition not in the source, a directory sitting where the source
-    // now has a file (or the reverse) is out of the way before anything is created, and the directory mtimes restored
-    // at the end are not disturbed by unlinks
-    if ((o.flags & VMIG_F_PRUNE) && !hash_only) {
-        call.phase(VMIG_PHASE_PRUNE);
-        rc = prune_extras(dst, man, false, &st.pruned, cancel);
-        if (rc) return rc;
-    }
-    call.phase(VMIG_PHASE_DATA);
-    if (cancel->load()) return fail(VMIG_ECANCELED, "before the destination's directories were made");
-    if (!hash_only) { rc = make_dirs(dst, man); if (rc) return rc; }
-
-    t0 = now_ns();
-    rc = run_blocks(plan.blocks, &io, skip_mode, hash_only, o, hashes.data(), &st, call.ctl, false, expect.empty() ? nullptr : expect.data());
-    st.ns_data = now_ns() - t0;
-    if (rc) { std::string keep = last_error_cstr(); io.close_all(man.files.size()); set_last_error_str(keep); return rc; }
-
-    t0 = now_ns();
-    call.phase(VMIG_PHASE_META);
-    rc = meta_pass(call, io, expect, &hashes, &st);
+// vmig_restore_paths: the chosen entries of a snapshot, checked against the part of its table they cover (DESIGN.md §6)
+int restore_paths_body(CallScope& call, const char* snap_dir, const char* snap_table, const char* dst_dir,
+                       const std::vector<std::string>& paths, const char* prior_path, const vmig_opts& o, vmig_stats* stats_out)
+{
+    const std::atomic<int>* cancel = call.cancel();
+    vmig_stats st; memset(&st, 0, sizeof st);
+    const uint64_t t_begin = now_ns();
+    const std::string src(snap_dir), dst(dst_dir);
+    struct stat sst;
+    if (stat(src.c_str(), &sst) != 0) return fail(VMIG_EIO, "stat %s: %s", src.c_str(), errno_str(errno).c_str());
+    if (!S_ISDIR(sst.st_mode)) return fail(VMIG_ENOTDIR, "%s is not a directory", src.c_str());
+    if (stat(dst.c_str(), &sst) != 0) return fail(VMIG_EIO, "stat %s: %s", dst.c_str(), errno_str(errno).c_str());
+    if (!S_ISDIR(sst.st_mode)) return fail(VMIG_ENOTDIR, "%s is not a directory", dst.c_str());
+    if (cancel->load()) return fail(VMIG_ECANCELED, "the control was cancelled before the call started");
+    std::vector<DeviceInfo> devs;                    // no CPU fallback: the GPU is there before anything is touched
+    int rc = ctx_select(o.gpu_mask, &devs);
     if (rc) return rc;
-    st.ns_meta = now_ns() - t0;
 
-    if ((o.flags & VMIG_F_VERIFY) && !hash_only) {
-        call.phase(VMIG_PHASE_VERIFY);
-        rc = verify_pass(call, o, io, hashes, &st);
-        if (rc) return rc;
-    }
+    uint64_t t0 = now_ns();
+    call.phase(VMIG_PHASE_WALK);
+    Selection sel;
+    rc = select_walk(src, paths, o.block_bytes, (o.flags & VMIG_F_SKIP_HIDDEN_TOPDIRS) != 0, &sel, cancel);
+    if (rc) return rc;
+    st.ns_walk = now_ns() - t0;
+    call.ctl->bytes_total.store(sel.man.bytes_total); call.ctl->blocks_total.store(sel.man.n_blocks);
 
     t0 = now_ns();
-    call.phase(VMIG_PHASE_TABLE);
-    rc = write_table(io, snapshot != nullptr, out_path, hashes, cancel);
+    BlockTable snap;
+    rc = load_table(snap_table, "snapshot", o.block_bytes, &snap);
     if (rc) return rc;
-    st.ns_table = now_ns() - t0;
-
-    if ((o.flags & VMIG_F_MOVE_SRC) && !hash_only) {
-        rc = finish_move(call, src, dst, man, out_path);
-        if (rc) return rc;
+    for (const std::string& p : sel.not_found) {
+        BlockTable under;
+        table_subset(snap, {p}, &under);
+        if (!under.files.empty())
+            return fail(VMIG_ECORRUPT, "%s is in the block table but not in the snapshot (missing)", under.files[0].rel.c_str());
+        return fail(VMIG_EINVAL, "%s is not in the snapshot", p.c_str());
     }
+    BlockTable part;                                 // records outside the selection are not looked at
+    table_subset(snap, sel.paths, &part);
+    std::vector<uint64_t> expect;
+    rc = match_table(sel.man, part, &expect);
+    if (rc) return rc;
+    st.ns_plan = now_ns() - t0;
+    return tree_passes(call, src, dst, sel.man, expect, prior_path, nullptr, o, st, nullptr, &sel, t_begin, stats_out);
+}
 
-    st.files_direct = io.n_direct.load();
-    st.bytes_total = man.bytes_total; st.blocks_total = man.n_blocks;
-    st.files = man.files.size(); st.dirs = man.dirs.size();
-    st.ns_total = now_ns() - t_begin;
-    if (stats_out) *stats_out = st;
-    if (snapshot && snapshot->out) {
-        vmig_snapshot_stats ss; memset(&ss, 0, sizeof ss);
-        ss.files_base_untrusted = plan.files_base_untrusted;
-        ss.files_linked = io.n_linked.load(); ss.bytes_linked = io.b_linked.load();
-        ss.files_backfilled = io.n_backfilled.load(); ss.bytes_backfilled = io.b_backfilled.load();
-        *snapshot->out = ss;
-    }
+// snap_dir and dst_dir the same directory or one inside the other (real paths); a path that does not resolve is left to
+// the call's own stat
+int check_restore_paths_dirs(const char* snap_dir, const char* dst_dir)
+{
+    char* a = realpath(snap_dir, nullptr);
+    char* b = realpath(dst_dir, nullptr);
+    const bool overlap = a && b && (path_inside(a, b) || path_inside(b, a));
+    const std::string as(a ? a : ""), bs(b ? b : "");
+    free(a); free(b);
+    if (overlap) return fail(VMIG_EINVAL, "snap_dir %s and dst_dir %s are the same directory or one is inside the other", as.c_str(), bs.c_str());
     return VMIG_OK;
 }
 
@@ -882,12 +976,6 @@ int migrate_tree_impl(const char* src_dir, const char* dst_dir, const char* prio
     const int rc = call.attach(o.ctl);
     if (rc) return rc;
     return call.finish(migrate_tree_body(call, src_dir, dst_dir, prior_path, out_path, o, stats_out, snap_path, snapshot));
-}
-
-// a is root or lies beneath it (both real paths)
-bool path_inside(const std::string& a, const std::string& root)
-{
-    return a == root || (a.size() > root.size() && a.compare(0, root.size(), root) == 0 && (root == "/" || a[root.size()] == '/'));
 }
 
 // vmig_snapshot_tree: a base directory equal to the destination, or either one inside the other, is refused -- a
@@ -1309,6 +1397,27 @@ int vmig_restore_tree(const char* snap_dir, const char* snap_table, const char* 
     if (!snap_table || !*snap_table) return fail(VMIG_EINVAL, "snap_table is NULL/empty: a snapshot is only restored against its block table");
     if (opts && (opts->flags & VMIG_F_MOVE_SRC)) return fail(VMIG_EINVAL, "VMIG_F_MOVE_SRC: a restore never consumes the snapshot");
     return migrate_tree_impl(snap_dir, dst_dir, prior_table, out_table, opts, stats, snap_table);
+}
+int vmig_restore_paths(const char* snap_dir, const char* snap_table, const char* dst_dir, uint32_t n_paths,
+                       const char* const* paths, const char* prior_table, const vmig_opts* opts, vmig_stats* stats)
+{
+    std::vector<std::string> sorted;
+    int rc = select_check_paths(n_paths, paths, &sorted);
+    if (rc) return rc;
+    if (!snap_table || !*snap_table) return fail(VMIG_EINVAL, "snap_table is NULL/empty: a snapshot is only restored against its block table");
+    if (!snap_dir || !*snap_dir) return fail(VMIG_EINVAL, "snap_dir is NULL/empty");
+    if (!dst_dir || !*dst_dir) return fail(VMIG_EINVAL, "dst_dir is NULL/empty");
+    const vmig_opts o = norm_opts(opts);                     // VMIG_CUFILE=1 in the environment is refused too
+    if (o.flags & VMIG_F_MOVE_SRC) return fail(VMIG_EINVAL, "VMIG_F_MOVE_SRC: a restore never consumes the snapshot");
+    if (o.flags & VMIG_F_HASH_ONLY) return fail(VMIG_EINVAL, "VMIG_F_HASH_ONLY: a partial restore writes its destination (vmig_scrub_store checks a version)");
+    if (o.flags & VMIG_F_CUFILE) return fail(VMIG_EINVAL, "VMIG_F_CUFILE: not supported for a partial restore");
+    rc = check_block_bytes(o);
+    if (!rc) rc = check_restore_paths_dirs(snap_dir, dst_dir);
+    if (rc) return rc;
+    CallScope call;
+    rc = call.attach(o.ctl);
+    if (rc) return rc;
+    return call.finish(restore_paths_body(call, snap_dir, snap_table, dst_dir, sorted, prior_table, o, stats));
 }
 int vmig_snapshot_tree(const char* src_dir, const char* dst_dir, const char* base_dir, const char* base_table,
                        const char* out_table, const vmig_opts* opts, vmig_stats* stats, vmig_snapshot_stats* snap_stats)

@@ -70,6 +70,49 @@ int open_beneath_walk(int root_fd, const std::string& rel, int flags, int* out_f
     }
 }
 
+int manifest_add(int dfd, const std::string& name, const std::string& rel, const struct stat& st, uint32_t block_bytes, Manifest* m)
+{
+    Entry e;
+    e.rel = rel;
+    e.mode = st.st_mode; e.uid = st.st_uid; e.gid = st.st_gid; e.mtime = st.st_mtim; e.atime = st.st_atim;
+    switch (st.st_mode & S_IFMT) {
+    case S_IFDIR:
+        e.type = kDir; m->dirs.push_back(e);
+        break;
+    case S_IFREG: {
+        e.type = kFile; e.size = (uint64_t)st.st_size;
+        e.n_blocks = (e.size + block_bytes - 1) / block_bytes;
+        e.dev = (uint64_t)st.st_dev; e.ino = (uint64_t)st.st_ino;
+        if (st.st_nlink > 1) e.target = inode_key(e.dev, e.ino);    // resolved to an index by finish_manifest
+        m->files.push_back(e);
+        break;
+    }
+    case S_IFLNK: {
+        e.type = kSymlink;
+        std::string buf((size_t)st.st_size + 256, '\0');
+        ssize_t k = readlinkat(dfd, name.c_str(), &buf[0], buf.size());
+        if (k < 0) return fail(VMIG_EIO, "readlink %s: %s", e.rel.c_str(), errno_str(errno).c_str());
+        buf.resize((size_t)k); e.target = buf;
+        m->symlinks.push_back(e);
+        break;
+    }
+    case S_IFCHR: case S_IFBLK: case S_IFIFO:
+        e.type = kSpecial; e.rdev = st.st_rdev; m->specials.push_back(e);
+        break;
+    case S_IFSOCK:
+        m->sockets_skipped++;        // GNU tar: "socket ignored"
+        break;
+    default: break;
+    }
+    return VMIG_OK;
+}
+
+std::string inode_key(uint64_t dev, uint64_t ino)
+{
+    char key[48]; snprintf(key, sizeof key, "%llx:%llx", (unsigned long long)dev, (unsigned long long)ino);
+    return key;
+}
+
 // dfd: open descriptor of the directory `rel`; consumed (closed) by this call.
 // defer_subdirs != nullptr: do not descend; list the sub-directories (name, rel) for the caller to walk (in parallel).
 static int walk_dir(int dfd, const std::string& rel, uint32_t block_bytes, bool skip_hidden_topdirs,
@@ -99,42 +142,11 @@ static int walk_dir(int dfd, const std::string& rel, uint32_t block_bytes, bool 
             const int e = errno; close(dfd_dup);
             return fail(VMIG_EIO, "lstat %s/%s: %s", rel.c_str(), n.c_str(), errno_str(e).c_str());
         }
-        Entry e;
-        e.rel = rel == "." ? n : rel + "/" + n;
-        e.mode = st.st_mode; e.uid = st.st_uid; e.gid = st.st_gid; e.mtime = st.st_mtim; e.atime = st.st_atim;
-        switch (st.st_mode & S_IFMT) {
-        case S_IFDIR:
-            if (skip_hidden_topdirs && depth == 0 && n[0] == '.') continue;   // `mv /root/src/*` misses these
-            e.type = kDir; m->dirs.push_back(e); subdirs.push_back({n, e.rel});
-            break;
-        case S_IFREG: {
-            e.type = kFile; e.size = (uint64_t)st.st_size;
-            e.n_blocks = (e.size + block_bytes - 1) / block_bytes;
-            e.dev = (uint64_t)st.st_dev; e.ino = (uint64_t)st.st_ino;
-            if (st.st_nlink > 1) {                   // group key (device:inode); resolved to an index after sorting
-                char key[48]; snprintf(key, sizeof key, "%llx:%llx", (unsigned long long)st.st_dev, (unsigned long long)st.st_ino);
-                e.target = key;
-            }
-            m->files.push_back(e);
-            break;
-        }
-        case S_IFLNK: {
-            e.type = kSymlink;
-            std::string buf((size_t)st.st_size + 256, '\0');
-            ssize_t k = readlinkat(dfd_dup, n.c_str(), &buf[0], buf.size());
-            if (k < 0) { const int er = errno; close(dfd_dup); return fail(VMIG_EIO, "readlink %s: %s", e.rel.c_str(), errno_str(er).c_str()); }
-            buf.resize((size_t)k); e.target = buf;
-            m->symlinks.push_back(e);
-            break;
-        }
-        case S_IFCHR: case S_IFBLK: case S_IFIFO:
-            e.type = kSpecial; e.rdev = st.st_rdev; m->specials.push_back(e);
-            break;
-        case S_IFSOCK:
-            m->sockets_skipped++;        // GNU tar: "socket ignored"
-            break;
-        default: break;
-        }
+        if (S_ISDIR(st.st_mode) && skip_hidden_topdirs && depth == 0 && n[0] == '.') continue;   // `mv /root/src/*` misses these
+        const std::string erel = rel == "." ? n : rel + "/" + n;
+        const int rc = manifest_add(dfd_dup, n, erel, st, block_bytes, m);
+        if (rc) { close(dfd_dup); return rc; }
+        if (S_ISDIR(st.st_mode)) subdirs.push_back({n, erel});
     }
     if (defer_subdirs) { *defer_subdirs = subdirs; close(dfd_dup); return VMIG_OK; }
     for (const auto& sd : subdirs) {
@@ -206,6 +218,12 @@ int walk_tree(const std::string& src_root, uint32_t block_bytes, bool skip_hidde
         }
     } else if (rfd2 >= 0) close(rfd2);
 
+    finish_manifest(m);
+    return VMIG_OK;
+}
+
+void finish_manifest(Manifest* m)
+{
     std::sort(m->files.begin(), m->files.end(), [](const Entry& a, const Entry& b) { return a.rel < b.rel; });
     // resolve hard links to indices; the primary of a group is its bytewise-smallest path
     // (a group with a single member inside the tree is just a regular file)
@@ -224,9 +242,9 @@ int walk_tree(const std::string& src_root, uint32_t block_bytes, bool skip_hidde
         e.target.clear();
     }
     uint64_t fb = 0;
+    m->bytes_total = 0;
     for (auto& e : m->files) { e.first_block = fb; fb += e.n_blocks; m->bytes_total += e.size; }
     m->n_blocks = fb;
-    return VMIG_OK;
 }
 
 MetaPolicy default_meta_policy(uint32_t flags)
@@ -381,7 +399,8 @@ int apply_file_meta(int fd, const std::string& path, const Entry& e, const MetaP
 }
 
 int replay_metadata(const std::string& dst_root, const Manifest& m, const MetaPolicy& pol,
-                    uint64_t* n_symlinks, uint64_t* n_hardlinks, uint64_t* n_specials, const std::atomic<int>* cancel)
+                    uint64_t* n_symlinks, uint64_t* n_hardlinks, uint64_t* n_specials, const std::atomic<int>* cancel,
+                    size_t first_dir)
 {
     size_t steps = 0;
     auto stop = [&](const std::string& rel) {
@@ -423,7 +442,7 @@ int replay_metadata(const std::string& dst_root, const Manifest& m, const MetaPo
         if (n_hardlinks) (*n_hardlinks)++;
     }
     if (!pol.no_metadata) {
-        for (size_t i = m.dirs.size(); i-- > 0;) {     // children before parents
+        for (size_t i = m.dirs.size(); i-- > first_dir;) {     // children before parents
             const Entry& e = m.dirs[i];
             if (int rc = stop(e.rel)) return rc;
             const std::string p = pjoin(dst_root, e.rel);
@@ -559,7 +578,8 @@ static int prune_dir(int dfd, const std::string& prefix, const std::unordered_se
     return rc;
 }
 
-int prune_extras(const std::string& dst_root, const Manifest& m, bool dry_run, uint64_t* n_extras, const std::atomic<int>* cancel)
+int prune_extras(const std::string& dst_root, const Manifest& m, bool dry_run, uint64_t* n_extras, const std::atomic<int>* cancel,
+                 const std::vector<std::string>* scope)
 {
     std::unordered_set<std::string> keep_dirs, keep_other;
     keep_dirs.reserve(m.dirs.size() * 2); keep_other.reserve((m.files.size() + m.symlinks.size() + m.specials.size()) * 2);
@@ -568,6 +588,19 @@ int prune_extras(const std::string& dst_root, const Manifest& m, bool dry_run, u
     for (auto& e : m.symlinks) keep_other.insert(e.rel);
     for (auto& e : m.specials) keep_other.insert(e.rel);
     *n_extras = 0;
+    if (scope) {
+        for (const std::string& rel : *scope) {
+            // a chosen directory that is not a real directory in the destination holds nothing to prune: the data pass
+            // replaces it (a symlink there is removed, never followed)
+            const std::string p = pjoin(dst_root, rel);
+            const int fd = open(p.c_str(), O_RDONLY | O_DIRECTORY | O_NOFOLLOW | O_CLOEXEC);
+            if (fd < 0 && (errno == ENOENT || errno == ENOTDIR || errno == ELOOP)) continue;
+            if (fd < 0) return fail(VMIG_EIO, "prune: open %s: %s", p.c_str(), errno_str(errno).c_str());
+            const int rc = prune_dir(fd, rel, keep_dirs, keep_other, dry_run, n_extras, cancel);
+            if (rc) return rc;
+        }
+        return VMIG_OK;
+    }
     int fd = open(dst_root.c_str(), O_RDONLY | O_DIRECTORY | O_CLOEXEC);
     if (fd < 0) return fail(VMIG_EIO, "prune: open %s: %s", dst_root.c_str(), errno_str(errno).c_str());
     return prune_dir(fd, "", keep_dirs, keep_other, dry_run, n_extras, cancel);

@@ -59,6 +59,13 @@ int open_beneath_walk(int root_fd, const std::string& rel, int flags, int* out_f
 // Walk src_root.  skip_hidden_topdirs reproduces `mv /root/src/*` (reference utils/copy.go:116).
 int walk_tree(const std::string& src_root, uint32_t block_bytes, bool skip_hidden_topdirs, Manifest* out,
               const std::atomic<int>* cancel = nullptr);
+// The walk's entry for `name` in the open directory dfd, lstat'ed as st, appended to m under `rel` (a socket is only
+// counted).  A regular file with more than one link carries its inode_key until finish_manifest groups it.
+int manifest_add(int dfd, const std::string& name, const std::string& rel, const struct stat& st, uint32_t block_bytes, Manifest* m);
+std::string inode_key(uint64_t dev, uint64_t ino);
+// Sort m's files bytewise, resolve the inode keys to hardlink_of (the group's smallest path is its primary) and lay the
+// blocks out in that order (first_block, n_blocks, bytes_total).
+void finish_manifest(Manifest* m);
 
 struct MetaPolicy {
     bool is_root;        // euid == 0: chown + exact modes (tar -p --same-owner defaults for root)
@@ -74,8 +81,10 @@ int make_dirs(const std::string& dst_root, const Manifest& m);
 // Symlinks, specials, hard links and empty regular files; then directory metadata bottom-up.  Checks cancel every
 // kMetaCheckEvery entries.
 static constexpr size_t kMetaCheckEvery = 1024;
+// Directory metadata is replayed for m.dirs[first_dir..] only (vmig_restore_paths leaves the destination root alone).
 int replay_metadata(const std::string& dst_root, const Manifest& m, const MetaPolicy& pol,
-                    uint64_t* n_symlinks, uint64_t* n_hardlinks, uint64_t* n_specials, const std::atomic<int>* cancel = nullptr);
+                    uint64_t* n_symlinks, uint64_t* n_hardlinks, uint64_t* n_specials, const std::atomic<int>* cancel = nullptr,
+                    size_t first_dir = 0);
 // True if the open file already carries the owner/mode/mtime apply_file_meta would give it (then it is left alone: a
 // diff pass that skips every block of a file must not move its ctime, the block table identifies files by it).
 bool file_meta_matches(int fd, const Entry& e, const MetaPolicy& pol);
@@ -85,8 +94,9 @@ int apply_file_meta(int fd, const std::string& path, const Entry& e, const MetaP
 int remove_source(const std::string& src_root, const Manifest& m);
 // VMIG_F_PRUNE: remove every destination entry the manifest does not list (directories recursively); entries are
 // handled by descriptor, symlinks are never followed.  dry_run only counts them (the verify pass uses that).
+// scope (nullable): only what lies beneath these manifest directories is looked at (vmig_restore_paths).
 int prune_extras(const std::string& dst_root, const Manifest& m, bool dry_run, uint64_t* n_extras,
-                 const std::atomic<int>* cancel = nullptr);
+                 const std::atomic<int>* cancel = nullptr, const std::vector<std::string>* scope = nullptr);
 // What remove_contents removed: entries unlinked or rmdir'ed, and the regular files among them whose link count was 1
 // just before the unlink (their space is freed unless a descriptor still holds them).
 struct RemoveCount { uint64_t entries = 0, files_freed = 0, bytes_freed = 0; };

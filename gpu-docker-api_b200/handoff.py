@@ -22,7 +22,7 @@ from typing import Callable, Optional
 import threading
 
 from . import (F_PRUNE, F_VERIFY, VMIG_ECANCELED, Ctl, GetContainerMergedLayer, GetVolumeMountPoint, VmigError, manifest,
-               migrate_tree, restore_tree, retire_versions, scrub_store, snapshot_tree)
+               migrate_tree, restore_paths, restore_tree, retire_versions, scrub_store, snapshot_tree)
 
 log = logging.getLogger("vmig.handoff")
 _root: dict = {"cwd": None}
@@ -74,6 +74,12 @@ def RestoreDirDiffVerified(snap, snapTable, dest, priorTable, outTable) -> dict:
     """utils.RestoreDirDiffVerified of the cgo shim: CopyDirDiffVerified from a snapshot that must still match its own
     block table (vmig_restore_tree); a partial, edited or rotted snapshot fails with VMIG_ECORRUPT."""
     return restore_tree(snap, snapTable, dest, priorTable or None, outTable or None, flags=F_VERIFY | F_PRUNE)
+
+
+def RestorePathsVerified(snap, snapTable, dest, priorTable, paths, ctl: Optional[Ctl] = None) -> dict:
+    """utils.RestorePathsVerified of the cgo shim: the chosen paths of a snapshot (vmig_restore_paths), each regular file
+    checked against the snapshot's table, verified, and pruned beneath the chosen directories only.  No table is written."""
+    return restore_paths(snap, snapTable, dest, paths, priorTable or None, flags=F_VERIFY | F_PRUNE, ctl=ctl)
 
 
 def SnapshotVersion(ctrVersionName: str) -> dict:
@@ -175,6 +181,21 @@ def RollbackFromSnapshot(targetCtrVersionName: str, newContainer: str, seedTable
     _, newTable = snapshotPaths(newContainer)
     newTable.parent.mkdir(parents=True, exist_ok=True)
     return RestoreDirDiffVerified(data, table, upper, seedTable, newTable)
+
+
+def RestorePathsFromSnapshot(targetCtrVersionName: str, container: str, paths: list, seedTable=None) -> dict:
+    """N1: put the chosen paths of version `target` back into `container`'s layer and leave everything else in it as it
+    is: a tenant who deleted or overwrote one file or directory gets it back without the whole-layer Rollback throwing
+    away what they did since.  Each restored file is checked against the snapshot's block table (RestorePathsVerified).
+      - The container must not be running: the upper dir of a mounted overlay must not change under it.
+      - The intended flow is Patch-like: HandoffCopy(old, new), then RestorePathsFromSnapshot(target, new, paths,
+        <new's blocks.vmig>), then start new.  seedTable is that table: files still as it recorded them are patched block
+        by block.  No table is written; the seed's records of the files this call rewrote go stale and the next diff
+        pass copies those in full.
+      - No REST route is added; the control plane stays as it is."""
+    data, table = snapshotPaths(targetCtrVersionName)
+    upper = GetContainerMergedLayer(container)
+    return RestorePathsVerified(data, table, upper, seedTable, paths)
 
 
 def HandoffCopy(oldContainer: str, newContainer: str, pause: Callable[[str], None], resume: Callable[[str], None],

@@ -186,6 +186,47 @@ int vmig_restore_tree(const char* snap_dir, const char* snap_table, const char* 
                       const char* prior_table, const char* out_table,
                       const vmig_opts* opts /*nullable*/, vmig_stats* stats /*nullable*/);
 
+/* Restore chosen entries of a snapshot (snap_dir with its block table snap_table) into dst_dir, each regular file with
+ * the guarantees vmig_restore_tree gives, and nothing in dst_dir outside those entries and their parent directories.
+ *   - paths[0..n_paths) are bytes relative to snap_dir, naming entries exactly as the table does.  VMIG_EINVAL, before
+ *     the GPU check and with nothing touched: n_paths == 0, a NULL array or entry, a path that is empty, absolute, has
+ *     an empty, "." or ".." component or ends in '/', two paths equal or one beneath the other (vmig_last_error() names
+ *     the index and the path); snap_table NULL/empty; snap_dir and dst_dir the same directory or one inside the other
+ *     (real paths); VMIG_F_MOVE_SRC, VMIG_F_HASH_ONLY or VMIG_F_CUFILE; a bad block_bytes.  A control cancelled before
+ *     the call is VMIG_ECANCELED; then comes VMIG_ENOGPU.
+ *   - A path is found when every proper prefix is a real directory under snap_dir (no symlink followed) and the entry
+ *     exists; it may be of any kind.  Not found: VMIG_ECORRUPT when the table has a record at or beneath it (missing),
+ *     else VMIG_EINVAL (not in the snapshot).  The selection -- the chosen entries and everything beneath the chosen
+ *     directories -- is walked as walk_tree walks (order, block layout, VMIG_F_SKIP_HIDDEN_TOPDIRS) and only it is read;
+ *     hard links are grouped inside the selection only (a path whose inode is also named outside it is restored as a
+ *     file of its own).
+ *   - Before dst_dir is touched, the table records at a chosen path or beneath a chosen directory must be exactly the
+ *     selection's regular-file paths with the table's sizes (VMIG_ECORRUPT: missing, extra or resized, as restore says
+ *     it).  Every block's XXH64 is checked on the GPU against the table as it passes and a block that fails is never
+ *     written; a hard-linked path's hashes are checked before any link is made.  Records outside the selection are not
+ *     looked at: a snapshot damaged elsewhere restores its intact part.
+ *   - dst_dir must exist (VMIG_EIO / VMIG_ENOTDIR).  No destination symlink is ever followed.  Each proper prefix of a
+ *     chosen path is made a real directory: an existing one is used as it is (owner and mode unchanged); a missing one,
+ *     or anything else in the way (symlink, file, special file, overlay whiteout, removed), becomes a directory with the
+ *     snapshot's owner, mode and mtime, applied after its contents.  The chosen entries and everything beneath them are
+ *     replaced exactly as vmig_restore_tree replaces them.  Nothing else in dst_dir is created, removed or modified; only
+ *     a parent directory's mtime moves, as any create in it moves it.
+ *   - VMIG_F_PRUNE removes, by descriptor, destination entries beneath each chosen directory that the snapshot's
+ *     subtree does not have, never anything elsewhere; with VMIG_F_VERIFY the chosen directories' entry sets are then
+ *     re-walked and must equal the snapshot's.  VMIG_F_VERIFY, VMIG_F_DIRECT_IO, VMIG_F_MTIME_NS, VMIG_F_NO_METADATA,
+ *     VMIG_F_SKIP_HIDDEN_TOPDIRS, lanes_per_gpu, gpu_mask and ctl act as in a restore.
+ *   - prior_table (nullable): the destination's own table, used as vmig_migrate_tree uses it (a file still its record
+ *     is patched in place; one whose blocks and metadata are unchanged is left alone).  No out table is written: the
+ *     records of the files this call rewrote go stale by the usual trust rule, and the next diff pass copies them in full.
+ * Phases WALK, (PRUNE), DATA, META, (VERIFY), DONE; bytes_total / blocks_total and stats are the selection's (dirs
+ * counts the selection's directories and the parents the call created).  On failure or cancel the destination may be
+ * partly written inside the selection and its parent chains, never with a block that failed a check; snap_dir and
+ * both tables are never modified. */
+int vmig_restore_paths(const char* snap_dir, const char* snap_table, const char* dst_dir,
+                       uint32_t n_paths, const char* const* paths,
+                       const char* prior_table /*nullable*/,
+                       const vmig_opts* opts /*nullable*/, vmig_stats* stats /*nullable*/);
+
 /* Incremental version snapshot: what vmig_snapshot_tree took from the base snapshot instead of the GPU's staging ring. */
 typedef struct vmig_snapshot_stats {
     uint64_t files_linked;          /* regular files that are a hard link to the base snapshot's file: no data written */
@@ -376,7 +417,7 @@ void vmig_host_free(void* p);
 
 /* ---- cancellation and progress ------------------------------------------------------------------
  * A control is a numeric id (cgo passes it in vmig_opts.ctl without any pointer rules).  It serves the entry points
- * that take vmig_opts: vmig_migrate_tree, vmig_restore_tree, vmig_snapshot_tree, vmig_scrub_store, vmig_retire_versions and vmig_migrate_buffer (a caller that
+ * that take vmig_opts: vmig_migrate_tree, vmig_restore_tree, vmig_restore_paths, vmig_snapshot_tree, vmig_scrub_store, vmig_retire_versions and vmig_migrate_buffer (a caller that
  * wants to cancel a copy or a move calls vmig_migrate_tree with the flags vmig_copy_dir / vmig_move_dir use).  One
  * control serves one call at a time: attaching it to a second concurrent call fails with VMIG_EINVAL.  The engine has
  * no deadline of its own; a deadline is the caller's timer calling vmig_ctl_cancel.

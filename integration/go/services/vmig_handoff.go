@@ -228,6 +228,25 @@ func RollbackFromSnapshot(targetCtrVersionName, newContainer, seedTable string) 
 	return errors.WithMessagef(utils.RestoreDirDiffVerified(data, table, upper, seedTable, newTable), "rollback to %s failed", targetCtrVersionName)
 }
 
+// N1 -- RestorePathsFromSnapshot puts the chosen paths of version `target` back into container's layer and leaves
+// everything else in it as it is: a tenant who deleted or overwrote one file or directory gets it back without the
+// whole-layer Rollback throwing away what they did since.  Each restored file is checked against the snapshot's block
+// table (utils.RestorePathsVerified).
+//   - The container must not be running: the upper dir of a mounted overlay must not change under it.
+//   - The intended flow is Patch-like: HandoffCopy(old, new), then RestorePathsFromSnapshot(target, new, paths,
+//     <new's blocks.vmig>), then start new.  seedTable is that table: files still as it recorded them are patched block
+//     by block.  No table is written; the seed's records of the files this call rewrote go stale and the next diff
+//     pass copies those in full.
+//   - No REST route is added; the control plane stays as it is.
+func RestorePathsFromSnapshot(targetCtrVersionName, container string, paths []string, seedTable string) error {
+	data, table := snapshotPaths(targetCtrVersionName)
+	upper, err := utils.GetContainerMergedLayer(container)
+	if err != nil {
+		return errors.WithMessagef(err, "utils.GetContainerMergedLayer failed, container: %s", container)
+	}
+	return errors.WithMessagef(utils.RestorePathsVerified(data, table, upper, seedTable, paths), "restore of %d paths from %s failed", len(paths), targetCtrVersionName)
+}
+
 // N2 -- HandoffCopy replaces utils.CopyOldMergedToNewContainerMerged in PatchContainer (replicaset.go:333):
 // the old container keeps running during pass 1 (the bulk of the bytes), is paused for pass 2, which re-reads
 // the source and moves only the blocks whose hash changed in between, and stays paused until the caller has

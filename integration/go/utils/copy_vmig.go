@@ -102,6 +102,37 @@ func RestoreDirDiffVerifiedContext(ctx context.Context, snap, snapTable, dest, p
 		})
 }
 
+// RestorePathsVerified puts the chosen paths (relative to snap, named as snapTable names them) of a snapshot back into
+// dest and touches nothing else there but their parent directories (vmig_restore_paths): each regular file is checked
+// against snapTable as RestoreDirDiffVerified checks it, the result is re-read through the GPU (VMIG_F_VERIFY), and
+// VMIG_F_PRUNE removes extras beneath the chosen directories only.  priorTable is dest's own table (files still as it
+// recorded them are patched block by block); no table is written.
+func RestorePathsVerified(snap, snapTable, dest, priorTable string, paths []string) error {
+	return RestorePathsVerifiedContext(context.Background(), snap, snapTable, dest, priorTable, paths)
+}
+
+// RestorePathsVerifiedContext is RestorePathsVerified that stops when ctx is done (see CopyDirDiffContext); the
+// snapshot, its table and priorTable are untouched either way.
+func RestorePathsVerifiedContext(ctx context.Context, snap, snapTable, dest, priorTable string, paths []string) error {
+	n := len(paths)
+	if n == 0 {
+		return errors.Errorf("RestorePathsVerified: no path to restore")
+	}
+	ptrSize := C.size_t(unsafe.Sizeof((*C.char)(nil)))
+	cpaths := (*[1 << 28]*C.char)(C.malloc(C.size_t(n) * ptrSize))[:n:n] // C memory: cgo forbids Go pointers to Go pointers
+	defer C.free(unsafe.Pointer(&cpaths[0]))
+	for i := 0; i < n; i++ {
+		cpaths[i] = C.CString(paths[i])
+		defer C.free(unsafe.Pointer(cpaths[i]))
+	}
+	ct := C.CString(snapTable)
+	defer C.free(unsafe.Pointer(ct))
+	return runDiff(ctx, "vmig_restore_paths", snap, dest, priorTable, "", C.VMIG_F_VERIFY|C.VMIG_F_PRUNE,
+		func(cs, cd, cp, _ *C.char, o *C.vmig_opts, st *C.vmig_stats, _ *C.vmig_snapshot_stats) C.int {
+			return C.vmig_restore_paths(cs, ct, cd, C.uint32_t(n), &cpaths[0], cp, o, st)
+		})
+}
+
 // SnapshotDirIncrementalVerified is SnapshotDirVerified that shares what did not change with the previous snapshot
 // baseDir, taken with baseTable (vmig_snapshot_tree): an unchanged file becomes a hard link to the base's, also when it
 // was renamed or moved since, and a changed or copied file takes every block the base holds from the base file that

@@ -1633,7 +1633,8 @@ int vmig_link_probe(int gpu, uint64_t bytes, double gbs[4])
 }
 
 // ---------------------------------------------------------------------------------------------
-// HBM-resident batch
+// HBM-resident batch.  Every call puts its copies and memsets on the handle's (non-blocking) stream and synchronises it
+// before it returns: the caller's buffer may go right after, and a pass issued next is ordered after them.
 struct vmig_resident {
     int dev; int sm_count; uint64_t n; uint32_t block_bytes;
     uint8_t* d_data; uint64_t* d_offs; uint32_t* d_lens; uint64_t* d_hashes; uint64_t* d_prior; uint8_t* d_valid;
@@ -1657,10 +1658,11 @@ static int resident_alloc(vmig_resident* r, uint64_t n_blocks, uint32_t block_by
     CU_API(cudaEventCreate(&r->e0)); CU_API(cudaEventCreate(&r->e1)); CU_API(cudaEventCreate(&r->e2)); CU_API(cudaEventCreate(&r->e3));
     std::vector<uint64_t> offs(n_blocks); std::vector<uint32_t> lens(n_blocks, block_bytes);
     for (uint64_t i = 0; i < n_blocks; i++) offs[i] = i * (uint64_t)block_bytes;
-    CU_API(cudaMemcpy(r->d_offs, offs.data(), n_blocks * 8, cudaMemcpyHostToDevice));
-    CU_API(cudaMemcpy(r->d_lens, lens.data(), n_blocks * 4, cudaMemcpyHostToDevice));
-    CU_API(cudaMemset(r->d_valid, 0, n_blocks)); CU_API(cudaMemset(r->d_prior, 0, n_blocks * 8));
-    CU_API(cudaMemset(r->d_data + n_blocks * (uint64_t)block_bytes, 0, kTailPad));
+    CU_API(cudaMemcpyAsync(r->d_offs, offs.data(), n_blocks * 8, cudaMemcpyHostToDevice, r->stream));
+    CU_API(cudaMemcpyAsync(r->d_lens, lens.data(), n_blocks * 4, cudaMemcpyHostToDevice, r->stream));
+    CU_API(cudaMemsetAsync(r->d_valid, 0, n_blocks, r->stream)); CU_API(cudaMemsetAsync(r->d_prior, 0, n_blocks * 8, r->stream));
+    CU_API(cudaMemsetAsync(r->d_data + n_blocks * (uint64_t)block_bytes, 0, kTailPad, r->stream));
+    CU_API(cudaStreamSynchronize(r->stream));        // offs / lens are locals
     return VMIG_OK;
 }
 
@@ -1706,22 +1708,25 @@ int vmig_resident_set_len(vmig_resident* r, uint64_t block, uint32_t len)
 {
     if (!r || block >= r->n || len > r->block_bytes) return fail(VMIG_EINVAL, "bad block/len");
     CU_API(cudaSetDevice(r->dev));
-    CU_API(cudaMemcpy(r->d_lens + block, &len, 4, cudaMemcpyHostToDevice));
+    CU_API(cudaMemcpyAsync(r->d_lens + block, &len, 4, cudaMemcpyHostToDevice, r->stream));
+    CU_API(cudaStreamSynchronize(r->stream));
     return VMIG_OK;
 }
 int vmig_resident_upload(vmig_resident* r, uint64_t block, const void* host, uint32_t len)
 {
     if (!r || block >= r->n || len > r->block_bytes || (len && !host)) return fail(VMIG_EINVAL, "bad block/len");
     CU_API(cudaSetDevice(r->dev));
-    if (len) CU_API(cudaMemcpy(r->d_data + block * (uint64_t)r->block_bytes, host, len, cudaMemcpyHostToDevice));
-    CU_API(cudaMemcpy(r->d_lens + block, &len, 4, cudaMemcpyHostToDevice));
+    if (len) CU_API(cudaMemcpyAsync(r->d_data + block * (uint64_t)r->block_bytes, host, len, cudaMemcpyHostToDevice, r->stream));
+    CU_API(cudaMemcpyAsync(r->d_lens + block, &len, 4, cudaMemcpyHostToDevice, r->stream));
+    CU_API(cudaStreamSynchronize(r->stream));
     return VMIG_OK;
 }
 int vmig_resident_download(vmig_resident* r, uint64_t block, void* host, uint32_t len)
 {
     if (!r || block >= r->n || len > r->block_bytes || !host) return fail(VMIG_EINVAL, "bad block/len");
     CU_API(cudaSetDevice(r->dev));
-    CU_API(cudaMemcpy(host, r->d_data + block * (uint64_t)r->block_bytes, len, cudaMemcpyDeviceToHost));
+    CU_API(cudaMemcpyAsync(host, r->d_data + block * (uint64_t)r->block_bytes, len, cudaMemcpyDeviceToHost, r->stream));
+    CU_API(cudaStreamSynchronize(r->stream));
     return VMIG_OK;
 }
 int vmig_resident_flip(vmig_resident* r, const uint64_t* blocks, uint64_t n)
@@ -1742,11 +1747,12 @@ int vmig_resident_set_prior(vmig_resident* r, const uint64_t* hashes, const uint
     CU_API(cudaSetDevice(r->dev));
     r->has_prior = hashes != nullptr && valid != nullptr;
     if (r->has_prior) {
-        CU_API(cudaMemcpy(r->d_prior, hashes, r->n * 8, cudaMemcpyHostToDevice));
-        CU_API(cudaMemcpy(r->d_valid, valid, r->n, cudaMemcpyHostToDevice));
+        CU_API(cudaMemcpyAsync(r->d_prior, hashes, r->n * 8, cudaMemcpyHostToDevice, r->stream));
+        CU_API(cudaMemcpyAsync(r->d_valid, valid, r->n, cudaMemcpyHostToDevice, r->stream));
     } else {
-        CU_API(cudaMemset(r->d_valid, 0, r->n));
+        CU_API(cudaMemsetAsync(r->d_valid, 0, r->n, r->stream));
     }
+    CU_API(cudaStreamSynchronize(r->stream));
     return VMIG_OK;
 }
 int vmig_resident_pass(vmig_resident* r, uint32_t iters, double* ms_hash_last, double* ms_total)
@@ -1776,11 +1782,15 @@ int vmig_resident_results(vmig_resident* r, uint64_t* hashes, uint32_t* survivor
 {
     if (!r) return fail(VMIG_EINVAL, "null handle");
     CU_API(cudaSetDevice(r->dev));
-    if (hashes) CU_API(cudaMemcpy(hashes, r->d_hashes, r->n * 8, cudaMemcpyDeviceToHost));
+    if (hashes) CU_API(cudaMemcpyAsync(hashes, r->d_hashes, r->n * 8, cudaMemcpyDeviceToHost, r->stream));
     uint32_t ns = 0;
-    CU_API(cudaMemcpy(&ns, r->d_nsurv, 4, cudaMemcpyDeviceToHost));
+    CU_API(cudaMemcpyAsync(&ns, r->d_nsurv, 4, cudaMemcpyDeviceToHost, r->stream));
+    CU_API(cudaStreamSynchronize(r->stream));
     if (n_survivors) *n_survivors = ns;
-    if (survivors && ns) CU_API(cudaMemcpy(survivors, r->d_survivors, (size_t)ns * 4, cudaMemcpyDeviceToHost));
+    if (survivors && ns) {
+        CU_API(cudaMemcpyAsync(survivors, r->d_survivors, (size_t)ns * 4, cudaMemcpyDeviceToHost, r->stream));
+        CU_API(cudaStreamSynchronize(r->stream));
+    }
     return VMIG_OK;
 }
 

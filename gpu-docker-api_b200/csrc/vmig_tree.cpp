@@ -247,12 +247,29 @@ void finish_manifest(Manifest* m)
     m->n_blocks = fb;
 }
 
+// The process umask, read without changing it.  umask(2) reads only by setting: a set-and-restore lets a call running at
+// the same time read 0 (and replay every mode unmasked), and any file another thread creates in between is made with
+// umask 0.  Linux reports it in /proc/self/status since 4.7; older kernels fall back to set-and-restore, one call at a time.
+static mode_t process_umask()
+{
+    if (FILE* f = fopen("/proc/self/status", "re")) {
+        char line[256]; unsigned um = 0; bool found = false;
+        while (!found && fgets(line, sizeof line, f)) found = sscanf(line, "Umask: %o", &um) == 1;
+        fclose(f);
+        if (found) return (mode_t)um;
+    }
+    static std::mutex mu;
+    std::lock_guard<std::mutex> lk(mu);
+    const mode_t um = umask(0);
+    umask(um);
+    return um;
+}
+
 MetaPolicy default_meta_policy(uint32_t flags)
 {
     MetaPolicy p;
     p.is_root = geteuid() == 0;
-    mode_t um = umask(0); umask(um);
-    p.umask_bits = um;
+    p.umask_bits = process_umask();
     p.mtime_ns = (flags & VMIG_F_MTIME_NS) != 0 || (flags & VMIG_F_MOVE_SRC) != 0;
     p.no_metadata = (flags & VMIG_F_NO_METADATA) != 0;
     p.keep_atime = (flags & VMIG_F_MOVE_SRC) != 0;

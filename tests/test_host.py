@@ -80,7 +80,8 @@ def test_source_side_path_safety_unit(shm_tmp):
     """csrc/vmig_tree.cpp alone (no GPU, no CUDA): open_beneath refuses symlinks and escapes, the walk does not
     descend through symlinked directories, remove_source cannot be steered out of the tree; prune_extras (VMIG_F_PRUNE)
     removes exactly the entries the manifest lacks and never follows a symlink; the walk gives the same manifest with
-    one thread and with eight (hard-link pair across two sub-walks included)."""
+    one thread and with eight (hard-link pair across two sub-walks included); the metadata policy reads the umask without
+    changing it, so a call running at the same time never sees umask 0."""
     import subprocess
     exe = shm_tmp / "tree_unit"
     csrc = ROOT / "gpu-docker-api_b200" / "csrc"

@@ -8,6 +8,8 @@
 #include <unistd.h>
 #include <cstdio>
 #include <cstdlib>
+#include <atomic>
+#include <thread>
 #include <string>
 #include <sys/stat.h>
 
@@ -116,6 +118,25 @@ int main(int argc, char** argv) {
         for (size_t i = 0; i < a.symlinks.size(); i++) CHECK(a.symlinks[i].rel == b.symlinks[i].rel);
         int links = 0; for (auto& e : b.files) if (e.hardlink_of >= 0) { links++; CHECK(b.files[(size_t)e.hardlink_of].rel == "d3/f0" && e.rel == "d9/hard"); }
         CHECK(links == 1);
+    }
+    {
+        // the metadata policy reads the umask without changing it: a thread watching the process umask while policies are
+        // built never sees another value (a set-and-restore read showed 0 to calls running at the same time)
+        const mode_t old = umask(027);
+        std::atomic<bool> stop{false}; std::atomic<int> other{0};
+        std::thread watch([&] {
+            while (!stop.load()) {
+                FILE* f = fopen("/proc/self/status", "r"); char line[256]; unsigned um = 027;
+                while (f && fgets(line, sizeof line, f)) if (sscanf(line, "Umask: %o", &um) == 1) break;
+                if (f) fclose(f);
+                if (um != 027) other++;
+            }
+        });
+        bool all = true;
+        for (int i = 0; i < 20000; i++) all = all && default_meta_policy(0).umask_bits == 027;
+        stop = true; watch.join();
+        umask(old);
+        CHECK(all && other.load() == 0);
     }
     printf("tree unit ok\n");
     return 0;

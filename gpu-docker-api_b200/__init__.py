@@ -54,6 +54,10 @@ SCRUB_KINDS = ("missing", "extra", "resized", "block", "hardlink", "unreadable",
 
 
 class Opts(C.Structure):
+    """vmig_opts (include/vmig.h).  io_threads and streams_per_gpu apply PER LANE: every one of the n_gpus *
+    lanes_per_gpu lanes runs io_threads copy threads (n >= 2: (n+1)*2//5 readers, the rest writers; 1: one of each;
+    0: the per-box budget divided among the lanes in flight) and keeps up to streams_per_gpu of its pipe's staging
+    slots in flight (0, or more than the pipe has: all of them)."""
     _fields_ = [("gpu_mask", C.c_uint32), ("block_bytes", C.c_uint32), ("streams_per_gpu", C.c_uint32),
                 ("flags", C.c_uint32), ("io_threads", C.c_uint32), ("lanes_per_gpu", C.c_uint32),
                 ("ctl", C.c_uint32), ("reserved", C.c_uint32)]
@@ -327,14 +331,16 @@ def restore_tree(snap, snap_table, dst, prior_table=None, out_table=None, *, gpu
 
 
 def restore_paths(snap, snap_table, dst, paths, prior_table=None, *, flags: int = 0, gpu_mask: int = 0,
-                  lanes_per_gpu: int = 0, block_bytes: int = 0, ctl: Optional[Ctl] = None) -> dict:
+                  lanes_per_gpu: int = 0, block_bytes: int = 0, io_threads: int = 0, streams_per_gpu: int = 0,
+                  ctl: Optional[Ctl] = None) -> dict:
     """Restore the chosen entries `paths` (str or bytes, relative to `snap`, named as the table names them) of a snapshot
     into `dst`, each regular file checked against `snap_table` as restore_tree checks it; nothing in `dst` outside those
     entries and their parent directories is touched.  prior_table: `dst`'s own table (unchanged blocks are not written);
     no table is written.  Returns the migrate_tree counters of the selection."""
     paths = list(paths)
     arr = (C.c_char_p * max(len(paths), 1))(*[_b(p) for p in paths])
-    o = Opts(gpu_mask=gpu_mask, block_bytes=block_bytes, flags=flags, lanes_per_gpu=lanes_per_gpu, ctl=_ctl_id(ctl))
+    o = Opts(gpu_mask=gpu_mask, block_bytes=block_bytes, flags=flags, lanes_per_gpu=lanes_per_gpu, io_threads=io_threads,
+             streams_per_gpu=streams_per_gpu, ctl=_ctl_id(ctl))
     st = Stats()
     _check(_lib.vmig_restore_paths(_b(snap), _b(snap_table), _b(dst), len(paths), arr, _b(prior_table), C.byref(o),
                                    C.byref(st)), f"vmig_restore_paths({snap} -> {dst}, {len(paths)} paths)")
@@ -475,7 +481,8 @@ class PinnedBuffer:
 
 
 def migrate_buffer(src: np.ndarray, dst: Optional[np.ndarray], prior_hashes=None, prior_valid=None, *,
-                   gpu_mask: int = 0, flags: int = 0, block_bytes: int = 0, ctl: Optional[Ctl] = None):
+                   gpu_mask: int = 0, flags: int = 0, block_bytes: int = 0, io_threads: int = 0, streams_per_gpu: int = 0,
+                   lanes_per_gpu: int = 0, ctl: Optional[Ctl] = None):
     """Host buffer -> host buffer through H2D / hash / diff / D2H.  Returns (hashes, stats)."""
     bb = block_bytes or BLOCK_BYTES
     n = src.size
@@ -483,7 +490,8 @@ def migrate_buffer(src: np.ndarray, dst: Optional[np.ndarray], prior_hashes=None
     out = np.zeros(nb, dtype=np.uint64)
     ph = None if prior_hashes is None else np.ascontiguousarray(prior_hashes, dtype=np.uint64)
     pv = None if prior_valid is None else np.ascontiguousarray(prior_valid, dtype=np.uint8)
-    o = Opts(gpu_mask=gpu_mask, block_bytes=block_bytes, flags=flags, ctl=_ctl_id(ctl))
+    o = Opts(gpu_mask=gpu_mask, block_bytes=block_bytes, flags=flags, io_threads=io_threads, streams_per_gpu=streams_per_gpu,
+             lanes_per_gpu=lanes_per_gpu, ctl=_ctl_id(ctl))
     st = Stats()
     _check(_lib.vmig_migrate_buffer(src.ctypes.data, None if dst is None else dst.ctypes.data, n,
                                     None if ph is None else ph.ctypes.data, None if pv is None else pv.ctypes.data,

@@ -124,6 +124,7 @@ public:
         std::atomic<void*> s_cfh{nullptr}, d_cfh{nullptr};   // cuFile handles of sfd / dfd (VMIG_F_CUFILE)
         std::atomic<bool> wrote{false};                  // at least one block of the file was written in this call
         std::atomic<bool> reused{false};                 // vmig_snapshot_tree: a changed block was found elsewhere in the base
+        int lent_mode = -1;                              // >= 0: open_dst lent the file a write bit; its mode before that
         void identify(const struct stat& st) { id_ino = (uint64_t)st.st_ino; id_ctime_ns = ctime_ns(st); }
     };
     std::string src_root, dst_root;
@@ -321,10 +322,13 @@ public:
                     fd = open(p.c_str(), O_WRONLY | O_CLOEXEC | O_NOFOLLOW | dflag);
                     // an ordinary user's own read-only file (tar would replace it): made writable for the patch; its mode no
                     // longer matches the source's, so block_done puts the source's back whether a block was written or not
+                    // (under VMIG_F_NO_METADATA the mode it had before the lend)
                     struct stat ws;
                     if (fd < 0 && errno == EACCES && lstat(p.c_str(), &ws) == 0 && S_ISREG(ws.st_mode) &&
-                        chmod(p.c_str(), (ws.st_mode & 07777) | S_IWUSR) == 0)
+                        chmod(p.c_str(), (ws.st_mode & 07777) | S_IWUSR) == 0) {
+                        s.lent_mode = (int)(ws.st_mode & 07777);
                         fd = open(p.c_str(), O_WRONLY | O_CLOEXEC | O_NOFOLLOW | dflag);
+                    }
                     if (fd < 0 && dflag && errno == EINVAL) fd = open(p.c_str(), O_WRONLY | O_CLOEXEC | O_NOFOLLOW); else s.d_direct = dflag != 0 && fd >= 0;
                 } else {
                     int rc = clear_path(p, "a regular file");     // tar replaces what is there
@@ -428,14 +432,19 @@ public:
         if (rc) return rc;
         const std::string p = pjoin(dst_root, e.rel);
         const bool inplace = fp.prior_rec != nullptr;
-        if (((inplace && fp.prior_rec->size != e.size) || (s.d_direct && (e.size & (kSector - 1)))) && ftruncate(fd, (off_t)e.size) != 0) {
+        // O_DIRECT writes whole sectors: cut the padding of the last one.  A file patched in place that took no write has
+        // none, and a truncate would move its mtime and ctime and so the identity its table records
+        const bool padded = s.d_direct && (e.size & (kSector - 1)) && (s.wrote.load() || !inplace);
+        if (((inplace && fp.prior_rec->size != e.size) || padded) && ftruncate(fd, (off_t)e.size) != 0) {
             close(fd); return fail(VMIG_EIO, "ftruncate %s: %s", p.c_str(), errno_str(errno).c_str());
         }
         // a patched-in-place file none of whose blocks changed and whose metadata is already right is not touched at all:
         // its ctime -- by which the block table knows it -- stays what the table recorded
         const bool untouched = inplace && !s.wrote.load() && fp.prior_rec->size == e.size && file_meta_matches(fd, e, pol);
         rc = untouched ? VMIG_OK : apply_file_meta(fd, p, e, pol);
-        struct stat ids;                             // nothing touches the file after this point: its ctime is final
+        if (!rc && pol.no_metadata && s.lent_mode >= 0 && fchmod(fd, (mode_t)s.lent_mode) != 0)
+            rc = fail(VMIG_EIO, "fchmod %s (mode lent for the patch): %s", p.c_str(), errno_str(errno).c_str());
+        struct stat ids;                            // nothing touches the file after this point: its ctime is final
         if (!rc && fstat(fd, &ids) == 0) s.identify(ids);
         { void* h = s.d_cfh.exchange(nullptr); if (h) cufile_handle_close(h); }
         if (close(fd) != 0 && !rc) rc = fail(VMIG_EIO, "close %s: %s", p.c_str(), errno_str(errno).c_str());

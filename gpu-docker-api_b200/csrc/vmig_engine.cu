@@ -421,7 +421,10 @@ int io_threads_default(uint32_t* readers, uint32_t* writers, uint32_t requested,
                        bool has_prior, bool hash_only)
 {
     long r = env_long("VMIG_READERS", 0), w = env_long("VMIG_WRITERS", 0);
-    if (requested) { r = (requested + 1) * 2 / 5; w = requested - r; }
+    // vmig_opts.io_threads = n: exactly n threads per lane split 2:3, never the budget below; one reader and one writer are
+    // the least a lane runs with
+    if (requested == 1) { r = 1; w = 1; }
+    else if (requested) { r = (requested + 1) * 2 / 5; w = requested - r; }
     if (r <= 0 || w <= 0) {
         cpu_set_t cur; CPU_ZERO(&cur);
         long ncpu = sched_getaffinity(0, sizeof cur, &cur) == 0 ? CPU_COUNT(&cur) : sysconf(_SC_NPROCESSORS_ONLN);
@@ -847,10 +850,10 @@ int run_lane(Pipe* pipe, const std::vector<BlockRef>& blocks, BlockIO* io, bool 
             a[2] += (b.t_hash - b.t_sub) / 1e6; a[3] += (b.t_d2h - b.t_hash) / 1e6; a[4] += (b.t_done - b.t_d2h) / 1e6; nb++;
         }
         fprintf(stderr, "[vmig trace] gpu %d: %zu batches in %.1f ms; mean ms/batch: read %.2f submit-wait %.2f h2d+hash %.2f d2h %.2f write %.2f; "
-                        "reader busy %.0f%% of %u, writer busy %.0f%% of %u; dispatcher waited %.1f ms for slots; kernel sum %.1f ms\n",
+                        "reader busy %.0f%% of %u, writer busy %.0f%% of %u; dispatcher waited %.1f ms for %d slots; kernel sum %.1f ms\n",
                 pipe->dev.dev, nb, wall, a[0] / nb, a[1] / nb, a[2] / nb, a[3] / nb, a[4] / nb,
                 100.0 * rd_busy.load() / 1e6 / (wall * n_readers), n_readers, 100.0 * wr_busy.load() / 1e6 / (wall * n_writers), n_writers,
-                slot_wait.load() / 1e6, stats->ms_kernel);
+                slot_wait.load() / 1e6, use_slots, stats->ms_kernel);
     }
     // the slots go back to the pool idle
     cudaSetDevice(pipe->dev.dev);

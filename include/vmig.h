@@ -78,7 +78,14 @@ const char* vmig_version(void);
                                            are left behind (reference utils/copy.go:116)           */
 #define VMIG_F_MTIME_NS          0x04u  /* keep nanosecond mtimes (mv does; GNU tar's default archive
                                            format keeps whole seconds only -> default off)         */
-#define VMIG_F_NO_METADATA       0x08u  /* data only: no chown/chmod/utimens                       */
+#define VMIG_F_NO_METADATA       0x08u  /* data only: no chown/chmod/utimens.  Directories that already exist and
+                                           regular files patched in place keep their owner and mode (a read-only
+                                           file an ordinary user's diff pass patches gets its own mode back), and
+                                           their mtime unless the call writes into them.  Whatever the call
+                                           creates -- every other file, every special file and symlink, missing
+                                           directories -- is owned by the caller, has the mtime of its creation and
+                                           the creation mode less the process umask: regular files and specials
+                                           0600, directories 0700                                            */
 #define VMIG_F_HASH_ONLY         0x10u  /* build the block table of src; dst is not touched        */
 #define VMIG_F_VERIFY            0x20u  /* after the copy, re-read the DESTINATION through the GPU and
                                            require its block hashes to equal the source's; with
@@ -112,9 +119,12 @@ const char* vmig_version(void);
 typedef struct vmig_opts {
     uint32_t gpu_mask;         /* 0 = every initialised GPU; blocks are sharded across the set   */
     uint32_t block_bytes;      /* 0 -> 4 MiB (4194304); must be a multiple of 4096               */
-    uint32_t streams_per_gpu;  /* side streams = staging slots in flight per GPU; 0 -> all (16)   */
+    uint32_t streams_per_gpu;  /* side streams = staging slots in flight PER LANE (each lane has its own pipe of
+                                  VMIG_SLOTS slots, 16 by default); 0 or more than the pipe has -> all of them     */
     uint32_t flags;            /* VMIG_F_*                                                       */
-    uint32_t io_threads;       /* 0 -> default: host reader+writer threads per GPU               */
+    uint32_t io_threads;       /* host copy threads PER LANE: n >= 2 -> exactly n, r = (n+1)*2/5 readers and n - r
+                                  writers; 1 -> one reader and one writer; 0 -> the per-box budget divided among
+                                  the lanes in flight (vmig_thread_plan)                                          */
     uint32_t lanes_per_gpu;    /* 0/1 -> one lane (staging-ring set + thread pipeline) per GPU of the
                                   mask; k -> k lanes per GPU, the block list is sharded over
                                   n_gpus*k lanes exactly as it is over n_gpus*k GPUs (more host

@@ -48,9 +48,10 @@ EXPORTS = [
     "vmig_resident_set_prior", "vmig_resident_pass", "vmig_resident_results", "vmig_table_info_read",
     "vmig_table_hashes", "vmig_dir_size", "vmig_to_bytes", "vmig_datagen_files", "vmig_manifest", "vmig_link_probe", "vmig_thread_plan",
     "vmig_ctl_open", "vmig_ctl_cancel", "vmig_ctl_progress", "vmig_ctl_close", "vmig_scrub_store",
-    "vmig_retire_versions", "vmig_restore_paths",
+    "vmig_retire_versions", "vmig_restore_paths", "vmig_compare_snapshot",
 ]
 SCRUB_KINDS = ("missing", "extra", "resized", "block", "hardlink", "unreadable", "table", "dir")
+COMPARE_KINDS = ("added", "removed", "type", "resized", "block", "target", "rdev", "hardlink", "mode", "owner", "mtime")
 
 
 class Opts(C.Structure):
@@ -99,6 +100,15 @@ class ScrubStats(C.Structure):
 class RetireStats(C.Structure):
     _fields_ = [(n, C.c_uint64) for n in ("versions_retired", "entries_removed", "files_freed", "bytes_freed", "records_stale",
                                           "records_restamped", "bytes_rehashed", "tables_rewritten")] + [("reserved", C.c_uint64 * 4)]
+
+    def as_dict(self) -> dict:
+        return {n: getattr(self, n) for n, _ in self._fields_ if n != "reserved"}
+
+
+class CompareStats(C.Structure):
+    _fields_ = [(n, C.c_uint64) for n in ("paths_added", "paths_removed", "paths_changed", "files_changed", "blocks_changed",
+                                          "bytes_restore", "files_read", "bytes_read", "files_trusted", "files_shared")] + \
+        [("reserved", C.c_uint64 * 4)]
 
     def as_dict(self) -> dict:
         return {n: getattr(self, n) for n, _ in self._fields_ if n != "reserved"}
@@ -159,6 +169,8 @@ _sig = {
                                        C.POINTER(C.c_char_p), C.POINTER(Opts), C.POINTER(Stats), C.POINTER(RetireStats)]),
     "vmig_restore_paths": (C.c_int, [C.c_char_p, C.c_char_p, C.c_char_p, C.c_uint32, C.POINTER(C.c_char_p), C.c_char_p,
                                      C.POINTER(Opts), C.POINTER(Stats)]),
+    "vmig_compare_snapshot": (C.c_int, [C.c_char_p, C.c_char_p, C.c_char_p, C.c_char_p, C.c_char_p, C.POINTER(Opts),
+                                        C.POINTER(Stats), C.POINTER(CompareStats)]),
 }
 for _n, (_r, _a) in _sig.items():
     _f = getattr(_lib, _n)
@@ -206,7 +218,8 @@ def _b(p) -> Optional[bytes]:
 
 
 class Ctl:
-    """A call control (vmig_ctl_*): pass it as ``ctl=`` to migrate_tree, restore_tree, restore_paths, snapshot_tree or migrate_buffer,
+    """A call control (vmig_ctl_*): pass it as ``ctl=`` to migrate_tree, restore_tree, restore_paths, snapshot_tree,
+    scrub_store, retire_versions, compare_snapshot or migrate_buffer,
     then cancel() from any thread (the call raises VmigError(VMIG_ECANCELED)) or read progress() while it runs.  ctypes
     releases the GIL during the call.  One control serves one call at a time; a deadline is a threading.Timer."""
 
@@ -445,6 +458,39 @@ def retire_versions(retire_pairs, keep_pairs, *, flags: int = 0, gpu_mask: int =
                                      arr(keep_pairs, 0), arr(keep_pairs, 1), C.byref(o), C.byref(st), C.byref(rs)),
            f"vmig_retire_versions({len(retire_pairs)} retired, {len(keep_pairs)} kept)")
     return {"stats": st.as_dict(), **rs.as_dict()}
+
+
+def parse_compare_report(path) -> list:
+    """The findings of a vmig_compare_snapshot report: dicts with kind, path (str, os.fsdecode of the raw name), block
+    (None for "-"), layer and snap (the report's fields as str, None for "-"; the paths of `target` and `hardlink` are
+    unescaped like path)."""
+    out = []
+    with open(path, "rb") as f:
+        for line in f.read().split(b"\n"):
+            if not line:
+                continue
+            kind, p, blk, lv, sv = os.fsdecode(line).split("\t")
+
+            def field(v):
+                if v == "-":
+                    return None
+                return os.fsdecode(unescape_report_path(v)) if kind in ("target", "hardlink") else v
+            out.append({"kind": kind, "path": os.fsdecode(unescape_report_path(p)), "block": None if blk == "-" else int(blk),
+                        "layer": field(lv), "snap": field(sv)})
+    return out
+
+
+def compare_snapshot(layer, snap, snap_table, report=None, layer_table=None, *, flags: int = 0, gpu_mask: int = 0,
+                     lanes_per_gpu: int = 0, block_bytes: int = 0, ctl: Optional[Ctl] = None) -> dict:
+    """List every difference between the layer `layer` and the version snapshot `snap` (checked against `snap_table`):
+    what restore_tree(snap, snap_table, layer, flags=F_PRUNE | flags) would change.  Writes nothing but `report` (one
+    line per finding, parse_compare_report reads it).  layer_table: a table of `layer` whose records still vouch for
+    their files (those are not read).  Returns the vmig_compare_stats fields plus the data pass's counters ("stats")."""
+    o = Opts(gpu_mask=gpu_mask, block_bytes=block_bytes, flags=flags, lanes_per_gpu=lanes_per_gpu, ctl=_ctl_id(ctl))
+    st, cs = Stats(), CompareStats()
+    _check(_lib.vmig_compare_snapshot(_b(layer), _b(layer_table), _b(snap), _b(snap_table), _b(report), C.byref(o),
+                                      C.byref(st), C.byref(cs)), f"vmig_compare_snapshot({layer} vs {snap})")
+    return {"stats": st.as_dict(), **cs.as_dict()}
 
 
 def hash_tree(src, out_table, *, gpu_mask: int = 0, block_bytes: int = 0) -> dict:

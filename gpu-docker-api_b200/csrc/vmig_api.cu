@@ -10,6 +10,7 @@
 #include "vmig_cufile.h"
 #include "vmig_reuse.h"
 #include "vmig_scrub.h"
+#include "vmig_compare.h"
 #include "vmig_retire.h"
 #include "vmig_plan.h"
 #include "vmig_select.h"
@@ -1305,6 +1306,104 @@ int retire_body(CallScope& call, const RetireArgs& a, const vmig_opts& o, vmig_s
     return VMIG_OK;
 }
 
+// ---------------------------------------------------------------------------------------------
+// vmig_compare_snapshot: the plan, the merge and the report are vmig_compare.cpp's; the layer files that need reading go
+// through the scrub's reader and data pass (one root: the layer, as version 0)
+int compare_body(CallScope& call, const char* layer_dir, const char* layer_table, const char* snap_dir, const char* snap_table,
+                 const char* report_path, const vmig_opts& o, vmig_stats* stats_out, vmig_compare_stats* cs_out)
+{
+    CallCtl* ctl = call.ctl;
+    const std::atomic<int>* cancel = call.cancel();
+    vmig_stats st; memset(&st, 0, sizeof st);
+    vmig_compare_stats cs; memset(&cs, 0, sizeof cs);
+    const uint64_t t_begin = now_ns();
+    if (cancel->load()) return fail(VMIG_ECANCELED, "the control was cancelled before the call started");
+    for (const char* d : {layer_dir, snap_dir}) {
+        struct stat sb;
+        if (stat(d, &sb) != 0 || !S_ISDIR(sb.st_mode)) return fail(VMIG_ENOTDIR, "%s is missing or not a directory", d);
+    }
+    BlockTable snap_tab, layer_tab;
+    const bool has_layer_tab = layer_table && *layer_table;
+    int rc = load_table(snap_table, "snapshot", o.block_bytes, &snap_tab);
+    if (!rc && has_layer_tab) rc = load_table(layer_table, "layer", o.block_bytes, &layer_tab);
+    if (rc) return rc;
+    std::vector<DeviceInfo> devs;                    // no CPU fallback: the GPU is there before anything is read
+    rc = ctx_select(o.gpu_mask, &devs);
+    if (rc) return rc;
+
+    // ---- walk both trees; the snapshot must be the tree its table describes
+    call.phase(VMIG_PHASE_WALK);
+    uint64_t t0 = now_ns();
+    const bool skip_hidden = (o.flags & VMIG_F_SKIP_HIDDEN_TOPDIRS) != 0;
+    Manifest snap, layer;
+    std::vector<uint64_t> snap_hashes;
+    rc = walk_tree(snap_dir, o.block_bytes, skip_hidden, &snap, cancel);
+    if (!rc) rc = match_table(snap, snap_tab, &snap_hashes);
+    if (!rc) rc = walk_tree(layer_dir, o.block_bytes, skip_hidden, &layer, cancel);
+    if (rc) return rc;
+    st.ns_walk = now_ns() - t0;
+
+    // ---- which layer files are read: shared and trusted ones are not
+    t0 = now_ns();
+    const BlockTable* ltab = has_layer_tab ? &layer_tab : nullptr;
+    ComparePlan plan;
+    rc = compare_plan(layer_dir, layer, snap, ltab, o.block_bytes, &plan);
+    if (rc) return rc;
+    ctl->bytes_total.store(plan.bytes_read); ctl->blocks_total.store(plan.blocks_read);
+    std::vector<int> root_fds(1, -1);
+    if (!plan.inodes.empty()) {
+        root_fds[0] = open(layer_dir, O_RDONLY | O_DIRECTORY | O_CLOEXEC);
+        if (root_fds[0] < 0) return fail(VMIG_ESRCCHANGED, "open %s: %s", layer_dir, errno_str(errno).c_str());
+    }
+    ScrubReader reader;
+    reader.root_fds = root_fds; reader.inodes = &plan.inodes; reader.direct = (o.flags & VMIG_F_DIRECT_IO) != 0;
+    reader.init();
+    ScrubIO io; io.r = &reader; io.block_bytes = o.block_bytes;
+    std::vector<BlockSpan> spans;
+    for (uint32_t u = 0; u < plan.inodes.size(); u++) spans.push_back({u, plan.inodes[u].size, plan.inodes[u].first_block, plan.inodes[u].n_blocks});
+    std::vector<BlockRef> blocks; blocks.reserve(plan.blocks_read);
+    interleave_blocks(spans, o.block_bytes, &blocks);
+    st.ns_plan = now_ns() - t0;
+
+    // ---- the data pass: K1 over every block of the distinct layer inodes that need reading, once
+    call.phase(VMIG_PHASE_DATA);
+    if (cancel->load()) { if (root_fds[0] >= 0) close(root_fds[0]); return fail(VMIG_ECANCELED, "before the data pass"); }
+    t0 = now_ns();
+    std::vector<uint64_t> read_hashes(plan.blocks_read, 0);
+    rc = run_blocks(blocks, &io, false, true, o, read_hashes.data(), &st, ctl, false);
+    reader.close_all();
+    if (root_fds[0] >= 0) close(root_fds[0]);
+    st.ns_data = now_ns() - t0;
+    if (rc) return rc;
+    for (uint32_t u = 0; u < plan.inodes.size(); u++)
+        if (reader.unreadable(u)) return fail(VMIG_EIO, "layer file %s: %s", plan.inodes[u].rel.c_str(), reader.why(u).c_str());
+
+    // ---- the findings, compared on the host (8 bytes per block), and the report
+    t0 = now_ns();
+    const std::vector<const uint64_t*> layer_hashes = compare_layer_hashes(plan, layer, snap, snap_hashes, ltab, read_hashes);
+    std::vector<CompareFinding> findings;
+    CompareCounts c;
+    compare_merge(layer, snap, snap_hashes, layer_hashes, o.block_bytes, (o.flags & VMIG_F_MTIME_NS) != 0,
+                  (o.flags & VMIG_F_NO_METADATA) != 0, &findings, &c);
+    if (report_path && *report_path) {
+        std::string raw;
+        for (const CompareFinding& f : findings) raw += compare_format(f);
+        rc = report_store(report_path, raw, "compare report", cancel);
+        if (rc) return rc;
+    }
+    st.ns_table = now_ns() - t0;
+    cs.paths_added = c.paths_added; cs.paths_removed = c.paths_removed; cs.paths_changed = c.paths_changed;
+    cs.files_changed = c.files_changed; cs.blocks_changed = c.blocks_changed; cs.bytes_restore = c.bytes_restore;
+    cs.files_read = plan.inodes.size(); cs.bytes_read = plan.bytes_read;
+    cs.files_trusted = plan.files_trusted; cs.files_shared = plan.files_shared;
+    st.files_direct = reader.n_direct.load();
+    st.bytes_total = plan.bytes_read; st.blocks_total = plan.blocks_read; st.files = plan.inodes.size();
+    st.ns_total = now_ns() - t_begin;
+    if (stats_out) *stats_out = st;
+    if (cs_out) *cs_out = cs;
+    return VMIG_OK;
+}
+
 }  // namespace
 
 // =============================================================================================
@@ -1484,6 +1583,23 @@ int vmig_retire_versions(uint32_t n_retire, const char* const* retire_dirs, cons
     rc = call.attach(o.ctl);
     if (rc) return rc;
     return call.finish(retire_body(call, a, o, stats, retire_stats));
+}
+int vmig_compare_snapshot(const char* layer_dir, const char* layer_table, const char* snap_dir, const char* snap_table,
+                          const char* report_path, const vmig_opts* opts, vmig_stats* stats, vmig_compare_stats* cmp_stats)
+{
+    if (!layer_dir || !*layer_dir) return fail(VMIG_EINVAL, "layer_dir is NULL/empty");
+    if (!snap_dir || !*snap_dir) return fail(VMIG_EINVAL, "snap_dir is NULL/empty");
+    if (!snap_table || !*snap_table) return fail(VMIG_EINVAL, "snap_table is NULL/empty: a layer is only compared with a snapshot through its block table");
+    const vmig_opts o = norm_opts(opts);                     // VMIG_CUFILE=1 in the environment is refused too
+    const uint32_t allowed = VMIG_F_DIRECT_IO | VMIG_F_SKIP_HIDDEN_TOPDIRS | VMIG_F_MTIME_NS | VMIG_F_NO_METADATA;
+    if (o.flags & ~allowed)
+        return fail(VMIG_EINVAL, "flags 0x%x: a compare takes only VMIG_F_DIRECT_IO, VMIG_F_SKIP_HIDDEN_TOPDIRS, VMIG_F_MTIME_NS and VMIG_F_NO_METADATA", o.flags & ~allowed);
+    int rc = check_block_bytes(o);
+    if (rc) return rc;
+    CallScope call;
+    rc = call.attach(o.ctl);
+    if (rc) return rc;
+    return call.finish(compare_body(call, layer_dir, layer_table, snap_dir, snap_table, report_path, o, stats, cmp_stats));
 }
 int vmig_copy_dir(const char* src_dir, const char* dst_dir) { return migrate_tree_impl(src_dir, dst_dir, nullptr, nullptr, nullptr, nullptr); }
 int vmig_move_dir(const char* src_dir, const char* dst_dir)

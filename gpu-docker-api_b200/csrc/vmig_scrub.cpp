@@ -40,7 +40,7 @@ size_t scrub_merge_table(uint32_t version, const Manifest& man, const BlockTable
     return n;
 }
 
-int scrub_group_inodes(const std::vector<const Manifest*>& mans, const std::vector<std::vector<int64_t>>& tab_of,
+int scrub_group_inodes(const std::vector<const Manifest*>& mans, const std::vector<std::vector<int64_t>>& sel,
                        uint32_t block_bytes, std::vector<ScrubInode>* inodes, std::vector<std::vector<uint32_t>>* inode_of)
 {
     inodes->clear();
@@ -51,9 +51,9 @@ int scrub_group_inodes(const std::vector<const Manifest*>& mans, const std::vect
         if (!mans[v]) continue;
         const Manifest& m = *mans[v];
         (*inode_of)[v].assign(m.files.size(), kNoInode);
-        for (size_t f = 0; f < m.files.size() && f < tab_of[v].size(); f++) {
+        for (size_t f = 0; f < m.files.size() && f < sel[v].size(); f++) {
             const Entry& e = m.files[f];
-            if (tab_of[v][f] < 0 || e.size == 0) continue;
+            if (sel[v][f] < 0 || e.size == 0) continue;
             auto it = seen.find({e.dev, e.ino});
             uint32_t u;
             if (it == seen.end()) {
@@ -123,11 +123,9 @@ void scrub_sort(std::vector<ScrubFinding>* v)
     });
 }
 
-int scrub_report_store(const std::string& path, const std::vector<ScrubFinding>& v, const std::atomic<int>* cancel)
+int report_store(const std::string& path, const std::string& raw, const char* what, const std::atomic<int>* cancel)
 {
-    if (cancel && cancel->load()) return fail(VMIG_ECANCELED, "cancelled before the scrub report %s was written", path.c_str());
-    std::string raw;
-    for (const ScrubFinding& f : v) raw += scrub_format(f);
+    if (cancel && cancel->load()) return fail(VMIG_ECANCELED, "cancelled before the %s %s was written", what, path.c_str());
     const std::string tmp = path + ".tmp." + std::to_string((long)getpid()) + "." + std::to_string((long)syscall(SYS_gettid));
     int fd = open(tmp.c_str(), O_WRONLY | O_CREAT | O_TRUNC | O_CLOEXEC, 0644);
     if (fd < 0) return fail(VMIG_EIO, "create %s: %s", tmp.c_str(), errno_str(errno).c_str());
@@ -139,9 +137,16 @@ int scrub_report_store(const std::string& path, const std::vector<ScrubFinding>&
     }
     if (fsync(fd) != 0) { const int e = errno; close(fd); unlink(tmp.c_str()); return fail(VMIG_EIO, "fsync %s: %s", tmp.c_str(), errno_str(e).c_str()); }
     close(fd);
-    if (cancel && cancel->load()) { unlink(tmp.c_str()); return fail(VMIG_ECANCELED, "cancelled before the scrub report %s was renamed into place", path.c_str()); }
+    if (cancel && cancel->load()) { unlink(tmp.c_str()); return fail(VMIG_ECANCELED, "cancelled before the %s %s was renamed into place", what, path.c_str()); }
     if (rename(tmp.c_str(), path.c_str()) != 0) { const int e = errno; unlink(tmp.c_str()); return fail(VMIG_EIO, "rename %s: %s", path.c_str(), errno_str(e).c_str()); }
     return VMIG_OK;
+}
+
+int scrub_report_store(const std::string& path, const std::vector<ScrubFinding>& v, const std::atomic<int>* cancel)
+{
+    std::string raw;
+    for (const ScrubFinding& f : v) raw += scrub_format(f);
+    return report_store(path, raw, "scrub report", cancel);
 }
 
 // ---------------------------------------------------------------------------------------------

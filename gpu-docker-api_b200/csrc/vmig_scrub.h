@@ -42,10 +42,11 @@ size_t scrub_merge_table(uint32_t version, const Manifest& man, const BlockTable
 struct ScrubInode { uint64_t dev, ino, size, first_block, n_blocks; uint32_t version; std::string rel; };
 static constexpr uint32_t kNoInode = 0xFFFFFFFFu;
 
-// Group the matched, non-empty regular files of every version (tab_of[v][f] >= 0; mans[v] may be null for a version
-// that was not walked) by (dev, ino).  (*inode_of)[v][f] is the inode's index, kNoInode where the path is not read.
-// Two paths of one inode with different sizes mean the store changed between the walks: VMIG_ESRCCHANGED.
-int scrub_group_inodes(const std::vector<const Manifest*>& mans, const std::vector<std::vector<int64_t>>& tab_of,
+// Group the selected, non-empty regular files of every version (sel[v][f] >= 0: for the scrub, the table index of a file
+// that matches its record; for vmig_compare_snapshot, a layer file to read; mans[v] may be null for a version that was
+// not walked) by (dev, ino).  (*inode_of)[v][f] is the inode's index, kNoInode where the path is not read.
+// Two paths of one inode with different sizes mean the tree changed between the walks: VMIG_ESRCCHANGED.
+int scrub_group_inodes(const std::vector<const Manifest*>& mans, const std::vector<std::vector<int64_t>>& sel,
                        uint32_t block_bytes, std::vector<ScrubInode>* inodes, std::vector<std::vector<uint32_t>>* inode_of);
 
 // Report paths: '\' -> "\\", tab -> "\t", newline -> "\n", any other byte below 0x20 -> "\xHH" (two lower-case hex
@@ -56,8 +57,11 @@ bool scrub_unescape(const std::string& s, std::string* out);
 std::string scrub_format(const ScrubFinding& f);
 // by version, then path (bytewise), then block ("-" first)
 void scrub_sort(std::vector<ScrubFinding>* v);
-// Atomic, like a block table: path.tmp.<pid>.<tid>, fsync, rename.  A non-zero *cancel before the rename removes the
-// .tmp and returns VMIG_ECANCELED; any failure leaves no .tmp.
+// A report file (raw: its lines), written atomically like a block table: path.tmp.<pid>.<tid>, fsync, rename.  `what`
+// names it in errors.  A non-zero *cancel before the rename removes the .tmp and returns VMIG_ECANCELED; any failure
+// leaves no .tmp.  vmig_scrub_store and vmig_compare_snapshot write their reports through it.
+int report_store(const std::string& path, const std::string& raw, const char* what, const std::atomic<int>* cancel);
+// The scrub's findings, formatted, through report_store
 int scrub_report_store(const std::string& path, const std::vector<ScrubFinding>& v, const std::atomic<int>* cancel);
 
 // The scrub's source of block bytes.  An inode is opened lazily beneath the root of the version that names it first

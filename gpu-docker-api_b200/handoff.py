@@ -21,8 +21,9 @@ from typing import Callable, Optional
 
 import threading
 
-from . import (F_PRUNE, F_VERIFY, VMIG_ECANCELED, Ctl, GetContainerMergedLayer, GetVolumeMountPoint, VmigError, manifest,
-               migrate_tree, restore_paths, restore_tree, retire_versions, scrub_store, snapshot_tree)
+from . import (F_PRUNE, F_VERIFY, VMIG_ECANCELED, Ctl, GetContainerMergedLayer, GetVolumeMountPoint, VmigError,
+               compare_snapshot, manifest, migrate_tree, restore_paths, restore_tree, retire_versions, scrub_store,
+               snapshot_tree)
 
 log = logging.getLogger("vmig.handoff")
 _root: dict = {"cwd": None}
@@ -196,6 +197,23 @@ def RestorePathsFromSnapshot(targetCtrVersionName: str, container: str, paths: l
     data, table = snapshotPaths(targetCtrVersionName)
     upper = GetContainerMergedLayer(container)
     return RestorePathsVerified(data, table, upper, seedTable, paths)
+
+
+def CompareWithVersion(targetCtrVersionName: str, container: str, report) -> dict:
+    """N1: list in `report` every difference between `container`'s layer and version `target`: what RollbackFromSnapshot
+    would change, and the paths RestorePathsFromSnapshot could be given.  The snapshot's table stands for its data, which
+    is not read; nothing is written but the report.  When the container's own version directory has no diff/, its
+    blocks.vmig is the table HandoffCopy wrote for the running layer: files still as it recorded them are not read, so
+    "what changed since the hand-off" costs only the files the tenant touched.
+      - No REST route is added; the control plane stays as it is."""
+    data, table = snapshotPaths(targetCtrVersionName)
+    upper = GetContainerMergedLayer(container)
+    ownData, ownTable = snapshotPaths(container)
+    layerTable = None
+    if not ownData.exists():
+        if ownTable.exists():
+            layerTable = ownTable
+    return compare_snapshot(upper, data, table, report, layerTable)
 
 
 def HandoffCopy(oldContainer: str, newContainer: str, pause: Callable[[str], None], resume: Callable[[str], None],

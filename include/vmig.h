@@ -405,6 +405,81 @@ int vmig_retire_versions(uint32_t n_retire, const char* const* retire_dirs, cons
                          const vmig_opts* opts /*nullable*/, vmig_stats* stats /*nullable*/,
                          vmig_retire_stats* retire_stats /*nullable*/);
 
+/* Comparison of a layer with a version snapshot: what vmig_compare_snapshot found and read. */
+typedef struct vmig_compare_stats {
+    uint64_t paths_added, paths_removed;   /* entries only in the layer / only in the snapshot (each path beneath counts) */
+    uint64_t paths_changed;                /* paths in both trees with at least one finding                            */
+    uint64_t files_changed;                /* regular file in both trees with a `resized` or `block` finding          */
+    uint64_t blocks_changed;               /* `block` findings                                                          */
+    uint64_t bytes_restore;                /* snapshot bytes a rollback must bring back (rule below)                   */
+    uint64_t files_read, bytes_read;       /* distinct layer inodes hashed through the GPU                              */
+    uint64_t files_trusted;                /* layer paths whose hashes came from layer_table, not from a read           */
+    uint64_t files_shared;                 /* layer paths that are the snapshot path's own inode: not read              */
+    uint64_t reserved[4];
+} vmig_compare_stats;
+
+/* List every difference between the layer layer_dir and the version snapshot snap_dir (written with its block table
+ * snap_table by vmig_snapshot_tree): everything vmig_restore_tree(snap_dir, snap_table, layer_dir, ..., VMIG_F_PRUNE |
+ * flags) would change -- entry type, permission bits, owner, mtime, symlink target, device numbers, hard-link grouping
+ * inside the tree and regular-file contents.  It previews a checked rollback.  Nothing is written anywhere except
+ * report_path, and no inode's ctime moves (in either tree or table), so every identity the next incremental snapshot
+ * or diff pass trusts stays valid.
+ *   - Refusals, in this order, each before anything is read or written: VMIG_EINVAL (layer_dir, snap_dir or snap_table
+ *     NULL or empty; flags other than VMIG_F_DIRECT_IO | VMIG_F_SKIP_HIDDEN_TOPDIRS | VMIG_F_MTIME_NS |
+ *     VMIG_F_NO_METADATA; bad block_bytes); a control cancelled before the call: VMIG_ECANCELED; VMIG_ENOTDIR (either
+ *     directory missing or not a directory); VMIG_ETABLE (either table does not load -- formats 01 and 02 -- or its
+ *     block_bytes differs from the call's); VMIG_ENOGPU (no CPU fallback, even when no layer file needs reading).
+ *   - Snapshot side: snap_dir is walked for metadata only and must match snap_table in paths and sizes, as a restore
+ *     requires at plan time; otherwise VMIG_ECORRUPT with the restore's message, and no report.  None of its file data
+ *     is read: its regular-file contents are taken to be its table's hashes.  A snapshot whose bytes rotted without a
+ *     change in size compares as its table says; finding that is vmig_scrub_store's job.
+ *   - Layer side: layer_dir is walked as a migration's source (no symlink followed).  A layer regular file needs its
+ *     block hashes when it and the snapshot's regular file at the same path both have at least one block, and takes
+ *     them from the first of these that applies:
+ *       shared   the layer path is the snapshot path's own inode (same st_dev, st_ino and size), as versions of one
+ *                incremental store share inodes: equal by construction, not read (files_shared);
+ *       trusted  layer_table (nullable) records the path and the file is still that record's inode, size and ctime --
+ *                the in-place diff path's trust rule: not read (files_trusted);
+ *       read     otherwise: each distinct inode read once through the block pipeline in hash-only mode, lanes, GPUs and
+ *                VMIG_F_DIRECT_IO as in vmig_scrub_store (files_read, bytes_read).  An inode that is no longer the walked
+ *                one (other inode, type or size, or shorter than its blocks) is VMIG_ESRCCHANGED; one that cannot be
+ *                opened or read is VMIG_EIO.
+ *     Files only in the layer are never read.  The block comparison is one 8-byte compare per block on the host.
+ *   - Both walks take the call's VMIG_F_SKIP_HIDDEN_TOPDIRS.  Sockets are skipped, as everywhere in the engine; xattrs
+ *     are not compared, as the engine drops them.
+ *   - report_path (nullable): one line per finding, sorted by path (bytewise), then kind in the order below, then block:
+ *       <kind>\t<path>\t<block|->\t<layer|->\t<snap|->\n
+ *     added     the path is only in the layer (every entry beneath an added directory is listed too)        - / -
+ *     removed   the path is only in the snapshot (likewise)                                                - / -
+ *     type      both have the path, as different S_IFMT                                one letter each of f d l c b p
+ *     resized   regular in both, different sizes                                                   decimal sizes
+ *     block     regular in both; block r is below both block counts and its (length, XXH64) differs   16 hex digits
+ *     target    symlink in both, different targets                                               escaped targets
+ *     rdev      char or block device in both, different device numbers                                major:minor
+ *     hardlink  regular in both; the set of other paths of the same tree sharing its inode differs (a link held
+ *               outside a tree does not count)          the group's smallest path in each tree, "-" when alone
+ *     mode      same type in both, different permission bits (07777)                          four octal digits
+ *     owner     same type in both, different uid or gid                                                 uid:gid
+ *     mtime     same type in both, different mtime: whole seconds (tar's precision, and what a default snapshot
+ *               keeps), nanoseconds with VMIG_F_MTIME_NS                                   sec or sec.nnnnnnnnn
+ *     With VMIG_F_NO_METADATA mode, owner and mtime are not compared.  The root is path "." and takes only mode,
+ *     owner and mtime findings.  Paths and targets are escaped as in the vmig_scrub_store report.  Written like a
+ *     table: tmp, fsync, rename; an empty file when there is no difference.  A failed or cancelled call leaves
+ *     report_path as it was, with no .tmp beside it.
+ *   - bytes_restore, summed over the snapshot's regular-file paths (each path of a hard-link group once): where the
+ *     layer has a regular file at the path, the snapshot lengths of the blocks past the layer file's last block or
+ *     whose (length, hash) differs; otherwise the snapshot file's whole size.  It is the content a rollback has to
+ *     bring back.  A rollback without a trusted seed table (prior_table) copies more than this: whole files.
+ *   - Control: vmig_opts.ctl as for the tree calls; phases WALK, DATA, DONE; a cancel is honoured per directory of the
+ *     walks, in the block pipeline and before the report is renamed into place.  bytes_total / blocks_total are the
+ *     bytes and blocks to be read.  stats (nullable): the vmig_stats of the data pass (bytes_h2d == bytes_read, 0 when
+ *     nothing needs reading).  cmp_stats (nullable): the counters above, written on success. */
+int vmig_compare_snapshot(const char* layer_dir, const char* layer_table /*nullable*/,
+                          const char* snap_dir, const char* snap_table,
+                          const char* report_path /*nullable*/,
+                          const vmig_opts* opts /*nullable*/, vmig_stats* stats /*nullable*/,
+                          vmig_compare_stats* cmp_stats /*nullable*/);
+
 /* utils.CopyDir(src, dest) (reference utils/copy.go:21-27) == vmig_migrate_tree with defaults. */
 int vmig_copy_dir(const char* src_dir, const char* dst_dir);
 
@@ -427,7 +502,7 @@ void vmig_host_free(void* p);
 
 /* ---- cancellation and progress ------------------------------------------------------------------
  * A control is a numeric id (cgo passes it in vmig_opts.ctl without any pointer rules).  It serves the entry points
- * that take vmig_opts: vmig_migrate_tree, vmig_restore_tree, vmig_restore_paths, vmig_snapshot_tree, vmig_scrub_store, vmig_retire_versions and vmig_migrate_buffer (a caller that
+ * that take vmig_opts: vmig_migrate_tree, vmig_restore_tree, vmig_restore_paths, vmig_snapshot_tree, vmig_scrub_store, vmig_retire_versions, vmig_compare_snapshot and vmig_migrate_buffer (a caller that
  * wants to cancel a copy or a move calls vmig_migrate_tree with the flags vmig_copy_dir / vmig_move_dir use).  One
  * control serves one call at a time: attaching it to a second concurrent call fails with VMIG_EINVAL.  The engine has
  * no deadline of its own; a deadline is the caller's timer calling vmig_ctl_cancel.

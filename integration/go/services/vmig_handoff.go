@@ -247,6 +247,29 @@ func RestorePathsFromSnapshot(targetCtrVersionName, container string, paths []st
 	return errors.WithMessagef(utils.RestorePathsVerified(data, table, upper, seedTable, paths), "restore of %d paths from %s failed", len(paths), targetCtrVersionName)
 }
 
+// N1 -- CompareWithVersion lists in report every difference between container's layer and version `target`: what
+// RollbackFromSnapshot would change, and the paths RestorePathsFromSnapshot could be given.  The snapshot's table stands
+// for its data, which is not read; nothing is written but the report.  When the container's own version directory has no
+// diff/, its blocks.vmig is the table HandoffCopy wrote for the running layer: files still as it recorded them are not
+// read, so "what changed since the hand-off" costs only the files the tenant touched.
+//   - No REST route is added; the control plane stays as it is.
+func CompareWithVersion(targetCtrVersionName, container, report string) (utils.CompareStats, error) {
+	data, table := snapshotPaths(targetCtrVersionName)
+	upper, err := utils.GetContainerMergedLayer(container)
+	if err != nil {
+		return utils.CompareStats{}, errors.WithMessagef(err, "utils.GetContainerMergedLayer failed, container: %s", container)
+	}
+	ownData, ownTable := snapshotPaths(container)
+	layerTable := ""
+	if _, err := os.Stat(ownData); os.IsNotExist(err) {
+		if _, err := os.Stat(ownTable); err == nil {
+			layerTable = ownTable
+		}
+	}
+	st, err := utils.CompareWithSnapshot(upper, layerTable, data, table, report)
+	return st, errors.WithMessagef(err, "compare of %s with %s failed", container, targetCtrVersionName)
+}
+
 // N2 -- HandoffCopy replaces utils.CopyOldMergedToNewContainerMerged in PatchContainer (replicaset.go:333):
 // the old container keeps running during pass 1 (the bulk of the bytes), is paused for pass 2, which re-reads
 // the source and moves only the blocks whose hash changed in between, and stays paused until the caller has

@@ -216,6 +216,67 @@ func ScrubSnapshotsContext(ctx context.Context, snapDirs, snapTables []string, r
 	return out, nil
 }
 
+// CompareStats is what CompareWithSnapshot found and read (vmig_compare_stats).
+type CompareStats struct {
+	PathsAdded, PathsRemoved, PathsChanged, FilesChanged, BlocksChanged uint64
+	BytesRestore                                                         uint64 // snapshot bytes a rollback must bring back
+	FilesRead, BytesRead, FilesTrusted, FilesShared                      uint64
+}
+
+// CompareWithSnapshot lists every difference between the layer and the snapshot snapDir (checked against snapTable)
+// in report: everything a rollback of the layer to that snapshot would change (vmig_compare_snapshot).  Nothing else is
+// written and no ctime moves.  layerTable ("" for none) is a table of the layer whose records still vouch for their
+// files; those files are not read.  The snapshot's file data is never read: its table stands for it.
+func CompareWithSnapshot(layer, layerTable, snapDir, snapTable, report string) (CompareStats, error) {
+	return CompareWithSnapshotContext(context.Background(), layer, layerTable, snapDir, snapTable, report)
+}
+
+// CompareWithSnapshotContext is CompareWithSnapshot that stops when ctx is done (see CopyDirDiffContext); no report is
+// written then.
+func CompareWithSnapshotContext(ctx context.Context, layer, layerTable, snapDir, snapTable, report string) (CompareStats, error) {
+	cl, cs, ct := C.CString(layer), C.CString(snapDir), C.CString(snapTable)
+	defer C.free(unsafe.Pointer(cl))
+	defer C.free(unsafe.Pointer(cs))
+	defer C.free(unsafe.Pointer(ct))
+	var clt, cr *C.char
+	if layerTable != "" {
+		clt = C.CString(layerTable)
+		defer C.free(unsafe.Pointer(clt))
+	}
+	if report != "" {
+		cr = C.CString(report)
+		defer C.free(unsafe.Pointer(cr))
+	}
+	var st C.vmig_stats
+	var cmp C.vmig_compare_stats
+	var o C.vmig_opts
+	var id C.uint32_t
+	if err := lockedCall("vmig_ctl_open", func() C.int { return C.vmig_ctl_open(&id) }); err != nil {
+		return CompareStats{}, err
+	}
+	defer C.vmig_ctl_close(id)
+	stop := context.AfterFunc(ctx, func() { C.vmig_ctl_cancel(id) })
+	defer stop()
+	o.ctl = id
+	var rc C.int
+	err := lockedCall("vmig_compare_snapshot", func() C.int {
+		rc = C.vmig_compare_snapshot(cl, clt, cs, ct, cr, &o, &st, &cmp)
+		return rc
+	})
+	if rc == C.VMIG_ECANCELED && ctx.Err() != nil {
+		return CompareStats{}, fmt.Errorf("%w: %v", ctx.Err(), err)
+	}
+	if err != nil {
+		return CompareStats{}, err
+	}
+	out := CompareStats{uint64(cmp.paths_added), uint64(cmp.paths_removed), uint64(cmp.paths_changed), uint64(cmp.files_changed),
+		uint64(cmp.blocks_changed), uint64(cmp.bytes_restore), uint64(cmp.files_read), uint64(cmp.bytes_read),
+		uint64(cmp.files_trusted), uint64(cmp.files_shared)}
+	log.Infof("vmig: compared %s with %s: %d added, %d removed, %d changed, %d bytes to restore; %d bytes read, %d files trusted, %d shared",
+		layer, snapDir, out.PathsAdded, out.PathsRemoved, out.PathsChanged, out.BytesRestore, out.BytesRead, out.FilesTrusted, out.FilesShared)
+	return out, nil
+}
+
 // RetireSnapshots removes the snapshots retireDirs[i] with their tables retireTables[i] and keeps keepDirs[i] /
 // keepTables[i] usable as bases (vmig_retire_versions): each retired table goes first, then its tree, never following
 // a symlink; then the kept tables' records whose ctime the removal moved are re-verified on the GPU and re-recorded.

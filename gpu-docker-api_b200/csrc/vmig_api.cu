@@ -100,6 +100,16 @@ public:
     }
 };
 
+// body(call) as one data-path call attached to control id (0: a private one)
+template <class Body>
+int in_call(uint32_t id, Body body)
+{
+    CallScope call;
+    const int rc = call.attach(id);
+    if (rc) return rc;
+    return call.finish(body(call));
+}
+
 // The block pipeline's first-error latch, reachable by CallCtl::cancel while run_blocks runs
 struct LatchLink {
     CallCtl* c;
@@ -457,14 +467,14 @@ public:
         if (src_root_fd < 0) return fail(VMIG_EIO, "open %s: %s", src_root.c_str(), errno_str(errno).c_str());
         return VMIG_OK;
     }
-    ~FileIO() { if (src_root_fd >= 0) close(src_root_fd); }
-    void close_all(size_t n) {
-        for (size_t i = 0; i < n; i++) {
+    ~FileIO() {
+        for (size_t i = 0; m && i < m->files.size(); i++) {     // what a failed data pass left open
             void* h = fs[i].s_cfh.exchange(nullptr); if (h) cufile_handle_close(h);
             h = fs[i].d_cfh.exchange(nullptr); if (h) cufile_handle_close(h);
             int a = fs[i].sfd.exchange(-1); if (a >= 0) close(a);
             int b = fs[i].dfd.exchange(-1); if (b >= 0) close(b);
         }
+        if (src_root_fd >= 0) close(src_root_fd);
     }
 };
 
@@ -688,7 +698,7 @@ int verify_pass(CallScope& call, const vmig_opts& o, const FileIO& io, const std
     std::vector<uint64_t> vh(man.n_blocks, 0);
     vmig_stats vst; memset(&vst, 0, sizeof vst);
     rc = run_blocks(vblocks, &vio, false, true, o, vh.data(), &vst, call.ctl, true);
-    if (rc) { std::string keep = last_error_cstr(); vio.close_all(man.files.size()); set_last_error_str(keep); return rc; }
+    if (rc) return rc;
     st->kernel_launches += vst.kernel_launches; st->ms_kernel += vst.ms_kernel; st->bytes_h2d += vst.bytes_h2d;
     for (auto& b : vblocks)
         if (vh[b.table_idx] != hashes[b.table_idx])
@@ -828,7 +838,7 @@ int tree_passes(CallScope& call, const std::string& src, const std::string& dst,
     t0 = now_ns();
     rc = run_blocks(plan.blocks, &io, skip_mode, hash_only, o, hashes.data(), &st, call.ctl, false, expect.empty() ? nullptr : expect.data());
     st.ns_data = now_ns() - t0;
-    if (rc) { std::string keep = last_error_cstr(); io.close_all(man.files.size()); set_last_error_str(keep); return rc; }
+    if (rc) return rc;
 
     t0 = now_ns();
     call.phase(VMIG_PHASE_META);
@@ -982,10 +992,9 @@ int migrate_tree_impl(const char* src_dir, const char* dst_dir, const char* prio
                       const SnapshotArgs* snapshot = nullptr)
 {
     const vmig_opts o = norm_opts(opts_in);
-    CallScope call;
-    const int rc = call.attach(o.ctl);
-    if (rc) return rc;
-    return call.finish(migrate_tree_body(call, src_dir, dst_dir, prior_path, out_path, o, stats_out, snap_path, snapshot));
+    return in_call(o.ctl, [&](CallScope& call) {
+        return migrate_tree_body(call, src_dir, dst_dir, prior_path, out_path, o, stats_out, snap_path, snapshot);
+    });
 }
 
 // vmig_snapshot_tree: a base directory equal to the destination, or either one inside the other, is refused -- a
@@ -1004,25 +1013,51 @@ int check_snapshot_paths(const char* dst_dir, const char* base_dir)
 }
 
 // ---------------------------------------------------------------------------------------------
-// vmig_scrub_store: the block pipeline reads each distinct inode of the store through a ScrubReader (vmig_scrub.h), in
-// hash-only mode; block b of inode u is BlockRef{file = u, table_idx = its index in the scrub's hash array}
-class ScrubIO : public BlockIO {
-public:
-    ScrubReader* r = nullptr;
-    uint32_t block_bytes = 4u << 20;
-    int read_block(const BlockRef& b, uint8_t* dst) override { return r->read(b.file, b.file_off, b.len, dst); }
-    int write_block(const BlockRef&, const uint8_t*) override { return fail(VMIG_EINVAL, "a scrub writes nothing"); }
-    uint32_t slot_align() override { return r->direct ? kSector : 512; }
-    std::string block_name(const BlockRef& b) override {
-        const ScrubInode& I = (*r->inodes)[b.file];
-        return I.rel + " (version " + std::to_string(I.version) + ") block " + std::to_string(b.file_off / block_bytes);
+// vmig_scrub_store, vmig_retire_versions and vmig_compare_snapshot read each distinct inode once (ScrubInode, vmig_scrub.h)
+
+// The root directories of a call's versions, opened as the call needs them and closed with the holder
+struct VersionRoots {
+    std::vector<int> fds;                            // -1: not opened
+    explicit VersionRoots(size_t n) : fds(n, -1) {}
+    VersionRoots(const VersionRoots&) = delete;
+    ~VersionRoots() { for (int fd : fds) if (fd >= 0) close(fd); }
+    int open(size_t v, const char* dir) {
+        fds[v] = ::open(dir, O_RDONLY | O_DIRECTORY | O_CLOEXEC);
+        return fds[v] >= 0 ? VMIG_OK : fail(VMIG_ESRCCHANGED, "open %s: %s", dir, errno_str(errno).c_str());
     }
 };
+
+// The data pass over inodes: every block through *reader (each inode opened beneath roots[its version]) in a migration's
+// block order, hashed by K1 in hash-only mode into *hashes at the inodes' block ranges.  What an unreadable inode means
+// is the caller's (reader->unreadable).  Sets the call's progress totals and st's data-pass fields.
+int inode_pass(CallScope& call, const vmig_opts& o, const std::vector<int>& roots, const std::vector<ScrubInode>& inodes,
+               ScrubReader* reader, std::vector<uint64_t>* hashes, vmig_stats* st)
+{
+    const uint64_t t0 = now_ns();
+    uint64_t bytes = 0, n_blocks = 0;
+    for (const ScrubInode& I : inodes) { bytes += I.size; n_blocks += I.n_blocks; }
+    call.ctl->bytes_total.store(bytes); call.ctl->blocks_total.store(n_blocks);
+    reader->root_fds = roots; reader->inodes = &inodes; reader->direct = (o.flags & VMIG_F_DIRECT_IO) != 0;
+    reader->block_bytes = o.block_bytes;
+    reader->init();
+    std::vector<BlockSpan> spans;
+    for (uint32_t u = 0; u < inodes.size(); u++) spans.push_back({u, inodes[u].size, inodes[u].first_block, inodes[u].n_blocks});
+    std::vector<BlockRef> blocks; blocks.reserve(n_blocks);
+    interleave_blocks(spans, o.block_bytes, &blocks);
+    call.phase(VMIG_PHASE_DATA);
+    if (call.cancel()->load()) return fail(VMIG_ECANCELED, "before the data pass");
+    hashes->assign(n_blocks, 0);
+    const int rc = run_blocks(blocks, reader, false, true, o, hashes->data(), st, call.ctl, false);
+    reader->close_all();
+    st->ns_data = now_ns() - t0;
+    st->files_direct = reader->n_direct.load();
+    st->bytes_total = bytes; st->blocks_total = n_blocks; st->files = inodes.size();
+    return rc;
+}
 
 int scrub_body(CallScope& call, uint32_t n, const char* const* dirs, const char* const* tables, const char* report_path,
                int32_t* verdicts_out, const vmig_opts& o, vmig_stats* stats_out, vmig_scrub_stats* ss_out)
 {
-    CallCtl* ctl = call.ctl;
     const std::atomic<int>* cancel = call.cancel();
     vmig_stats st; memset(&st, 0, sizeof st);
     vmig_scrub_stats ss; memset(&ss, 0, sizeof ss);
@@ -1057,43 +1092,23 @@ int scrub_body(CallScope& call, uint32_t n, const char* const* dirs, const char*
     }
     st.ns_walk = now_ns() - t0;
 
-    // ---- one block list over the distinct inodes
+    // ---- the distinct inodes, and the roots they are opened beneath
     t0 = now_ns();
     std::vector<ScrubInode> inodes;
     std::vector<std::vector<uint32_t>> inode_of;
     rc = scrub_group_inodes(walked, tab_of, o.block_bytes, &inodes, &inode_of);
     if (rc) return rc;
-    uint64_t n_blocks = 0;
-    for (const ScrubInode& I : inodes) { ss.bytes_unique += I.size; n_blocks += I.n_blocks; }
-    ctl->bytes_total.store(ss.bytes_unique); ctl->blocks_total.store(n_blocks);
-    std::vector<int> root_fds(n, -1);
-    auto close_roots = [&] { for (int& fd : root_fds) if (fd >= 0) { close(fd); fd = -1; } };
+    VersionRoots roots(n);
     for (const ScrubInode& I : inodes)
-        if (root_fds[I.version] < 0) {
-            root_fds[I.version] = open(dirs[I.version], O_RDONLY | O_DIRECTORY | O_CLOEXEC);
-            if (root_fds[I.version] < 0) { const int e = errno; close_roots(); return fail(VMIG_ESRCCHANGED, "open %s: %s", dirs[I.version], errno_str(e).c_str()); }
-        }
-    ScrubReader reader;
-    reader.root_fds = root_fds; reader.inodes = &inodes; reader.direct = (o.flags & VMIG_F_DIRECT_IO) != 0;
-    reader.init();
-    ScrubIO io; io.r = &reader; io.block_bytes = o.block_bytes;
-    // the block order of a migration
-    std::vector<BlockSpan> spans;
-    for (uint32_t u = 0; u < inodes.size(); u++) spans.push_back({u, inodes[u].size, inodes[u].first_block, inodes[u].n_blocks});
-    std::vector<BlockRef> blocks; blocks.reserve(n_blocks);
-    interleave_blocks(spans, o.block_bytes, &blocks);
+        if (roots.fds[I.version] < 0 && (rc = roots.open(I.version, dirs[I.version]))) return rc;
     st.ns_plan = now_ns() - t0;
 
     // ---- the data pass: K1 over every distinct block, once
-    call.phase(VMIG_PHASE_DATA);
-    if (cancel->load()) { close_roots(); return fail(VMIG_ECANCELED, "before the data pass"); }
-    t0 = now_ns();
-    std::vector<uint64_t> hashes(n_blocks, 0);
-    rc = run_blocks(blocks, &io, false, true, o, hashes.data(), &st, ctl, false);
-    reader.close_all();
-    close_roots();
-    st.ns_data = now_ns() - t0;
+    ScrubReader reader;
+    std::vector<uint64_t> hashes;
+    rc = inode_pass(call, o, roots.fds, inodes, &reader, &hashes, &st);
     if (rc) return rc;
+    ss.bytes_unique = st.bytes_total;
 
     // ---- compare every table record with the hashes of the inode it names
     t0 = now_ns();
@@ -1134,8 +1149,6 @@ int scrub_body(CallScope& call, uint32_t n, const char* const* dirs, const char*
         if (rc) return rc;
     }
     st.ns_table = now_ns() - t0;
-    st.files_direct = reader.n_direct.load();
-    st.bytes_total = ss.bytes_unique; st.blocks_total = n_blocks; st.files = inodes.size();
     st.ns_total = now_ns() - t_begin;
     if (verdicts_out) std::copy(verdict.begin(), verdict.end(), verdicts_out);
     if (stats_out) *stats_out = st;
@@ -1144,8 +1157,8 @@ int scrub_body(CallScope& call, uint32_t n, const char* const* dirs, const char*
 }
 
 // ---------------------------------------------------------------------------------------------
-// vmig_retire_versions: the removal and the re-stamp plan are vmig_retire.cpp's; the re-verify is the scrub's data pass
-// over the stale records' inodes
+// vmig_retire_versions: the removal and the re-stamp plan are vmig_retire.cpp's; the re-verify is inode_pass over
+// the stale records' inodes
 // The real path of p without following its last component (it may be a symlink, or missing): realpath of the parent
 // plus the name.  A parent that does not exist leaves p as given (nothing can be removed beneath it).
 int real_parent_path(const char* p, std::string* out)
@@ -1214,7 +1227,6 @@ int check_retire_args(uint32_t n_retire, const char* const* retire_dirs, const c
 
 int retire_body(CallScope& call, const RetireArgs& a, const vmig_opts& o, vmig_stats* stats_out, vmig_retire_stats* rs_out)
 {
-    CallCtl* ctl = call.ctl;
     const std::atomic<int>* cancel = call.cancel();
     vmig_stats st; memset(&st, 0, sizeof st);
     vmig_retire_stats rs; memset(&rs, 0, sizeof rs);
@@ -1243,49 +1255,29 @@ int retire_body(CallScope& call, const RetireArgs& a, const vmig_opts& o, vmig_s
 
     // ---- the kept records whose ctime moved, grouped by inode
     call.phase(VMIG_PHASE_WALK);
-    std::vector<int> root_fds(n_keep, -1);
-    auto close_roots = [&] { for (int& fd : root_fds) if (fd >= 0) { close(fd); fd = -1; } };
-    for (size_t k = 0; k < n_keep; k++) {
-        root_fds[k] = open(a.keep_dirs[k].c_str(), O_RDONLY | O_DIRECTORY | O_CLOEXEC);
-        if (root_fds[k] < 0) { const int e = errno; close_roots(); return fail(VMIG_ESRCCHANGED, "open %s: %s", a.keep_dirs[k].c_str(), errno_str(e).c_str()); }
-    }
+    VersionRoots roots(n_keep);
+    for (size_t k = 0; k < n_keep; k++)
+        if ((rc = roots.open(k, a.keep_dirs[k].c_str()))) return rc;
     std::vector<const BlockTable*> tabs;
     for (const BlockTable& t : tab) tabs.push_back(&t);
     std::vector<StaleRecord> stale;
     std::vector<ScrubInode> inodes;
     std::vector<uint32_t> inode_of;
-    rc = retire_find_stale(root_fds, tabs, &stale, cancel);
+    rc = retire_find_stale(roots.fds, tabs, &stale, cancel);
     if (!rc) rc = retire_group(stale, tabs, o.block_bytes, &inodes, &inode_of);
-    if (rc) { close_roots(); return rc; }
+    if (rc) return rc;
     st.ns_walk = now_ns() - t0;
-    t0 = now_ns();
-    uint64_t n_blocks = 0;
-    for (const ScrubInode& I : inodes) { rs.bytes_rehashed += I.size; n_blocks += I.n_blocks; }
     rs.records_stale = stale.size();
-    ctl->bytes_total.store(rs.bytes_rehashed); ctl->blocks_total.store(n_blocks);
-    ScrubReader reader;
-    reader.root_fds = root_fds; reader.inodes = &inodes; reader.direct = (o.flags & VMIG_F_DIRECT_IO) != 0;
-    reader.init();
-    ScrubIO io; io.r = &reader; io.block_bytes = o.block_bytes;
-    std::vector<BlockSpan> spans;
-    for (uint32_t u = 0; u < inodes.size(); u++) spans.push_back({u, inodes[u].size, inodes[u].first_block, inodes[u].n_blocks});
-    std::vector<BlockRef> blocks; blocks.reserve(n_blocks);
-    interleave_blocks(spans, o.block_bytes, &blocks);
-    st.ns_plan = now_ns() - t0;
 
     // ---- re-verify each stale inode once: K1 in hash-only mode, compared on the host
-    call.phase(VMIG_PHASE_DATA);
-    if (cancel->load()) { close_roots(); return fail(VMIG_ECANCELED, "before the data pass"); }
-    t0 = now_ns();
-    std::vector<uint64_t> hashes(n_blocks, 0);
-    rc = run_blocks(blocks, &io, false, true, o, hashes.data(), &st, ctl, false);
-    reader.close_all();
-    st.ns_data = now_ns() - t0;
-    if (rc) { close_roots(); return rc; }
+    ScrubReader reader;
+    std::vector<uint64_t> hashes;
+    rc = inode_pass(call, o, roots.fds, inodes, &reader, &hashes, &st);
+    if (rc) return rc;
+    rs.bytes_rehashed = st.bytes_total;
     std::vector<bool> unreadable(inodes.size());
     for (uint32_t u = 0; u < inodes.size(); u++) unreadable[u] = reader.unreadable(u);
-    const std::vector<size_t> chosen = retire_decide(root_fds, tabs, stale, inodes, inode_of, hashes, unreadable);
-    close_roots();
+    const std::vector<size_t> chosen = retire_decide(roots.fds, tabs, stale, inodes, inode_of, hashes, unreadable);
     rs.records_restamped = chosen.size();
 
     // ---- rewrite each kept table that gained a verified identity
@@ -1298,8 +1290,6 @@ int retire_body(CallScope& call, const RetireArgs& a, const vmig_opts& o, vmig_s
         rs.tables_rewritten++;
     }
     st.ns_table = now_ns() - t0;
-    st.files_direct = reader.n_direct.load();
-    st.bytes_total = rs.bytes_rehashed; st.blocks_total = n_blocks; st.files = inodes.size();
     st.ns_total = now_ns() - t_begin;
     if (stats_out) *stats_out = st;
     if (rs_out) *rs_out = rs;
@@ -1308,11 +1298,10 @@ int retire_body(CallScope& call, const RetireArgs& a, const vmig_opts& o, vmig_s
 
 // ---------------------------------------------------------------------------------------------
 // vmig_compare_snapshot: the plan, the merge and the report are vmig_compare.cpp's; the layer files that need reading go
-// through the scrub's reader and data pass (one root: the layer, as version 0)
+// through inode_pass (one root: the layer, as version 0)
 int compare_body(CallScope& call, const char* layer_dir, const char* layer_table, const char* snap_dir, const char* snap_table,
                  const char* report_path, const vmig_opts& o, vmig_stats* stats_out, vmig_compare_stats* cs_out)
 {
-    CallCtl* ctl = call.ctl;
     const std::atomic<int>* cancel = call.cancel();
     vmig_stats st; memset(&st, 0, sizeof st);
     vmig_compare_stats cs; memset(&cs, 0, sizeof cs);
@@ -1349,31 +1338,14 @@ int compare_body(CallScope& call, const char* layer_dir, const char* layer_table
     ComparePlan plan;
     rc = compare_plan(layer_dir, layer, snap, ltab, o.block_bytes, &plan);
     if (rc) return rc;
-    ctl->bytes_total.store(plan.bytes_read); ctl->blocks_total.store(plan.blocks_read);
-    std::vector<int> root_fds(1, -1);
-    if (!plan.inodes.empty()) {
-        root_fds[0] = open(layer_dir, O_RDONLY | O_DIRECTORY | O_CLOEXEC);
-        if (root_fds[0] < 0) return fail(VMIG_ESRCCHANGED, "open %s: %s", layer_dir, errno_str(errno).c_str());
-    }
-    ScrubReader reader;
-    reader.root_fds = root_fds; reader.inodes = &plan.inodes; reader.direct = (o.flags & VMIG_F_DIRECT_IO) != 0;
-    reader.init();
-    ScrubIO io; io.r = &reader; io.block_bytes = o.block_bytes;
-    std::vector<BlockSpan> spans;
-    for (uint32_t u = 0; u < plan.inodes.size(); u++) spans.push_back({u, plan.inodes[u].size, plan.inodes[u].first_block, plan.inodes[u].n_blocks});
-    std::vector<BlockRef> blocks; blocks.reserve(plan.blocks_read);
-    interleave_blocks(spans, o.block_bytes, &blocks);
+    VersionRoots roots(1);
+    if (!plan.inodes.empty() && (rc = roots.open(0, layer_dir))) return rc;
     st.ns_plan = now_ns() - t0;
 
     // ---- the data pass: K1 over every block of the distinct layer inodes that need reading, once
-    call.phase(VMIG_PHASE_DATA);
-    if (cancel->load()) { if (root_fds[0] >= 0) close(root_fds[0]); return fail(VMIG_ECANCELED, "before the data pass"); }
-    t0 = now_ns();
-    std::vector<uint64_t> read_hashes(plan.blocks_read, 0);
-    rc = run_blocks(blocks, &io, false, true, o, read_hashes.data(), &st, ctl, false);
-    reader.close_all();
-    if (root_fds[0] >= 0) close(root_fds[0]);
-    st.ns_data = now_ns() - t0;
+    ScrubReader reader;
+    std::vector<uint64_t> read_hashes;
+    rc = inode_pass(call, o, roots.fds, plan.inodes, &reader, &read_hashes, &st);
     if (rc) return rc;
     for (uint32_t u = 0; u < plan.inodes.size(); u++)
         if (reader.unreadable(u)) return fail(VMIG_EIO, "layer file %s: %s", plan.inodes[u].rel.c_str(), reader.why(u).c_str());
@@ -1396,8 +1368,6 @@ int compare_body(CallScope& call, const char* layer_dir, const char* layer_table
     cs.files_changed = c.files_changed; cs.blocks_changed = c.blocks_changed; cs.bytes_restore = c.bytes_restore;
     cs.files_read = plan.inodes.size(); cs.bytes_read = plan.bytes_read;
     cs.files_trusted = plan.files_trusted; cs.files_shared = plan.files_shared;
-    st.files_direct = reader.n_direct.load();
-    st.bytes_total = plan.bytes_read; st.blocks_total = plan.blocks_read; st.files = plan.inodes.size();
     st.ns_total = now_ns() - t_begin;
     if (stats_out) *stats_out = st;
     if (cs_out) *cs_out = cs;
@@ -1522,10 +1492,7 @@ int vmig_restore_paths(const char* snap_dir, const char* snap_table, const char*
     rc = check_block_bytes(o);
     if (!rc) rc = check_restore_paths_dirs(snap_dir, dst_dir);
     if (rc) return rc;
-    CallScope call;
-    rc = call.attach(o.ctl);
-    if (rc) return rc;
-    return call.finish(restore_paths_body(call, snap_dir, snap_table, dst_dir, sorted, prior_table, o, stats));
+    return in_call(o.ctl, [&](CallScope& call) { return restore_paths_body(call, snap_dir, snap_table, dst_dir, sorted, prior_table, o, stats); });
 }
 int vmig_snapshot_tree(const char* src_dir, const char* dst_dir, const char* base_dir, const char* base_table,
                        const char* out_table, const vmig_opts* opts, vmig_stats* stats, vmig_snapshot_stats* snap_stats)
@@ -1555,10 +1522,7 @@ int vmig_scrub_store(uint32_t n, const char* const* snap_dirs, const char* const
     if (o.flags & ~allowed) return fail(VMIG_EINVAL, "flags 0x%x: a scrub takes only VMIG_F_DIRECT_IO and VMIG_F_SKIP_HIDDEN_TOPDIRS", o.flags & ~allowed);
     int rc = check_block_bytes(o);
     if (rc) return rc;
-    CallScope call;
-    rc = call.attach(o.ctl);
-    if (rc) return rc;
-    return call.finish(scrub_body(call, n, snap_dirs, snap_tables, report_path, verdicts, o, stats, scrub_stats));
+    return in_call(o.ctl, [&](CallScope& call) { return scrub_body(call, n, snap_dirs, snap_tables, report_path, verdicts, o, stats, scrub_stats); });
 }
 int vmig_retire_versions(uint32_t n_retire, const char* const* retire_dirs, const char* const* retire_tables,
                          uint32_t n_keep, const char* const* keep_dirs, const char* const* keep_tables,
@@ -1579,10 +1543,7 @@ int vmig_retire_versions(uint32_t n_retire, const char* const* retire_dirs, cons
     RetireArgs a;
     rc = check_retire_args(n_retire, retire_dirs, retire_tables, n_keep, keep_dirs, keep_tables, &a);
     if (rc) return rc;
-    CallScope call;
-    rc = call.attach(o.ctl);
-    if (rc) return rc;
-    return call.finish(retire_body(call, a, o, stats, retire_stats));
+    return in_call(o.ctl, [&](CallScope& call) { return retire_body(call, a, o, stats, retire_stats); });
 }
 int vmig_compare_snapshot(const char* layer_dir, const char* layer_table, const char* snap_dir, const char* snap_table,
                           const char* report_path, const vmig_opts* opts, vmig_stats* stats, vmig_compare_stats* cmp_stats)
@@ -1596,10 +1557,9 @@ int vmig_compare_snapshot(const char* layer_dir, const char* layer_table, const 
         return fail(VMIG_EINVAL, "flags 0x%x: a compare takes only VMIG_F_DIRECT_IO, VMIG_F_SKIP_HIDDEN_TOPDIRS, VMIG_F_MTIME_NS and VMIG_F_NO_METADATA", o.flags & ~allowed);
     int rc = check_block_bytes(o);
     if (rc) return rc;
-    CallScope call;
-    rc = call.attach(o.ctl);
-    if (rc) return rc;
-    return call.finish(compare_body(call, layer_dir, layer_table, snap_dir, snap_table, report_path, o, stats, cmp_stats));
+    return in_call(o.ctl, [&](CallScope& call) {
+        return compare_body(call, layer_dir, layer_table, snap_dir, snap_table, report_path, o, stats, cmp_stats);
+    });
 }
 int vmig_copy_dir(const char* src_dir, const char* dst_dir) { return migrate_tree_impl(src_dir, dst_dir, nullptr, nullptr, nullptr, nullptr); }
 int vmig_move_dir(const char* src_dir, const char* dst_dir)

@@ -5,8 +5,6 @@
 #include <fcntl.h>
 #include <unistd.h>
 #include <sys/stat.h>
-#include <map>
-#include <utility>
 
 namespace vmig {
 
@@ -69,24 +67,11 @@ int retire_group(const std::vector<StaleRecord>& stale, const std::vector<const 
 {
     inodes->clear();
     inode_of->assign(stale.size(), kNoInode);
-    std::map<std::pair<uint64_t, uint64_t>, uint32_t> seen;
-    uint64_t fb = 0;
+    InodeGroups groups{inodes, block_bytes, "retire"};
     for (size_t r = 0; r < stale.size(); r++) {
-        const StaleRecord& s = stale[r];
-        const TableFile& rec = tabs[s.version]->files[s.file];
-        auto it = seen.find({s.dev, rec.ino});
-        if (it == seen.end()) {
-            const uint64_t nb = (rec.size + block_bytes - 1) / block_bytes;
-            it = seen.emplace(std::make_pair(s.dev, rec.ino), (uint32_t)inodes->size()).first;
-            inodes->push_back({s.dev, rec.ino, rec.size, fb, nb, s.version, rec.rel});
-            fb += nb;
-        } else if ((*inodes)[it->second].size != rec.size) {
-            const ScrubInode& I = (*inodes)[it->second];
-            return fail(VMIG_ESRCCHANGED, "inode %llu is %llu bytes as version %u's %s and %llu bytes as version %u's %s: the store changed during the retire",
-                        (unsigned long long)rec.ino, (unsigned long long)I.size, I.version, I.rel.c_str(), (unsigned long long)rec.size,
-                        s.version, rec.rel.c_str());
-        }
-        (*inode_of)[r] = it->second;
+        const TableFile& rec = tabs[stale[r].version]->files[stale[r].file];
+        const int rc = groups.add(stale[r].dev, rec.ino, rec.size, stale[r].version, rec.rel, &(*inode_of)[r]);
+        if (rc) return rc;
     }
     return VMIG_OK;
 }

@@ -32,8 +32,7 @@ struct StaleRecord { uint32_t version; uint32_t file; uint64_t dev; int64_t ctim
 int retire_find_stale(const std::vector<int>& root_fds, const std::vector<const BlockTable*>& tabs,
                       std::vector<StaleRecord>* out, const std::atomic<int>* cancel);
 
-// Group stale records by (dev, ino) into the scrub's inodes (opened at the first record's path; block ranges laid out
-// in order).  (*inode_of)[r] is record r's inode.  Two records of one inode with different sizes: VMIG_ESRCCHANGED.
+// Group stale records into the scrub's inodes by the scrub's rule (InodeGroups).  (*inode_of)[r] is record r's inode.
 int retire_group(const std::vector<StaleRecord>& stale, const std::vector<const BlockTable*>& tabs, uint32_t block_bytes,
                  std::vector<ScrubInode>* inodes, std::vector<uint32_t>* inode_of);
 

@@ -9,7 +9,6 @@
 #include <algorithm>
 #include <cctype>
 #include <cstdlib>
-#include <map>
 #include <tuple>
 #include <utility>
 
@@ -40,13 +39,29 @@ size_t scrub_merge_table(uint32_t version, const Manifest& man, const BlockTable
     return n;
 }
 
+int InodeGroups::add(uint64_t dev, uint64_t ino, uint64_t size, uint32_t version, const std::string& rel, uint32_t* u)
+{
+    auto it = seen.find({dev, ino});
+    if (it == seen.end()) {
+        const uint64_t nb = (size + block_bytes - 1) / block_bytes;
+        it = seen.emplace(std::make_pair(dev, ino), (uint32_t)inodes->size()).first;
+        inodes->push_back({dev, ino, size, next_block, nb, version, rel});
+        next_block += nb;
+    } else if ((*inodes)[it->second].size != size) {
+        const ScrubInode& I = (*inodes)[it->second];
+        return fail(VMIG_ESRCCHANGED, "inode %llu is %llu bytes as version %u's %s and %llu bytes as version %u's %s: the store changed during the %s",
+                    (unsigned long long)ino, (unsigned long long)I.size, I.version, I.rel.c_str(), (unsigned long long)size, version, rel.c_str(), call);
+    }
+    *u = it->second;
+    return VMIG_OK;
+}
+
 int scrub_group_inodes(const std::vector<const Manifest*>& mans, const std::vector<std::vector<int64_t>>& sel,
                        uint32_t block_bytes, std::vector<ScrubInode>* inodes, std::vector<std::vector<uint32_t>>* inode_of)
 {
     inodes->clear();
     inode_of->assign(mans.size(), {});
-    std::map<std::pair<uint64_t, uint64_t>, uint32_t> seen;
-    uint64_t fb = 0;
+    InodeGroups groups{inodes, block_bytes, "scrub"};
     for (size_t v = 0; v < mans.size(); v++) {
         if (!mans[v]) continue;
         const Manifest& m = *mans[v];
@@ -54,22 +69,8 @@ int scrub_group_inodes(const std::vector<const Manifest*>& mans, const std::vect
         for (size_t f = 0; f < m.files.size() && f < sel[v].size(); f++) {
             const Entry& e = m.files[f];
             if (sel[v][f] < 0 || e.size == 0) continue;
-            auto it = seen.find({e.dev, e.ino});
-            uint32_t u;
-            if (it == seen.end()) {
-                u = (uint32_t)inodes->size();
-                const uint64_t nb = (e.size + block_bytes - 1) / block_bytes;
-                inodes->push_back({e.dev, e.ino, e.size, fb, nb, (uint32_t)v, e.rel});
-                fb += nb;
-                seen.emplace(std::make_pair(e.dev, e.ino), u);
-            } else {
-                u = it->second;
-                const ScrubInode& I = (*inodes)[u];
-                if (I.size != e.size)
-                    return fail(VMIG_ESRCCHANGED, "inode %llu is %llu bytes as version %u's %s and %llu bytes as version %zu's %s: the store changed during the scrub",
-                                (unsigned long long)e.ino, (unsigned long long)I.size, I.version, I.rel.c_str(), (unsigned long long)e.size, v, e.rel.c_str());
-            }
-            (*inode_of)[v][f] = u;
+            const int rc = groups.add(e.dev, e.ino, e.size, (uint32_t)v, e.rel, &(*inode_of)[v][f]);
+            if (rc) return rc;
         }
     }
     return VMIG_OK;
@@ -155,6 +156,12 @@ void ScrubReader::init()
     n_st = inodes->size();
     st.reset(new State[n_st ? n_st : 1]);
     for (size_t u = 0; u < n_st; u++) st[u].reads_left.store((uint32_t)(*inodes)[u].n_blocks);
+}
+
+std::string ScrubReader::block_name(const BlockRef& b)
+{
+    const ScrubInode& I = (*inodes)[b.file];
+    return I.rel + " (version " + std::to_string(I.version) + ") block " + std::to_string(b.file_off / block_bytes);
 }
 
 void ScrubReader::adopt(uint32_t u, int fd, bool is_direct)

@@ -8,10 +8,13 @@
 #pragma once
 #include <stdint.h>
 #include <atomic>
+#include <map>
 #include <memory>
 #include <mutex>
 #include <string>
+#include <utility>
 #include <vector>
+#include "vmig_engine.h"
 #include "vmig_table.h"
 #include "vmig_tree.h"
 
@@ -42,10 +45,23 @@ size_t scrub_merge_table(uint32_t version, const Manifest& man, const BlockTable
 struct ScrubInode { uint64_t dev, ino, size, first_block, n_blocks; uint32_t version; std::string rel; };
 static constexpr uint32_t kNoInode = 0xFFFFFFFFu;
 
+// The grouping rule of every call that reads each distinct inode once: an inode is its (st_dev, st_ino), opened at the
+// first path that names it, its block range laid out after those of the inodes seen before it.  A second size for one
+// inode means the store changed between the walks: VMIG_ESRCCHANGED, "...during the <call>".
+struct InodeGroups {
+    std::vector<ScrubInode>* inodes;
+    uint32_t block_bytes;
+    const char* call;                          // "scrub", "retire"
+    std::map<std::pair<uint64_t, uint64_t>, uint32_t> seen;
+    uint64_t next_block = 0;
+    // *u: the index in *inodes of the inode (dev, ino), which version's rel names with size bytes
+    int add(uint64_t dev, uint64_t ino, uint64_t size, uint32_t version, const std::string& rel, uint32_t* u);
+};
+
 // Group the selected, non-empty regular files of every version (sel[v][f] >= 0: for the scrub, the table index of a file
 // that matches its record; for vmig_compare_snapshot, a layer file to read; mans[v] may be null for a version that was
-// not walked) by (dev, ino).  (*inode_of)[v][f] is the inode's index, kNoInode where the path is not read.
-// Two paths of one inode with different sizes mean the tree changed between the walks: VMIG_ESRCCHANGED.
+// not walked) by InodeGroups' rule, named "scrub".  (*inode_of)[v][f] is the inode's index, kNoInode where the path is
+// not read.
 int scrub_group_inodes(const std::vector<const Manifest*>& mans, const std::vector<std::vector<int64_t>>& sel,
                        uint32_t block_bytes, std::vector<ScrubInode>* inodes, std::vector<std::vector<uint32_t>>* inode_of);
 
@@ -69,16 +85,22 @@ int scrub_report_store(const std::string& path, const std::vector<ScrubFinding>&
 // longer the walked one (other dev/ino, not a regular file, other size, shorter than its blocks, or its path gone) is
 // VMIG_ESRCCHANGED, a call failure as everywhere else.  Any other open or read error does NOT fail: the inode is marked
 // unreadable, its remaining blocks are not read, and read() returns VMIG_OK so the pipeline's first-error latch stays
-// clear.  Thread-safe; the descriptor is closed after the inode's last block.
-class ScrubReader {
+// clear.  Thread-safe; the descriptor is closed after the inode's last block.  It is the block pipeline's backend in
+// hash-only mode: block b of inode u is BlockRef{file = u, table_idx = its index in the call's hash array}.
+class ScrubReader : public BlockIO {
 public:
     std::vector<int> root_fds;                 // per version; -1 for a version that is not read (not owned)
     const std::vector<ScrubInode>* inodes = nullptr;
     bool direct = false;                       // VMIG_F_DIRECT_IO
+    uint32_t block_bytes = 4u << 20;           // numbers the blocks in block_name
     std::atomic<uint64_t> n_direct{0};         // descriptors really opened O_DIRECT
 
     void init();                               // after inodes is set: one reads_left per block
     int read(uint32_t u, uint64_t off, uint32_t len, uint8_t* dst);
+    int read_block(const BlockRef& b, uint8_t* dst) override { return read(b.file, b.file_off, b.len, dst); }
+    int write_block(const BlockRef&, const uint8_t*) override { return fail(VMIG_EINVAL, "a scrub writes nothing"); }
+    uint32_t slot_align() override { return direct ? kSector : 512; }
+    std::string block_name(const BlockRef& b) override;   // "<rel> (version N) block K"
     void adopt(uint32_t u, int fd, bool is_direct);   // use this open descriptor for inode u (tests/scrub_unit.cpp)
     bool unreadable(uint32_t u) const { return st[u].bad.load(); }
     std::string why(uint32_t u);               // the error that made u unreadable

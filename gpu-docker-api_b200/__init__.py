@@ -48,7 +48,7 @@ EXPORTS = [
     "vmig_resident_set_prior", "vmig_resident_pass", "vmig_resident_results", "vmig_table_info_read",
     "vmig_table_hashes", "vmig_dir_size", "vmig_to_bytes", "vmig_datagen_files", "vmig_manifest", "vmig_link_probe", "vmig_thread_plan",
     "vmig_ctl_open", "vmig_ctl_cancel", "vmig_ctl_progress", "vmig_ctl_close", "vmig_scrub_store",
-    "vmig_retire_versions", "vmig_restore_paths", "vmig_compare_snapshot",
+    "vmig_retire_versions", "vmig_restore_paths", "vmig_compare_snapshot", "vmig_rollback_layer",
 ]
 SCRUB_KINDS = ("missing", "extra", "resized", "block", "hardlink", "unreadable", "table", "dir")
 COMPARE_KINDS = ("added", "removed", "type", "resized", "block", "target", "rdev", "hardlink", "mode", "owner", "mtime")
@@ -114,6 +114,15 @@ class CompareStats(C.Structure):
         return {n: getattr(self, n) for n, _ in self._fields_ if n != "reserved"}
 
 
+class RollbackStats(C.Structure):
+    _fields_ = [(n, C.c_uint64) for n in ("files_kept", "files_patched", "files_rebuilt", "files_created", "blocks_fetched",
+                                          "bytes_fetched", "files_trusted", "files_read", "bytes_read", "bytes_copied")] + \
+        [("reserved", C.c_uint64 * 4)]
+
+    def as_dict(self) -> dict:
+        return {n: getattr(self, n) for n, _ in self._fields_ if n != "reserved"}
+
+
 class TableInfo(C.Structure):
     _fields_ = [("block_bytes", C.c_uint32), ("algo", C.c_uint32), ("n_files", C.c_uint64),
                 ("n_blocks", C.c_uint64), ("bytes_total", C.c_uint64)]
@@ -171,6 +180,8 @@ _sig = {
                                      C.POINTER(Opts), C.POINTER(Stats)]),
     "vmig_compare_snapshot": (C.c_int, [C.c_char_p, C.c_char_p, C.c_char_p, C.c_char_p, C.c_char_p, C.POINTER(Opts),
                                         C.POINTER(Stats), C.POINTER(CompareStats)]),
+    "vmig_rollback_layer": (C.c_int, [C.c_char_p, C.c_char_p, C.c_char_p, C.c_char_p, C.c_char_p, C.POINTER(Opts),
+                                      C.POINTER(Stats), C.POINTER(RollbackStats)]),
 }
 for _n, (_r, _a) in _sig.items():
     _f = getattr(_lib, _n)
@@ -219,7 +230,7 @@ def _b(p) -> Optional[bytes]:
 
 class Ctl:
     """A call control (vmig_ctl_*): pass it as ``ctl=`` to migrate_tree, restore_tree, restore_paths, snapshot_tree,
-    scrub_store, retire_versions, compare_snapshot or migrate_buffer,
+    scrub_store, retire_versions, compare_snapshot, rollback_layer or migrate_buffer,
     then cancel() from any thread (the call raises VmigError(VMIG_ECANCELED)) or read progress() while it runs.  ctypes
     releases the GIL during the call.  One control serves one call at a time; a deadline is a threading.Timer."""
 
@@ -491,6 +502,22 @@ def compare_snapshot(layer, snap, snap_table, report=None, layer_table=None, *, 
     _check(_lib.vmig_compare_snapshot(_b(layer), _b(layer_table), _b(snap), _b(snap_table), _b(report), C.byref(o),
                                       C.byref(st), C.byref(cs)), f"vmig_compare_snapshot({layer} vs {snap})")
     return {"stats": st.as_dict(), **cs.as_dict()}
+
+
+def rollback_layer(layer, snap, snap_table, out_table=None, layer_table=None, *, flags: int = 0, gpu_mask: int = 0,
+                   lanes_per_gpu: int = 0, block_bytes: int = 0, io_threads: int = 0, streams_per_gpu: int = 0,
+                   ctl: Optional[Ctl] = None) -> dict:
+    """Roll the layer `layer` back to the version snapshot `snap` (checked against `snap_table`) in place: afterwards it is
+    what restore_tree(snap, snap_table, layer, flags=F_PRUNE | flags) leaves, but only the snapshot blocks the layer does
+    not already hold are read.  layer_table: a table of `layer` whose records still vouch for their files (those are not
+    read); out_table may be the same path.  Returns the vmig_rollback_stats fields plus the counters of both data passes
+    ("stats")."""
+    o = Opts(gpu_mask=gpu_mask, block_bytes=block_bytes, flags=flags, lanes_per_gpu=lanes_per_gpu, io_threads=io_threads,
+             streams_per_gpu=streams_per_gpu, ctl=_ctl_id(ctl))
+    st, rs = Stats(), RollbackStats()
+    _check(_lib.vmig_rollback_layer(_b(layer), _b(layer_table), _b(snap), _b(snap_table), _b(out_table), C.byref(o),
+                                    C.byref(st), C.byref(rs)), f"vmig_rollback_layer({layer} to {snap})")
+    return {"stats": st.as_dict(), **rs.as_dict()}
 
 
 def hash_tree(src, out_table, *, gpu_mask: int = 0, block_bytes: int = 0) -> dict:

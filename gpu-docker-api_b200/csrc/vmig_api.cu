@@ -11,6 +11,7 @@
 #include "vmig_reuse.h"
 #include "vmig_scrub.h"
 #include "vmig_compare.h"
+#include "vmig_rollback.h"
 #include "vmig_retire.h"
 #include "vmig_plan.h"
 #include "vmig_select.h"
@@ -642,8 +643,10 @@ struct SnapshotArgs {
 
 // After the data pass: hard-linked paths take their primary's hashes, empty regular files are created, then the rest of
 // the tree's metadata is replayed (vmig_tree.h replay_metadata).
+// make_empty == false: the caller has already put every empty regular file in place (vmig_rollback_layer keeps one
+// that is already right).
 int meta_pass(CallScope& call, FileIO& io, const std::vector<uint64_t>& expect, std::vector<uint64_t>* hashes, vmig_stats* st,
-              size_t first_dir)
+              size_t first_dir, bool make_empty = true)
 {
     const Manifest& man = *io.m;
     const std::atomic<int>* cancel = call.cancel();
@@ -665,7 +668,7 @@ int meta_pass(CallScope& call, FileIO& io, const std::vector<uint64_t>& expect, 
     if (io.hash_only) return VMIG_OK;
     size_t steps = 0;
     for (auto& e : man.files) {                    // empty regular files carry no blocks
-        if (e.hardlink_of >= 0 || e.n_blocks) continue;
+        if (e.hardlink_of >= 0 || e.n_blocks || !make_empty) continue;
         if (steps++ % kMetaCheckEvery == 0 && cancel->load()) return fail(VMIG_ECANCELED, "before creating %s", e.rel.c_str());
         const std::string p = pjoin(io.dst_root, e.rel);
         int rc = clear_path(p, "an empty regular file"); if (rc) return rc;
@@ -974,16 +977,22 @@ int restore_paths_body(CallScope& call, const char* snap_dir, const char* snap_t
     return tree_passes(call, src, dst, sel.man, expect, prior_path, nullptr, o, st, nullptr, &sel, t_begin, stats_out);
 }
 
-// snap_dir and dst_dir the same directory or one inside the other (real paths); a path that does not resolve is left to
-// the call's own stat
+// a is b, or either lies inside the other (real paths; a path that does not resolve is left to the call's own checks)
+bool real_paths_overlap(const char* a, const char* b, std::string* ra, std::string* rb)
+{
+    char* x = realpath(a, nullptr);
+    char* y = realpath(b, nullptr);
+    *ra = x ? x : ""; *rb = y ? y : "";
+    free(x); free(y);
+    return !ra->empty() && !rb->empty() && (path_inside(*ra, *rb) || path_inside(*rb, *ra));
+}
+
+// snap_dir and dst_dir the same directory or one inside the other
 int check_restore_paths_dirs(const char* snap_dir, const char* dst_dir)
 {
-    char* a = realpath(snap_dir, nullptr);
-    char* b = realpath(dst_dir, nullptr);
-    const bool overlap = a && b && (path_inside(a, b) || path_inside(b, a));
-    const std::string as(a ? a : ""), bs(b ? b : "");
-    free(a); free(b);
-    if (overlap) return fail(VMIG_EINVAL, "snap_dir %s and dst_dir %s are the same directory or one is inside the other", as.c_str(), bs.c_str());
+    std::string as, bs;
+    if (real_paths_overlap(snap_dir, dst_dir, &as, &bs))
+        return fail(VMIG_EINVAL, "snap_dir %s and dst_dir %s are the same directory or one is inside the other", as.c_str(), bs.c_str());
     return VMIG_OK;
 }
 
@@ -1297,8 +1306,61 @@ int retire_body(CallScope& call, const RetireArgs& a, const vmig_opts& o, vmig_s
 }
 
 // ---------------------------------------------------------------------------------------------
-// vmig_compare_snapshot: the plan, the merge and the report are vmig_compare.cpp's; the layer files that need reading go
-// through inode_pass (one root: the layer, as version 0)
+// The layer side of vmig_compare_snapshot and vmig_rollback_layer: the layer's walk, where each layer file takes its block
+// hashes from (compare_plan: a shared inode, a trusted record of the layer's table, or a read), and the data pass over the
+// files that need reading, each distinct inode once through inode_pass (one root: the layer, as version 0)
+struct LayerSide {
+    Manifest man;
+    ComparePlan plan;
+    VersionRoots roots{1};
+    std::vector<uint64_t> read_hashes;
+    std::vector<const uint64_t*> hashes;     // per layer file (compare_layer_hashes)
+};
+
+int layer_plan(const char* layer_dir, const Manifest& snap, const BlockTable* ltab, const vmig_opts& o, const std::atomic<int>* cancel,
+               LayerSide* L, vmig_stats* st)
+{
+    uint64_t t0 = now_ns();
+    int rc = walk_tree(layer_dir, o.block_bytes, (o.flags & VMIG_F_SKIP_HIDDEN_TOPDIRS) != 0, &L->man, cancel);
+    if (rc) return rc;
+    st->ns_walk += now_ns() - t0;
+    t0 = now_ns();
+    rc = compare_plan(layer_dir, L->man, snap, ltab, o.block_bytes, &L->plan);
+    if (!rc && !L->plan.inodes.empty()) rc = L->roots.open(0, layer_dir);
+    st->ns_plan += now_ns() - t0;
+    return rc;
+}
+
+// K1 over every block of the distinct layer inodes that need reading, once; then every layer file's hashes
+int layer_hash_pass(CallScope& call, const vmig_opts& o, const Manifest& snap, const std::vector<uint64_t>& snap_hashes,
+                    const BlockTable* ltab, LayerSide* L, vmig_stats* st)
+{
+    ScrubReader reader;
+    const int rc = inode_pass(call, o, L->roots.fds, L->plan.inodes, &reader, &L->read_hashes, st);
+    if (rc) return rc;
+    for (uint32_t u = 0; u < L->plan.inodes.size(); u++)
+        if (reader.unreadable(u)) return fail(VMIG_EIO, "layer file %s: %s", L->plan.inodes[u].rel.c_str(), reader.why(u).c_str());
+    L->hashes = compare_layer_hashes(L->plan, L->man, snap, snap_hashes, ltab, L->read_hashes);
+    return VMIG_OK;
+}
+
+// Both calls' refusals after the arguments: a cancelled control, a missing directory, a table that does not load, no GPU
+int layer_call_checks(CallScope& call, const char* layer_dir, const char* layer_table, const char* snap_dir, const char* snap_table,
+                      const vmig_opts& o, BlockTable* snap_tab, BlockTable* layer_tab)
+{
+    if (call.cancel()->load()) return fail(VMIG_ECANCELED, "the control was cancelled before the call started");
+    for (const char* d : {layer_dir, snap_dir}) {
+        struct stat sb;
+        if (stat(d, &sb) != 0 || !S_ISDIR(sb.st_mode)) return fail(VMIG_ENOTDIR, "%s is missing or not a directory", d);
+    }
+    int rc = load_table(snap_table, "snapshot", o.block_bytes, snap_tab);
+    if (!rc && layer_table && *layer_table) rc = load_table(layer_table, "layer", o.block_bytes, layer_tab);
+    if (rc) return rc;
+    std::vector<DeviceInfo> devs;                    // no CPU fallback: the GPU is there before anything is read
+    return ctx_select(o.gpu_mask, &devs);
+}
+
+// vmig_compare_snapshot: the plan, the merge and the report are vmig_compare.cpp's
 int compare_body(CallScope& call, const char* layer_dir, const char* layer_table, const char* snap_dir, const char* snap_table,
                  const char* report_path, const vmig_opts& o, vmig_stats* stats_out, vmig_compare_stats* cs_out)
 {
@@ -1306,56 +1368,30 @@ int compare_body(CallScope& call, const char* layer_dir, const char* layer_table
     vmig_stats st; memset(&st, 0, sizeof st);
     vmig_compare_stats cs; memset(&cs, 0, sizeof cs);
     const uint64_t t_begin = now_ns();
-    if (cancel->load()) return fail(VMIG_ECANCELED, "the control was cancelled before the call started");
-    for (const char* d : {layer_dir, snap_dir}) {
-        struct stat sb;
-        if (stat(d, &sb) != 0 || !S_ISDIR(sb.st_mode)) return fail(VMIG_ENOTDIR, "%s is missing or not a directory", d);
-    }
     BlockTable snap_tab, layer_tab;
-    const bool has_layer_tab = layer_table && *layer_table;
-    int rc = load_table(snap_table, "snapshot", o.block_bytes, &snap_tab);
-    if (!rc && has_layer_tab) rc = load_table(layer_table, "layer", o.block_bytes, &layer_tab);
+    int rc = layer_call_checks(call, layer_dir, layer_table, snap_dir, snap_table, o, &snap_tab, &layer_tab);
     if (rc) return rc;
-    std::vector<DeviceInfo> devs;                    // no CPU fallback: the GPU is there before anything is read
-    rc = ctx_select(o.gpu_mask, &devs);
-    if (rc) return rc;
+    const BlockTable* ltab = layer_table && *layer_table ? &layer_tab : nullptr;
 
-    // ---- walk both trees; the snapshot must be the tree its table describes
+    // ---- walk both trees (the snapshot must be the tree its table describes); which layer files are read
     call.phase(VMIG_PHASE_WALK);
     uint64_t t0 = now_ns();
-    const bool skip_hidden = (o.flags & VMIG_F_SKIP_HIDDEN_TOPDIRS) != 0;
-    Manifest snap, layer;
+    Manifest snap;
     std::vector<uint64_t> snap_hashes;
-    rc = walk_tree(snap_dir, o.block_bytes, skip_hidden, &snap, cancel);
+    rc = walk_tree(snap_dir, o.block_bytes, (o.flags & VMIG_F_SKIP_HIDDEN_TOPDIRS) != 0, &snap, cancel);
     if (!rc) rc = match_table(snap, snap_tab, &snap_hashes);
-    if (!rc) rc = walk_tree(layer_dir, o.block_bytes, skip_hidden, &layer, cancel);
     if (rc) return rc;
     st.ns_walk = now_ns() - t0;
-
-    // ---- which layer files are read: shared and trusted ones are not
-    t0 = now_ns();
-    const BlockTable* ltab = has_layer_tab ? &layer_tab : nullptr;
-    ComparePlan plan;
-    rc = compare_plan(layer_dir, layer, snap, ltab, o.block_bytes, &plan);
+    LayerSide L;
+    rc = layer_plan(layer_dir, snap, ltab, o, cancel, &L, &st);
+    if (!rc) rc = layer_hash_pass(call, o, snap, snap_hashes, ltab, &L, &st);
     if (rc) return rc;
-    VersionRoots roots(1);
-    if (!plan.inodes.empty() && (rc = roots.open(0, layer_dir))) return rc;
-    st.ns_plan = now_ns() - t0;
-
-    // ---- the data pass: K1 over every block of the distinct layer inodes that need reading, once
-    ScrubReader reader;
-    std::vector<uint64_t> read_hashes;
-    rc = inode_pass(call, o, roots.fds, plan.inodes, &reader, &read_hashes, &st);
-    if (rc) return rc;
-    for (uint32_t u = 0; u < plan.inodes.size(); u++)
-        if (reader.unreadable(u)) return fail(VMIG_EIO, "layer file %s: %s", plan.inodes[u].rel.c_str(), reader.why(u).c_str());
 
     // ---- the findings, compared on the host (8 bytes per block), and the report
     t0 = now_ns();
-    const std::vector<const uint64_t*> layer_hashes = compare_layer_hashes(plan, layer, snap, snap_hashes, ltab, read_hashes);
     std::vector<CompareFinding> findings;
     CompareCounts c;
-    compare_merge(layer, snap, snap_hashes, layer_hashes, o.block_bytes, (o.flags & VMIG_F_MTIME_NS) != 0,
+    compare_merge(L.man, snap, snap_hashes, L.hashes, o.block_bytes, (o.flags & VMIG_F_MTIME_NS) != 0,
                   (o.flags & VMIG_F_NO_METADATA) != 0, &findings, &c);
     if (report_path && *report_path) {
         std::string raw;
@@ -1366,11 +1402,300 @@ int compare_body(CallScope& call, const char* layer_dir, const char* layer_table
     st.ns_table = now_ns() - t0;
     cs.paths_added = c.paths_added; cs.paths_removed = c.paths_removed; cs.paths_changed = c.paths_changed;
     cs.files_changed = c.files_changed; cs.blocks_changed = c.blocks_changed; cs.bytes_restore = c.bytes_restore;
-    cs.files_read = plan.inodes.size(); cs.bytes_read = plan.bytes_read;
-    cs.files_trusted = plan.files_trusted; cs.files_shared = plan.files_shared;
+    cs.files_read = L.plan.inodes.size(); cs.bytes_read = L.plan.bytes_read;
+    cs.files_trusted = L.plan.files_trusted; cs.files_shared = L.plan.files_shared;
     st.ns_total = now_ns() - t_begin;
     if (stats_out) *stats_out = st;
     if (cs_out) *cs_out = cs;
+    return VMIG_OK;
+}
+
+// ---------------------------------------------------------------------------------------------
+// vmig_rollback_layer: the actions, the fetch list and the copy runs are vmig_rollback.cpp's.  The snapshot blocks the
+// layer lacks are read beneath the snapshot's root and written into the layer file each action names, made ready when its
+// first block is written (RollbackIO::prepare); the rest of the tree is a pruning restore's (prune_extras, meta_pass,
+// verify_pass, write_table over the snapshot's manifest).
+class RollbackIO : public BlockIO {
+public:
+    const Manifest* snap = nullptr;
+    const RollbackPlan* plan = nullptr;
+    const std::vector<LayerId>* ids = nullptr;      // per layer file (rollback_identify)
+    std::string layer_root;
+    int snap_fd = -1;                               // snapshot files are opened beneath it (not owned)
+    bool direct = false;                            // VMIG_F_DIRECT_IO
+    uint32_t block_bytes = 4u << 20;
+    const std::atomic<int>* cancel = nullptr;       // checked per copy chunk of a rebuilt file
+    std::atomic<uint64_t> n_direct{0}, b_copied{0};      // descriptors opened O_DIRECT; bytes copied from old inodes
+    RebuildGuard rebuild_guard;                          // the call's own unlinks of rebuilt paths
+
+    void init() {
+        fs.reset(new FS[plan->files.size() ? plan->files.size() : 1]);
+        for (size_t i = 0; i < plan->files.size(); i++) {
+            fs[i].reads_left.store(plan->files[i].n_fetch); fs[i].blocks_left.store(plan->files[i].n_fetch);
+        }
+    }
+    uint32_t slot_align() override { return direct ? kSector : 512; }
+    std::string block_name(const BlockRef& b) override {
+        return snap->files[plan->files[b.file].snap].rel + " block " + std::to_string(b.file_off / block_bytes);
+    }
+
+    // Make file i of the plan ready to take its fetched blocks: a patched file opened in place (no O_TRUNC), checked and
+    // set to the snapshot's size; a rebuilt one replaced by a new inode that first takes the equal blocks from the old
+    // one; a created one made new.  *out: the descriptor to write into.
+    int prepare(uint32_t i, int* out) {
+        const RollbackFile& rf = plan->files[i];
+        const Entry& s = snap->files[rf.snap];
+        const std::string p = pjoin(layer_root, s.rel);
+        FS& f = fs[i];
+        const int dflag = direct ? O_DIRECT : 0;
+        int fd = -1, rc = VMIG_OK;
+        if (rf.action == kRbPatch) {
+            fd = open(p.c_str(), O_WRONLY | O_CLOEXEC | O_NOFOLLOW | dflag);
+            if (fd < 0 && dflag && errno == EINVAL) fd = open(p.c_str(), O_WRONLY | O_CLOEXEC | O_NOFOLLOW); else f.d_direct = dflag && fd >= 0;
+            if (fd < 0) return fail(VMIG_EIO, "open %s for writing: %s", p.c_str(), errno_str(errno).c_str());
+            const LayerId& id = (*ids)[(size_t)rf.layer];
+            rc = rollback_check_fd(fd, id, p);
+            if (!rc && id.size != s.size && ftruncate(fd, (off_t)s.size) != 0) rc = fail(VMIG_EIO, "ftruncate %s: %s", p.c_str(), errno_str(errno).c_str());
+        } else {
+            int old = -1;
+            if (rf.action == kRbRebuild) {
+                // read only when bytes are copied from it: an unreadable file with nothing to give is just replaced
+                const int oflags = rf.n_runs ? O_RDONLY | O_NONBLOCK : O_PATH;
+                old = open(p.c_str(), oflags | O_CLOEXEC | O_NOFOLLOW);
+                if (old < 0) return fail(errno == ENOENT ? VMIG_ESRCCHANGED : VMIG_EIO, "open %s: %s", p.c_str(), errno_str(errno).c_str());
+                rc = rebuild_guard.clear(old, (*ids)[(size_t)rf.layer], rf.n_runs != 0, p);
+            } else {
+                rc = clear_path(p, "a regular file");           // tar replaces what is there
+            }
+            if (!rc) {
+                fd = open(p.c_str(), O_WRONLY | O_CREAT | O_EXCL | O_CLOEXEC | O_NOFOLLOW | dflag, 0600);
+                if (fd < 0 && dflag && errno == EINVAL) fd = open(p.c_str(), O_WRONLY | O_CREAT | O_EXCL | O_CLOEXEC | O_NOFOLLOW, 0600); else f.d_direct = dflag && fd >= 0;
+                if (fd < 0) rc = fail(VMIG_EIO, "create %s: %s", p.c_str(), errno_str(errno).c_str());
+            }
+            for (uint64_t k = 0; !rc && k < rf.n_runs; k++) {
+                const CopyRun& u = plan->runs[rf.first_run + k];
+                rc = copy_range_at(old, u.off, fd, u.off, u.len, f.d_direct, false, p, cancel);
+                if (!rc) b_copied += u.len;
+            }
+            if (old >= 0) close(old);
+        }
+        if (rc) { if (fd >= 0) close(fd); return rc; }
+        if (f.d_direct) n_direct++;
+        *out = fd;
+        return VMIG_OK;
+    }
+    // O_DIRECT writes whole sectors: cut the padding of the last one
+    int finish(uint32_t i, int fd) {
+        const Entry& s = snap->files[plan->files[i].snap];
+        int rc = VMIG_OK;
+        if (fs[i].d_direct && (s.size & (kSector - 1)) && ftruncate(fd, (off_t)s.size) != 0)
+            rc = fail(VMIG_EIO, "ftruncate %s/%s: %s", layer_root.c_str(), s.rel.c_str(), errno_str(errno).c_str());
+        if (close(fd) != 0 && !rc) rc = fail(VMIG_EIO, "close %s/%s: %s", layer_root.c_str(), s.rel.c_str(), errno_str(errno).c_str());
+        return rc;
+    }
+
+    int read_block(const BlockRef& b, uint8_t* dst) override {
+        FS& f = fs[b.file];
+        const Entry& s = snap->files[plan->files[b.file].snap];
+        int fd = f.sfd.load(std::memory_order_acquire);
+        if (fd < 0) {
+            std::lock_guard<std::mutex> lk(stripes[b.file & 63]);
+            fd = f.sfd.load(std::memory_order_acquire);
+            if (fd < 0) {
+                int rc = VMIG_EIO;
+                if (direct) { rc = open_beneath(snap_fd, s.rel, O_RDONLY | O_NONBLOCK | O_DIRECT, &fd); f.s_direct = rc == VMIG_OK; }
+                if (rc) rc = open_beneath(snap_fd, s.rel, O_RDONLY | O_NONBLOCK, &fd);
+                if (rc) return rc;
+                struct stat st;
+                if (fstat(fd, &st) != 0 || !S_ISREG(st.st_mode) || (uint64_t)st.st_size != s.size) {
+                    close(fd);
+                    return fail(VMIG_ESRCCHANGED, "snapshot file %s is not the walked file any more", s.rel.c_str());
+                }
+                if (f.s_direct) n_direct++;
+                f.sfd.store(fd, std::memory_order_release);
+            }
+        }
+        size_t got;
+        const int rc = xfer_block(f.s_direct, true, b.len, &got, [&](size_t pos, size_t n) { return pread(fd, dst + pos, n, (off_t)(b.file_off + pos)); });
+        if (rc < 0) return fail(VMIG_EIO, "pread %s: %s", s.rel.c_str(), errno_str(errno).c_str());
+        if (rc) return fail(VMIG_ESRCCHANGED, "snapshot file %s shrank (wanted %u bytes at %llu, got %zu)", s.rel.c_str(), b.len, (unsigned long long)b.file_off, got);
+        if (f.reads_left.fetch_sub(1) == 1) close(f.sfd.exchange(-1));
+        return VMIG_OK;
+    }
+    int write_block(const BlockRef& b, const uint8_t* src) override {
+        FS& f = fs[b.file];
+        int fd = f.dfd.load(std::memory_order_acquire);
+        if (fd < 0) {                               // one writer per file (write_key): no other thread opens it
+            const int rc = prepare(b.file, &fd);
+            if (rc) return rc;
+            f.dfd.store(fd, std::memory_order_release);
+        }
+        size_t put;
+        const int rc = xfer_block(f.d_direct, true, b.len, &put, [&](size_t pos, size_t n) { return pwrite(fd, src + pos, n, (off_t)(b.file_off + pos)); });
+        const std::string& rel = snap->files[plan->files[b.file].snap].rel;
+        if (rc < 0) return fail(VMIG_EIO, "pwrite %s/%s: %s", layer_root.c_str(), rel.c_str(), errno_str(errno).c_str());
+        if (rc) return fail(VMIG_EIO, "pwrite %s/%s: wrote 0 bytes", layer_root.c_str(), rel.c_str());
+        return VMIG_OK;
+    }
+    int block_done(const BlockRef& b, bool) override {
+        if (fs[b.file].blocks_left.fetch_sub(1) != 1) return VMIG_OK;
+        const int fd = fs[b.file].dfd.exchange(-1);
+        return fd >= 0 ? finish(b.file, fd) : VMIG_OK;
+    }
+    ~RollbackIO() {
+        for (size_t i = 0; fs && i < plan->files.size(); i++) {     // what a failed pass left open
+            const int a = fs[i].sfd.exchange(-1); if (a >= 0) close(a);
+            const int d = fs[i].dfd.exchange(-1); if (d >= 0) close(d);
+        }
+    }
+
+private:
+    struct FS {
+        std::atomic<int> sfd{-1}, dfd{-1};
+        std::atomic<uint64_t> reads_left{0}, blocks_left{0};
+        bool s_direct = false, d_direct = false;
+    };
+    std::unique_ptr<FS[]> fs;
+    std::mutex stripes[64];
+};
+
+int rollback_body(CallScope& call, const char* layer_dir, const char* layer_table, const char* snap_dir, const char* snap_table,
+                  const char* out_table, const vmig_opts& o, vmig_stats* stats_out, vmig_rollback_stats* rs_out)
+{
+    const std::atomic<int>* cancel = call.cancel();
+    vmig_stats st; memset(&st, 0, sizeof st);
+    const uint64_t t_begin = now_ns();
+    BlockTable snap_tab, layer_tab;
+    int rc = layer_call_checks(call, layer_dir, layer_table, snap_dir, snap_table, o, &snap_tab, &layer_tab);
+    if (rc) return rc;
+    const BlockTable* ltab = layer_table && *layer_table ? &layer_tab : nullptr;
+    const std::string layer(layer_dir);
+
+    // ---- the snapshot's walk, which must be the tree its table describes before the layer is touched
+    call.phase(VMIG_PHASE_WALK);
+    uint64_t t0 = now_ns();
+    Manifest snap;
+    std::vector<uint64_t> snap_hashes;
+    rc = walk_tree(snap_dir, o.block_bytes, (o.flags & VMIG_F_SKIP_HIDDEN_TOPDIRS) != 0, &snap, cancel);
+    if (!rc) rc = match_table(snap, snap_tab, &snap_hashes);
+    if (rc) return rc;
+    st.ns_walk = now_ns() - t0;
+
+    // ---- what the snapshot does not list goes first, as in a pruning restore; the layer is walked as it then stands
+    call.phase(VMIG_PHASE_PRUNE);
+    rc = prune_extras(layer, snap, false, &st.pruned, cancel);
+    if (rc) return rc;
+
+    // ---- the layer's hashes (compare's read plan), each identity they speak for taken before the read and after it
+    call.phase(VMIG_PHASE_DATA);
+    LayerSide L;
+    std::vector<LayerId> ids;
+    rc = layer_plan(layer_dir, snap, ltab, o, cancel, &L, &st);
+    if (!rc) rc = rollback_identify(layer, L.man, L.plan, ltab, &ids);
+    if (!rc) rc = layer_hash_pass(call, o, snap, snap_hashes, ltab, &L, &st);
+    if (!rc) rc = rollback_recheck_paths(layer, L.man, ids);
+    if (rc) return rc;
+    const uint64_t hashed_bytes = st.bytes_total, hashed_blocks = st.blocks_total;
+
+    // ---- the plan: one action per snapshot file, the sparse fetch list, the copy runs
+    t0 = now_ns();
+    RollbackPlan rp;
+    rollback_plan(L.man, snap, snap_hashes, L.plan, L.hashes, ids, o.block_bytes, geteuid(), &rp);
+    call.ctl->bytes_total.store(hashed_bytes + rp.bytes_fetched); call.ctl->blocks_total.store(hashed_blocks + rp.blocks_fetched);
+    st.ns_plan += now_ns() - t0;
+
+    // ---- the fetch pass: every block the layer lacks, checked by K1 against the snapshot's table before it is written
+    t0 = now_ns();
+    if (cancel->load()) return fail(VMIG_ECANCELED, "before the layer's directories were made");
+    rc = make_dirs(layer, snap);
+    if (rc) return rc;
+    RollbackIO rio;
+    rio.snap = &snap; rio.plan = &rp; rio.ids = &ids; rio.layer_root = layer; rio.direct = (o.flags & VMIG_F_DIRECT_IO) != 0;
+    rio.block_bytes = o.block_bytes; rio.cancel = cancel;
+    rio.init();
+    VersionRoots sroot(1);
+    if (!rp.fetch.empty() && (rc = sroot.open(0, snap_dir))) return rc;
+    rio.snap_fd = sroot.fds[0];
+    for (uint32_t i = 0; i < rp.files.size(); i++) {        // files that take no block from the snapshot
+        const RollbackFile& rf = rp.files[i];
+        if (rf.n_fetch || rf.action == kRbKeep) continue;
+        if (cancel->load()) return fail(VMIG_ECANCELED, "before %s was made ready", snap.files[rf.snap].rel.c_str());
+        int fd;
+        rc = rio.prepare(i, &fd);
+        if (!rc) rc = rio.finish(i, fd);
+        if (rc) return rc;
+    }
+    std::vector<uint64_t> fetched(snap.n_blocks, 0);
+    rc = run_blocks(rp.fetch, &rio, false, false, o, fetched.data(), &st, call.ctl, false, snap_hashes.data());
+    st.ns_data += now_ns() - t0;
+    if (rc) return rc;
+
+    // ---- metadata: each regular file's where it differs, then the restore's replay; the layer now holds the table's bytes
+    t0 = now_ns();
+    call.phase(VMIG_PHASE_META);
+    FileIO io;
+    io.src_root = snap_dir; io.dst_root = layer; io.pol = default_meta_policy(o.flags); io.block_bytes = o.block_bytes;
+    io.direct = (o.flags & VMIG_F_DIRECT_IO) != 0;
+    TreePlan whole;                                  // every block of the snapshot's files: what VMIG_F_VERIFY re-reads
+    whole.files.resize(snap.files.size());
+    {
+        std::vector<BlockSpan> spans;
+        for (uint32_t f = 0; f < snap.files.size(); f++)
+            if (snap.files[f].hardlink_of < 0 && snap.files[f].n_blocks) spans.push_back({f, snap.files[f].size, snap.files[f].first_block, snap.files[f].n_blocks});
+        interleave_blocks(spans, o.block_bytes, &whole.blocks);
+    }
+    io.init_files(snap, whole);
+    for (size_t i = 0; i < rp.files.size(); i++) {
+        if (i % kMetaCheckEvery == 0 && cancel->load()) return fail(VMIG_ECANCELED, "before the metadata of %s", snap.files[rp.files[i].snap].rel.c_str());
+        const Entry& e = snap.files[rp.files[i].snap];
+        const std::string p = pjoin(layer, e.rel);
+        const int fd = open(p.c_str(), O_RDONLY | O_CLOEXEC | O_NOFOLLOW | O_NONBLOCK);
+        if (fd < 0 && errno != EACCES) return fail(VMIG_EIO, "open %s: %s", p.c_str(), errno_str(errno).c_str());
+        if (fd < 0) rc = apply_file_meta(-1, p, e, io.pol);          // an ordinary user's unreadable file: by path
+        else rc = file_meta_matches(fd, e, io.pol) ? VMIG_OK : apply_file_meta(fd, p, e, io.pol);     // a kept file's ctime stays
+        if (fd >= 0) close(fd);
+        if (rc) return rc;
+    }
+    std::vector<uint64_t> hashes(snap_hashes);
+    rc = meta_pass(call, io, snap_hashes, &hashes, &st, 0, false);
+    if (rc) return rc;
+    st.ns_meta = now_ns() - t0;
+
+    vmig_opts vo = o;
+    vo.flags |= VMIG_F_PRUNE;                        // the verify's entry-set check is the pruning restore's
+    if (o.flags & VMIG_F_VERIFY) {
+        call.phase(VMIG_PHASE_VERIFY);
+        rc = verify_pass(call, vo, io, hashes, &st, nullptr);
+        if (rc) return rc;
+    }
+
+    // ---- the table: the snapshot's hashes, and each layer file's identity as the call leaves it
+    t0 = now_ns();
+    call.phase(VMIG_PHASE_TABLE);
+    for (uint32_t f = 0; f < snap.files.size(); f++) {
+        if (snap.files[f].hardlink_of >= 0) continue;
+        const std::string p = pjoin(layer, snap.files[f].rel);
+        struct stat ls;
+        if (lstat(p.c_str(), &ls) != 0) return fail(VMIG_EIO, "lstat %s: %s", p.c_str(), errno_str(errno).c_str());
+        io.fs[f].identify(ls);
+    }
+    rc = write_table(io, false, out_table, hashes, cancel);
+    if (rc) return rc;
+    st.ns_table = now_ns() - t0;
+
+    st.files_direct += rio.n_direct.load();
+    st.bytes_total = hashed_bytes + rp.bytes_fetched; st.blocks_total = hashed_blocks + rp.blocks_fetched;
+    st.files = snap.files.size(); st.dirs = snap.dirs.size();
+    st.ns_total = now_ns() - t_begin;
+    if (stats_out) *stats_out = st;
+    if (rs_out) {
+        vmig_rollback_stats rs; memset(&rs, 0, sizeof rs);
+        rs.files_kept = rp.files_kept; rs.files_patched = rp.files_patched; rs.files_rebuilt = rp.files_rebuilt;
+        rs.files_created = rp.files_created; rs.blocks_fetched = rp.blocks_fetched; rs.bytes_fetched = rp.bytes_fetched;
+        rs.files_trusted = L.plan.files_trusted; rs.files_read = L.plan.inodes.size(); rs.bytes_read = L.plan.bytes_read;
+        rs.bytes_copied = rio.b_copied.load();
+        *rs_out = rs;
+    }
     return VMIG_OK;
 }
 
@@ -1559,6 +1884,34 @@ int vmig_compare_snapshot(const char* layer_dir, const char* layer_table, const 
     if (rc) return rc;
     return in_call(o.ctl, [&](CallScope& call) {
         return compare_body(call, layer_dir, layer_table, snap_dir, snap_table, report_path, o, stats, cmp_stats);
+    });
+}
+int vmig_rollback_layer(const char* layer_dir, const char* layer_table, const char* snap_dir, const char* snap_table,
+                        const char* out_table, const vmig_opts* opts, vmig_stats* stats, vmig_rollback_stats* rb_stats)
+{
+    if (!layer_dir || !*layer_dir) return fail(VMIG_EINVAL, "layer_dir is NULL/empty");
+    if (!snap_dir || !*snap_dir) return fail(VMIG_EINVAL, "snap_dir is NULL/empty");
+    if (!snap_table || !*snap_table) return fail(VMIG_EINVAL, "snap_table is NULL/empty: a layer is only rolled back to a snapshot through its block table");
+    const vmig_opts o = norm_opts(opts);                     // VMIG_CUFILE=1 in the environment is refused too
+    const uint32_t allowed = VMIG_F_DIRECT_IO | VMIG_F_SKIP_HIDDEN_TOPDIRS | VMIG_F_MTIME_NS | VMIG_F_NO_METADATA | VMIG_F_VERIFY | VMIG_F_PRUNE;
+    if (o.flags & ~allowed)
+        return fail(VMIG_EINVAL, "flags 0x%x: a rollback takes only VMIG_F_DIRECT_IO, VMIG_F_SKIP_HIDDEN_TOPDIRS, VMIG_F_MTIME_NS, "
+                    "VMIG_F_NO_METADATA, VMIG_F_VERIFY and VMIG_F_PRUNE", o.flags & ~allowed);
+    int rc = check_block_bytes(o);
+    if (rc) return rc;
+    std::string rl, rs;
+    if (real_paths_overlap(layer_dir, snap_dir, &rl, &rs))
+        return fail(VMIG_EINVAL, "layer_dir %s and snap_dir %s are the same directory or one is inside the other", rl.c_str(), rs.c_str());
+    if (out_table && *out_table) {
+        std::string ro, rt;
+        rc = real_parent_path(out_table, &ro);
+        if (!rc) rc = real_parent_path(snap_table, &rt);
+        if (rc) return rc;
+        if (ro == rt || (!rs.empty() && path_inside(ro, rs)))
+            return fail(VMIG_EINVAL, "out_table %s is the snapshot's table or lies inside snap_dir: the store is never written", out_table);
+    }
+    return in_call(o.ctl, [&](CallScope& call) {
+        return rollback_body(call, layer_dir, layer_table, snap_dir, snap_table, out_table, o, stats, rb_stats);
     });
 }
 int vmig_copy_dir(const char* src_dir, const char* dst_dir) { return migrate_tree_impl(src_dir, dst_dir, nullptr, nullptr, nullptr, nullptr); }

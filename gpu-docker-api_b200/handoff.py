@@ -22,8 +22,8 @@ from typing import Callable, Optional
 import threading
 
 from . import (F_PRUNE, F_VERIFY, VMIG_ECANCELED, Ctl, GetContainerMergedLayer, GetVolumeMountPoint, VmigError,
-               compare_snapshot, manifest, migrate_tree, restore_paths, restore_tree, retire_versions, scrub_store,
-               snapshot_tree)
+               compare_snapshot, manifest, migrate_tree, restore_paths, restore_tree, retire_versions, rollback_layer,
+               scrub_store, snapshot_tree)
 
 log = logging.getLogger("vmig.handoff")
 _root: dict = {"cwd": None}
@@ -214,6 +214,24 @@ def CompareWithVersion(targetCtrVersionName: str, container: str, report) -> dic
         if ownTable.exists():
             layerTable = ownTable
     return compare_snapshot(upper, data, table, report, layerTable)
+
+
+def RollbackInPlace(targetCtrVersionName: str, container: str) -> dict:
+    """N1: roll the stopped container's layer back to version `target` in place: afterwards it is what
+    RollbackFromSnapshot would leave, but only the snapshot blocks the layer does not already hold are read, so a
+    rollback costs what differs, not the size of the version.  When the container's own version directory has no diff/,
+    its blocks.vmig is the table HandoffCopy wrote for the layer: it is the layer's table (files still as it recorded them
+    are not read) and is rewritten for the rolled-back layer.  Otherwise no table is written.
+      - The container must not be running: the upper dir of a mounted overlay must not change under it.
+      - No REST route is added; the control plane stays as it is."""
+    data, table = snapshotPaths(targetCtrVersionName)
+    upper = GetContainerMergedLayer(container)
+    ownData, ownTable = snapshotPaths(container)
+    layerTable = None
+    if not ownData.exists():
+        if ownTable.exists():
+            layerTable = ownTable
+    return rollback_layer(upper, data, table, layerTable, layerTable, flags=F_VERIFY)
 
 
 def HandoffCopy(oldContainer: str, newContainer: str, pause: Callable[[str], None], resume: Callable[[str], None],

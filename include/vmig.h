@@ -469,7 +469,9 @@ typedef struct vmig_compare_stats {
  *   - bytes_restore, summed over the snapshot's regular-file paths (each path of a hard-link group once): where the
  *     layer has a regular file at the path, the snapshot lengths of the blocks past the layer file's last block or
  *     whose (length, hash) differs; otherwise the snapshot file's whole size.  It is the content a rollback has to
- *     bring back.  A rollback without a trusted seed table (prior_table) copies more than this: whole files.
+ *     bring back: vmig_rollback_layer reads exactly this from the snapshot (its bytes_fetched), less what this sum
+ *     counts for the second and later paths of a snapshot hard-link group, which the rollback links to the group's
+ *     first path instead of reading them.  vmig_restore_tree reads the whole snapshot.
  *   - Control: vmig_opts.ctl as for the tree calls; phases WALK, DATA, DONE; a cancel is honoured per directory of the
  *     walks, in the block pipeline and before the report is renamed into place.  bytes_total / blocks_total are the
  *     bytes and blocks to be read.  stats (nullable): the vmig_stats of the data pass (bytes_h2d == bytes_read, 0 when
@@ -479,6 +481,91 @@ int vmig_compare_snapshot(const char* layer_dir, const char* layer_table /*nulla
                           const char* report_path /*nullable*/,
                           const vmig_opts* opts /*nullable*/, vmig_stats* stats /*nullable*/,
                           vmig_compare_stats* cmp_stats /*nullable*/);
+
+/* An in-place rollback of a layer to a version snapshot: what vmig_rollback_layer did and read. */
+typedef struct vmig_rollback_stats {
+    uint64_t files_kept;            /* regular files whose size and every block already were the snapshot's: not written   */
+    uint64_t files_patched;         /* written in place: only the differing blocks, then cut or grown to the snapshot's size */
+    uint64_t files_rebuilt;         /* replaced by a new inode: blocks the old inode held copied from it, the rest fetched  */
+    uint64_t files_created;         /* no usable regular file at the path: fetched from the snapshot in full                */
+    uint64_t blocks_fetched, bytes_fetched;   /* snapshot blocks read and checked on the GPU                                */
+    uint64_t files_trusted;         /* layer files whose hashes came from layer_table                                       */
+    uint64_t files_read, bytes_read;          /* distinct layer inodes hashed on the GPU                                    */
+    uint64_t bytes_copied;          /* rebuilt files' bytes copied from their old inode (copy_file_range)                   */
+    uint64_t reserved[4];
+} vmig_rollback_stats;
+
+/* Roll the layer layer_dir back to the version snapshot snap_dir (written with its block table snap_table by
+ * vmig_snapshot_tree) in place, reading from the snapshot only the blocks the layer does not already hold.  Its cost is
+ * the difference between the layer and the version -- the layer bytes that have to be hashed (none that layer_table
+ * still vouches for) plus vmig_compare_snapshot's bytes_restore -- where vmig_restore_tree reads the whole version.
+ *   - Result: on success layer_dir is what vmig_restore_tree(snap_dir, snap_table, layer_dir, NULL, out_table,
+ *     flags | VMIG_F_PRUNE) leaves: entries, types, contents, permission bits, owners, mtimes (whole seconds, or ns with
+ *     VMIG_F_MTIME_NS), symlink targets, device numbers and in-tree hard-link grouping.  The call always prunes;
+ *     VMIG_F_PRUNE is accepted and changes nothing.
+ *   - Refusals, in this order, each before anything is read or written: VMIG_EINVAL (layer_dir, snap_dir or snap_table
+ *     NULL or empty; flags other than VMIG_F_DIRECT_IO | VMIG_F_SKIP_HIDDEN_TOPDIRS | VMIG_F_MTIME_NS |
+ *     VMIG_F_NO_METADATA | VMIG_F_VERIFY | VMIG_F_PRUNE; bad block_bytes; layer_dir and snap_dir the same directory or
+ *     one inside the other, by real path; out_table equal to snap_table or inside snap_dir -- out_table == layer_table
+ *     is allowed, it is how a hand-off's table is carried forward); a control cancelled before the call:
+ *     VMIG_ECANCELED; VMIG_ENOTDIR (either directory missing or not a directory); VMIG_ETABLE (either table does not
+ *     load, or its block_bytes differs from the call's); VMIG_ENOGPU (no CPU fallback, even when nothing needs reading).
+ *   - Snapshot side: snap_dir is walked for metadata and must match snap_table in paths and sizes before the layer is
+ *     touched (VMIG_ECORRUPT with the restore's message otherwise).  Then the layer is pruned as a pruning restore
+ *     prunes it, and walked.
+ *   - Layer hashes: exactly vmig_compare_snapshot's sources -- the snapshot path's own inode (shared), a record of
+ *     layer_table the file still is (trusted), or one hash-only read per distinct inode through the GPU (files_read,
+ *     bytes_read).  The identity each speaks for (a trusted file's record; otherwise an lstat taken before the read)
+ *     must still be what an lstat shows after the read, or the call fails with VMIG_ESRCCHANGED.
+ *   - One action per snapshot regular file (a hard-link group's first path; the others are linked to it afterwards):
+ *       keep     the layer file at the path is patchable, has the same size and every (length, XXH64) equal: nothing is
+ *                read or written; its metadata is replayed only where it differs, so its ctime and identity stay;
+ *       patch    patchable and something differs: the file is set to the snapshot's size, then the differing blocks --
+ *                and every block past the layer file's old end -- are fetched and written in place.  Patchable: a
+ *                regular file whose hashes came from a trusted record or a read (not a shared inode), with one link,
+ *                writable by the caller (root, or the owner with S_IWUSR: a read-only file is replaced, as tar replaces
+ *                it), and neither path is in a hard-link group;
+ *       rebuild  a regular file that is not patchable (an inode shared with the snapshot -- a restore never lets a layer
+ *                share an inode with the store --, a link held outside the tree, a hard-link group): the old inode is
+ *                opened, the path replaced by a new file, the blocks equal at the same index copied from the old inode
+ *                in coalesced runs (copy_file_range), the rest fetched (the old inode is opened for reading only when
+ *                something is copied from it);
+ *       create   no regular file at the path: every block is fetched.
+ *     The match is positional (same path, same block index), as vmig_compare_snapshot's.
+ *   - Before the first write into a patched file and before copying from a rebuilt file's old inode, the open
+ *     descriptor's inode, size and ctime must be the ones the plan trusted, else VMIG_ESRCCHANGED naming the path.  The
+ *     call's own unlink of another path of a rebuilt inode (a layer hard-link group the snapshot holds as separate
+ *     files) moves its ctime too; that change, and only that, is allowed for.  The
+ *     layer must not be in use (as for vmig_restore_paths).
+ *   - What is checked: every fetched block is hashed by K1 against snap_table, as a restore checks it, and a mismatch is
+ *     VMIG_ECORRUPT before any block of its batch is written.  Snapshot blocks that are not fetched are not read: the
+ *     layer already holds bytes with the table's hash.  A rotted snapshot block the layer does not need therefore
+ *     neither fails the call nor reaches the layer; finding it is vmig_scrub_store's job.
+ *   - The store is only read: nothing is written under snap_dir.  After success no layer regular file shares an inode
+ *     with a snapshot file.  Replacing a layer path that was a hard link to a snapshot inode unlinks it, which moves
+ *     that inode's ctime as every unlink does (its table record then no longer vouches for it, so the next snapshot
+ *     based on that version re-reads it); no other snapshot inode's ctime moves.
+ *   - VMIG_F_VERIFY: every regular file of the layer is re-read through the GPU and must hash as snap_table says, then
+ *     the layer's entry set must be the snapshot's (the pruning restore's check).
+ *   - out_table (nullable): the restore's out table -- snap_table's paths, sizes and hashes, and the identities of the
+ *     layer files as the call leaves them.  Handed back as layer_table it vouches for every file.
+ *   - Control: vmig_opts.ctl as for the tree calls; phases WALK, PRUNE, DATA (the layer's hash pass, then the fetch
+ *     pass), META, (VERIFY), TABLE, DONE.  bytes_total / blocks_total are the layer bytes to hash plus the snapshot
+ *     bytes to fetch.  A cancel is honoured per directory of the walks, per entry of the prune, in both block
+ *     pipeline passes, per <= 64 MiB chunk of a rebuilt file's copy, per <= 1024 metadata entries and before the table
+ *     is renamed into place.  A failed or cancelled call leaves what a failed restore leaves: no out_table and no .tmp,
+ *     both tables and the snapshot untouched, the layer possibly partly written but never with a block that failed a
+ *     check; a file patched part way carries a moved ctime, so the next pass copies it in full.
+ *   - stats (nullable): the vmig_stats of both passes (bytes_h2d == bytes_read + bytes_fetched, plus the re-read with
+ *     VMIG_F_VERIFY).  rb_stats (nullable): the counters above, written on success.  On the same layer state with the
+ *     same layer_table, files_read and bytes_read equal vmig_compare_snapshot's, and bytes_fetched equals its
+ *     bytes_restore less the second and later paths of snapshot hard-link groups.  One exception to the first: the
+ *     prune runs before the layer's trust is taken, so a file layer_table vouches for whose extra hard link the prune
+ *     removes has a moved ctime and is read, where a compare of the state before the call trusts it. */
+int vmig_rollback_layer(const char* layer_dir, const char* layer_table /*nullable*/,
+                        const char* snap_dir, const char* snap_table, const char* out_table /*nullable*/,
+                        const vmig_opts* opts /*nullable*/, vmig_stats* stats /*nullable*/,
+                        vmig_rollback_stats* rb_stats /*nullable*/);
 
 /* utils.CopyDir(src, dest) (reference utils/copy.go:21-27) == vmig_migrate_tree with defaults. */
 int vmig_copy_dir(const char* src_dir, const char* dst_dir);
@@ -502,7 +589,7 @@ void vmig_host_free(void* p);
 
 /* ---- cancellation and progress ------------------------------------------------------------------
  * A control is a numeric id (cgo passes it in vmig_opts.ctl without any pointer rules).  It serves the entry points
- * that take vmig_opts: vmig_migrate_tree, vmig_restore_tree, vmig_restore_paths, vmig_snapshot_tree, vmig_scrub_store, vmig_retire_versions, vmig_compare_snapshot and vmig_migrate_buffer (a caller that
+ * that take vmig_opts: vmig_migrate_tree, vmig_restore_tree, vmig_restore_paths, vmig_snapshot_tree, vmig_scrub_store, vmig_retire_versions, vmig_compare_snapshot, vmig_rollback_layer and vmig_migrate_buffer (a caller that
  * wants to cancel a copy or a move calls vmig_migrate_tree with the flags vmig_copy_dir / vmig_move_dir use).  One
  * control serves one call at a time: attaching it to a second concurrent call fails with VMIG_EINVAL.  The engine has
  * no deadline of its own; a deadline is the caller's timer calling vmig_ctl_cancel.

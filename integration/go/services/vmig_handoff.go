@@ -270,6 +270,30 @@ func CompareWithVersion(targetCtrVersionName, container, report string) (utils.C
 	return st, errors.WithMessagef(err, "compare of %s with %s failed", container, targetCtrVersionName)
 }
 
+// N1 -- RollbackInPlace rolls the stopped container's layer back to version `target` in place: afterwards it is what
+// RollbackFromSnapshot would leave, but only the snapshot blocks the layer does not already hold are read, so a rollback
+// costs what differs, not the size of the version.  When the container's own version directory has no diff/, its
+// blocks.vmig is the table HandoffCopy wrote for the layer: it is the layer's table (files still as it recorded them
+// are not read) and is rewritten for the rolled-back layer.  Otherwise no table is written.
+//   - The container must not be running: the upper dir of a mounted overlay must not change under it.
+//   - No REST route is added; the control plane stays as it is.
+func RollbackInPlace(targetCtrVersionName, container string) (utils.RollbackStats, error) {
+	data, table := snapshotPaths(targetCtrVersionName)
+	upper, err := utils.GetContainerMergedLayer(container)
+	if err != nil {
+		return utils.RollbackStats{}, errors.WithMessagef(err, "utils.GetContainerMergedLayer failed, container: %s", container)
+	}
+	ownData, ownTable := snapshotPaths(container)
+	layerTable := ""
+	if _, err := os.Stat(ownData); os.IsNotExist(err) {
+		if _, err := os.Stat(ownTable); err == nil {
+			layerTable = ownTable
+		}
+	}
+	st, err := utils.RollbackLayer(upper, layerTable, data, table, layerTable)
+	return st, errors.WithMessagef(err, "rollback of %s to %s failed", container, targetCtrVersionName)
+}
+
 // N2 -- HandoffCopy replaces utils.CopyOldMergedToNewContainerMerged in PatchContainer (replicaset.go:333):
 // the old container keeps running during pass 1 (the bulk of the bytes), is paused for pass 2, which re-reads
 // the source and moves only the blocks whose hash changed in between, and stays paused until the caller has

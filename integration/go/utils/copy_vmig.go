@@ -277,6 +277,69 @@ func CompareWithSnapshotContext(ctx context.Context, layer, layerTable, snapDir,
 	return out, nil
 }
 
+// RollbackStats is what RollbackLayer did and read (vmig_rollback_stats).
+type RollbackStats struct {
+	FilesKept, FilesPatched, FilesRebuilt, FilesCreated uint64
+	BlocksFetched, BytesFetched                         uint64 // snapshot blocks read and checked on the GPU
+	FilesTrusted, FilesRead, BytesRead                  uint64
+	BytesCopied                                         uint64 // rebuilt files' bytes copied from their old inode
+}
+
+// RollbackLayer rolls the layer back to the snapshot snapDir (checked against snapTable) in place
+// (vmig_rollback_layer): afterwards it is what a verified, pruning restore of the snapshot into it leaves, but only the
+// snapshot blocks the layer does not already hold are read.  layerTable ("" for none) is a table of the layer whose
+// records still vouch for their files; outTable ("" for none) receives the layer's new table and may be layerTable.
+func RollbackLayer(layer, layerTable, snapDir, snapTable, outTable string) (RollbackStats, error) {
+	return RollbackLayerContext(context.Background(), layer, layerTable, snapDir, snapTable, outTable)
+}
+
+// RollbackLayerContext is RollbackLayer that stops when ctx is done (see CopyDirDiffContext); no out table is written
+// then, and the layer may be partly rolled back (never with a block that failed its check).
+func RollbackLayerContext(ctx context.Context, layer, layerTable, snapDir, snapTable, outTable string) (RollbackStats, error) {
+	cl, cs, ct := C.CString(layer), C.CString(snapDir), C.CString(snapTable)
+	defer C.free(unsafe.Pointer(cl))
+	defer C.free(unsafe.Pointer(cs))
+	defer C.free(unsafe.Pointer(ct))
+	var clt, co *C.char
+	if layerTable != "" {
+		clt = C.CString(layerTable)
+		defer C.free(unsafe.Pointer(clt))
+	}
+	if outTable != "" {
+		co = C.CString(outTable)
+		defer C.free(unsafe.Pointer(co))
+	}
+	var st C.vmig_stats
+	var rb C.vmig_rollback_stats
+	var o C.vmig_opts
+	o.flags = C.VMIG_F_VERIFY
+	var id C.uint32_t
+	if err := lockedCall("vmig_ctl_open", func() C.int { return C.vmig_ctl_open(&id) }); err != nil {
+		return RollbackStats{}, err
+	}
+	defer C.vmig_ctl_close(id)
+	stop := context.AfterFunc(ctx, func() { C.vmig_ctl_cancel(id) })
+	defer stop()
+	o.ctl = id
+	var rc C.int
+	err := lockedCall("vmig_rollback_layer", func() C.int {
+		rc = C.vmig_rollback_layer(cl, clt, cs, ct, co, &o, &st, &rb)
+		return rc
+	})
+	if rc == C.VMIG_ECANCELED && ctx.Err() != nil {
+		return RollbackStats{}, fmt.Errorf("%w: %v", ctx.Err(), err)
+	}
+	if err != nil {
+		return RollbackStats{}, err
+	}
+	out := RollbackStats{uint64(rb.files_kept), uint64(rb.files_patched), uint64(rb.files_rebuilt), uint64(rb.files_created),
+		uint64(rb.blocks_fetched), uint64(rb.bytes_fetched), uint64(rb.files_trusted), uint64(rb.files_read), uint64(rb.bytes_read),
+		uint64(rb.bytes_copied)}
+	log.Infof("vmig: rolled %s back to %s: %d kept, %d patched, %d rebuilt, %d created; %d bytes fetched, %d read, %d copied",
+		layer, snapDir, out.FilesKept, out.FilesPatched, out.FilesRebuilt, out.FilesCreated, out.BytesFetched, out.BytesRead, out.BytesCopied)
+	return out, nil
+}
+
 // RetireSnapshots removes the snapshots retireDirs[i] with their tables retireTables[i] and keeps keepDirs[i] /
 // keepTables[i] usable as bases (vmig_retire_versions): each retired table goes first, then its tree, never following
 // a symlink; then the kept tables' records whose ctime the removal moved are re-verified on the GPU and re-recorded.

@@ -49,6 +49,7 @@ EXPORTS = [
     "vmig_table_hashes", "vmig_dir_size", "vmig_to_bytes", "vmig_datagen_files", "vmig_manifest", "vmig_link_probe", "vmig_thread_plan",
     "vmig_ctl_open", "vmig_ctl_cancel", "vmig_ctl_progress", "vmig_ctl_close", "vmig_scrub_store",
     "vmig_retire_versions", "vmig_restore_paths", "vmig_compare_snapshot", "vmig_rollback_layer",
+    "vmig_snapshot_layer",
 ]
 SCRUB_KINDS = ("missing", "extra", "resized", "block", "hardlink", "unreadable", "table", "dir")
 COMPARE_KINDS = ("added", "removed", "type", "resized", "block", "target", "rdev", "hardlink", "mode", "owner", "mtime")
@@ -123,6 +124,15 @@ class RollbackStats(C.Structure):
         return {n: getattr(self, n) for n, _ in self._fields_ if n != "reserved"}
 
 
+class LayerSnapshotStats(C.Structure):
+    _fields_ = [(n, C.c_uint64) for n in ("files_linked", "bytes_linked", "files_backfilled", "bytes_backfilled",
+                                          "files_base_untrusted", "files_trusted", "bytes_trusted", "files_read",
+                                          "bytes_read")] + [("reserved", C.c_uint64 * 4)]
+
+    def as_dict(self) -> dict:
+        return {n: getattr(self, n) for n, _ in self._fields_ if n != "reserved"}
+
+
 class TableInfo(C.Structure):
     _fields_ = [("block_bytes", C.c_uint32), ("algo", C.c_uint32), ("n_files", C.c_uint64),
                 ("n_blocks", C.c_uint64), ("bytes_total", C.c_uint64)]
@@ -182,6 +192,8 @@ _sig = {
                                         C.POINTER(Stats), C.POINTER(CompareStats)]),
     "vmig_rollback_layer": (C.c_int, [C.c_char_p, C.c_char_p, C.c_char_p, C.c_char_p, C.c_char_p, C.POINTER(Opts),
                                       C.POINTER(Stats), C.POINTER(RollbackStats)]),
+    "vmig_snapshot_layer": (C.c_int, [C.c_char_p, C.c_char_p, C.c_char_p, C.c_char_p, C.c_char_p, C.c_char_p,
+                                      C.POINTER(Opts), C.POINTER(Stats), C.POINTER(LayerSnapshotStats)]),
 }
 for _n, (_r, _a) in _sig.items():
     _f = getattr(_lib, _n)
@@ -230,7 +242,7 @@ def _b(p) -> Optional[bytes]:
 
 class Ctl:
     """A call control (vmig_ctl_*): pass it as ``ctl=`` to migrate_tree, restore_tree, restore_paths, snapshot_tree,
-    scrub_store, retire_versions, compare_snapshot, rollback_layer or migrate_buffer,
+    scrub_store, retire_versions, compare_snapshot, rollback_layer, snapshot_layer or migrate_buffer,
     then cancel() from any thread (the call raises VmigError(VMIG_ECANCELED)) or read progress() while it runs.  ctypes
     releases the GIL during the call.  One control serves one call at a time; a deadline is a threading.Timer."""
 
@@ -385,6 +397,21 @@ def snapshot_tree(src, dst, base=None, base_table=None, out_table=None, *, flags
     _check(_lib.vmig_snapshot_tree(_b(src), _b(dst), _b(base), _b(base_table), _b(out_table), C.byref(o), C.byref(st),
                                    C.byref(ss)), f"vmig_snapshot_tree({src} -> {dst}, base {base})")
     return {**st.as_dict(), **ss.as_dict()}
+
+
+def snapshot_layer(layer, dst, base, base_table, out_table, layer_table, *, flags: int = 0, gpu_mask: int = 0,
+                   block_bytes: int = 0, io_threads: int = 0, streams_per_gpu: int = 0, lanes_per_gpu: int = 0,
+                   ctl: Optional[Ctl] = None) -> dict:
+    """The snapshot snapshot_tree(layer, dst, base, base_table, out_table) writes, with the layer's hashes taken from
+    `layer_table` (the table written for the layer's files) wherever it still vouches for a file: of such a file only the
+    blocks the base does not hold are read.  F_VERIFY re-reads what was written or backfilled, not what was linked.
+    out_table may be layer_table.  Returns the migrate_tree counters plus the vmig_layer_snapshot_stats fields."""
+    o = Opts(gpu_mask=gpu_mask, block_bytes=block_bytes, flags=flags, io_threads=io_threads,
+             streams_per_gpu=streams_per_gpu, lanes_per_gpu=lanes_per_gpu, ctl=_ctl_id(ctl))
+    st, ls = Stats(), LayerSnapshotStats()
+    _check(_lib.vmig_snapshot_layer(_b(layer), _b(layer_table), _b(dst), _b(base), _b(base_table), _b(out_table), C.byref(o),
+                                    C.byref(st), C.byref(ls)), f"vmig_snapshot_layer({layer} -> {dst}, base {base})")
+    return {**st.as_dict(), **ls.as_dict()}
 
 
 def unescape_report_path(s: str) -> bytes:

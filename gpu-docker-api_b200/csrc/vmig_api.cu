@@ -158,21 +158,24 @@ public:
     }
     std::unique_ptr<FS[]> fs;
     std::mutex stripes[64];
-    // one FS per manifest file; a file's blocks count down to the close of its source and to its finalization
+    // one FS per manifest file; a file's blocks in the plan's list count down to the close of its source and to its
+    // finalization.  A file with blocks the plan already skipped (vmig_snapshot_layer) is finished from the base.
     void init_files(const Manifest& man, const TreePlan& p) {
         m = &man; plan = &p;
         fs.reset(new FS[man.files.size() ? man.files.size() : 1]);
-        for (uint32_t f = 0; f < man.files.size(); f++) {
-            const Entry& e = man.files[f];
-            if (e.hardlink_of >= 0 || e.n_blocks == 0) continue;
-            fs[f].reads_left.store((uint32_t)e.n_blocks); fs[f].blocks_left.store((uint32_t)e.n_blocks);
+        for (const BlockRef& b : p.blocks) { fs[b.file].reads_left.fetch_add(1, std::memory_order_relaxed); fs[b.file].blocks_left.fetch_add(1, std::memory_order_relaxed); }
+        if (!p.skipped.empty()) {
+            skipped = p.skipped;
+            for (uint32_t f = 0; f < man.files.size(); f++)
+                if (p.files[f].layer_rec)
+                    for (uint64_t r = 0; r < man.files[f].n_blocks; r++) if (p.skipped[man.files[f].first_block + r]) { fs[f].reused.store(true); break; }
         }
     }
 
     // vmig_snapshot_tree: the base snapshot whose files supply the blocks K1 found unchanged, at the same path and offset
     // or anywhere else in the base (bidx: every block of every trusted base file, by hash and length)
     std::string base_root;
-    BaseIndex bidx;
+    const BaseIndex* bidx = nullptr;                       // the plan's index (TreePlan::bidx)
     const uint64_t* hashes = nullptr;                      // the call's block hashes (a file's are all there when it finalizes)
     std::vector<uint8_t> skipped;                          // per table block: 1 = not written, its bytes are in the base
     std::mutex link_mu;
@@ -183,7 +186,7 @@ public:
     static constexpr size_t kLinkTries = 16;               // base files of equal content tried as a link target, per file
     bool done_on_writer(const BlockRef& b) override { return plan->files[b.file].base_rec != nullptr || fs[b.file].reused.load(); }
     bool reusable(const BlockRef& b, uint64_t hash) override {
-        if (bidx.empty() || !bidx.contains(hash, b.len)) return false;
+        if (!bidx || !bidx->contains(hash, b.len)) return false;
         skipped[b.table_idx] = 1;
         fs[b.file].reused.store(true);
         return true;
@@ -192,7 +195,7 @@ public:
     // Open base file g and check that it still is the file its record describes: same inode, and the recorded ctime or
     // the one this call's own link to it left.  Anything else changed it, and the bytes it was to supply are gone.
     int open_base(uint32_t g, int* out, struct stat* bs) {
-        const TableFile& bf = bidx.t->files[g];
+        const TableFile& bf = bidx->t->files[g];
         const std::string bp = pjoin(base_root, bf.rel);
         const int bfd = open(bp.c_str(), O_RDONLY | O_NOFOLLOW | O_CLOEXEC);
         bool same = bfd >= 0 && fstat(bfd, bs) == 0 && S_ISREG(bs->st_mode) && (uint64_t)bs->st_ino == bf.ino;
@@ -221,14 +224,14 @@ public:
         for (uint64_t r = 0; r < e.n_blocks && !any_skipped; r++) any_skipped = skipped[e.first_block + r] != 0;
         if (!any_skipped) return VMIG_OK;
         const FilePlan& fp = plan->files[f];
-        const int same = fp.base_rec ? (int)(fp.base_rec - bidx.t->files.data()) : -1;
+        const int same = fp.base_rec ? (int)(fp.base_rec - bidx->t->files.data()) : -1;
         const uint64_t* h = hashes + e.first_block;
         const std::string p = pjoin(dst_root, e.rel);
         if (!s.wrote.load() && fp.solo) {
             std::vector<uint32_t> cands;
-            link_candidates(bidx, same, e.size, block_bytes, h, &cands, kLinkTries);
+            link_candidates(*bidx, same, e.size, block_bytes, h, &cands, kLinkTries);
             for (uint32_t g : cands) {
-                const TableFile& bf = bidx.t->files[g];
+                const TableFile& bf = bidx->t->files[g];
                 { std::lock_guard<std::mutex> lk(link_mu); if (linked_inos.count(bf.ino)) continue; }
                 int bfd; struct stat bs;
                 int rc = open_base(g, &bfd, &bs);
@@ -254,7 +257,7 @@ public:
             }
         }
         std::vector<ReuseRun> runs;
-        int rc = plan_backfill(bidx, same, e.size, block_bytes, h, &skipped[e.first_block], e.rel, &runs);
+        int rc = plan_backfill(*bidx, same, e.size, block_bytes, h, &skipped[e.first_block], e.rel, &runs);
         if (rc) return rc;
         int dfd; rc = open_dst(f, &dfd);
         std::unordered_map<uint32_t, int> bfds;              // base files this file takes bytes from, each checked once
@@ -268,7 +271,7 @@ public:
                 if (rc) break;
                 it = bfds.emplace(u.file, bfd).first;
             }
-            rc = copy_range_at(it->second, u.src_off, dfd, u.dst_off, u.len, s.d_direct, false, pjoin(base_root, bidx.t->files[u.file].rel), cancel);
+            rc = copy_range_at(it->second, u.src_off, dfd, u.dst_off, u.len, s.d_direct, false, pjoin(base_root, bidx->t->files[u.file].rel), cancel);
             bytes += u.len;
         }
         for (auto& kv : bfds) close(kv.second);
@@ -434,13 +437,20 @@ public:
         if (!written && fp.base_rec) skipped[b.table_idx] = 1;          // (a reused block was marked by reusable())
         if (s.blocks_left.fetch_sub(1) != 1) return VMIG_OK;
         if (hash_only) return VMIG_OK;
-        const Entry& e = m->files[b.file];
+        return finish_file(b.file);
+    }
+    // The file's last block passed (or none is read: vmig_snapshot_layer's unread files): link or backfill from the base,
+    // else cut and apply metadata, and take the identity the table records
+    int finish_file(uint32_t f) {
+        FS& s = fs[f];
+        const FilePlan& fp = plan->files[f];
+        const Entry& e = m->files[f];
         if (fp.base_rec || s.reused.load()) {
             bool linked = false;
-            int rc = finish_from_base(b.file, &linked);
+            int rc = finish_from_base(f, &linked);
             if (rc || linked) return rc;
         }
-        int fd; int rc = open_dst(b.file, &fd);      // also covers "every block was skipped"
+        int fd; int rc = open_dst(f, &fd);      // also covers "every block was skipped"
         if (rc) return rc;
         const std::string p = pjoin(dst_root, e.rel);
         const bool inplace = fp.prior_rec != nullptr;
@@ -504,7 +514,7 @@ bool is_pinned(const void* p) {
 // contiguous byte-balanced ranges only when there are fewer than two files per lane
 // ctl: the call's control; a cancel sets this pipeline's first-error latch.  verify: progress goes to bytes_verified.
 int run_blocks(const std::vector<BlockRef>& blocks, BlockIO* io, bool has_prior, bool hash_only, const vmig_opts& o,
-               uint64_t* hashes, vmig_stats* st, CallCtl* ctl, bool verify, const uint64_t* expect = nullptr)
+               uint64_t* hashes, vmig_stats* st, CallCtl* ctl, bool verify, const BlockExpect* expect = nullptr)
 {
     std::vector<DeviceInfo> devs;
     int rc = ctx_select(o.gpu_mask, &devs);
@@ -639,6 +649,10 @@ struct SnapshotArgs {
     const char* base_dir;              // both NULL: a full snapshot
     const char* base_table;
     vmig_snapshot_stats* out;          // nullable
+    // vmig_snapshot_layer: both tables already loaded, and the source's own table
+    const BlockTable* base_loaded = nullptr;
+    const BlockTable* layer = nullptr;
+    vmig_layer_snapshot_stats* layer_out = nullptr;    // nullable
 };
 
 // After the data pass: hard-linked paths take their primary's hashes, empty regular files are created, then the rest of
@@ -683,9 +697,18 @@ int meta_pass(CallScope& call, FileIO& io, const std::vector<uint64_t>& expect, 
     return replay_metadata(io.dst_root, man, io.pol, &st->symlinks, &st->hardlinks, &st->specials, cancel, first_dir);
 }
 
-// VMIG_F_VERIFY: read the destination back through the same GPU path (hash only) and compare block tables
+// The manifest files that carry blocks (a hard-link group's first path): what VMIG_F_VERIFY re-reads, except
+// vmig_snapshot_layer's linked files
+std::vector<uint32_t> data_files(const Manifest& man)
+{
+    std::vector<uint32_t> out;
+    for (uint32_t f = 0; f < man.files.size(); f++) if (man.files[f].hardlink_of < 0 && man.files[f].n_blocks) out.push_back(f);
+    return out;
+}
+
+// VMIG_F_VERIFY: read the given destination files back through the same GPU path (hash only) and compare block tables
 int verify_pass(CallScope& call, const vmig_opts& o, const FileIO& io, const std::vector<uint64_t>& hashes, vmig_stats* st,
-                const std::vector<std::string>* prune_scope)
+                const std::vector<std::string>* prune_scope, const std::vector<uint32_t>& files)
 {
     const Manifest& man = *io.m;
     FileIO vio;
@@ -694,10 +717,14 @@ int verify_pass(CallScope& call, const vmig_opts& o, const FileIO& io, const std
     vio.cufile = io.cufile;
     TreePlan blank;                  // nothing patched in place or taken from a base: every block is read back
     blank.files.resize(man.files.size());
+    {
+        std::vector<BlockSpan> spans;
+        for (uint32_t f : files) spans.push_back({f, man.files[f].size, man.files[f].first_block, man.files[f].n_blocks});
+        interleave_blocks(spans, o.block_bytes, &blank.blocks);
+    }
     vio.init_files(man, blank);
     int rc = vio.open_root(); if (rc) return rc;
-    std::vector<BlockRef> vblocks = io.plan->blocks;
-    for (auto& b : vblocks) { b.prior_hash = 0; b.prior_valid = 0; }
+    const std::vector<BlockRef>& vblocks = blank.blocks;
     std::vector<uint64_t> vh(man.n_blocks, 0);
     vmig_stats vst; memset(&vst, 0, sizeof vst);
     rc = run_blocks(vblocks, &vio, false, true, o, vh.data(), &vst, call.ctl, true);
@@ -771,6 +798,49 @@ bool path_inside(const std::string& a, const std::string& root)
     return a == root || (a.size() > root.size() && a.compare(0, root.size(), root) == 0 && (root == "/" || a[root.size()] == '/'));
 }
 
+// vmig_snapshot_layer: the trusted layer files none of whose blocks is read are linked or backfilled from the base, then
+// finished, as their last block's writer finishes a file that was read; spread over as many threads as a lane has writers
+int finish_unread(CallScope& call, const vmig_opts& o, FileIO& io, const std::vector<uint32_t>& files)
+{
+    if (files.empty()) return VMIG_OK;
+    uint32_t readers, writers;
+    io_threads_default(&readers, &writers, o.io_threads, 1, 1, files.size() >= 32, true, false);
+    const size_t n_threads = std::min<size_t>(files.size(), std::max<uint32_t>(writers, 1));
+    std::atomic<size_t> next{0};
+    std::atomic<int> err{0};
+    std::string err_msg; std::mutex err_mu;
+    auto work = [&] {
+        for (size_t i = next++; i < files.size() && !err.load(); i = next++) {
+            const uint32_t f = files[i];
+            const int rc = call.cancel()->load() ? fail(VMIG_ECANCELED, "before %s was finished from the base", io.m->files[f].rel.c_str())
+                                                 : io.finish_file(f);
+            int none = 0;
+            if (rc && err.compare_exchange_strong(none, rc)) { std::lock_guard<std::mutex> lk(err_mu); err_msg = last_error_cstr(); }
+        }
+    };
+    std::vector<std::thread> th;
+    for (size_t t = 1; t < n_threads; t++) th.emplace_back(work);
+    work();
+    for (auto& t : th) t.join();
+    if (err.load()) set_last_error_str(err_msg);
+    return err.load();
+}
+
+// vmig_snapshot_layer, after the data pass: every trusted layer file must still be its record, or the hashes the
+// snapshot took from the record may not be the bytes the layer holds
+int recheck_trusted(const std::string& src, const Manifest& man, const TreePlan& plan)
+{
+    for (uint32_t f = 0; f < man.files.size(); f++) {
+        const TableFile* rec = plan.files[f].layer_rec;
+        if (!rec) continue;
+        struct stat ls;
+        if (lstat(pjoin(src, man.files[f].rel).c_str(), &ls) != 0 || !is_recorded_file(ls, *rec))
+            return fail(VMIG_ESRCCHANGED, "layer file %s changed during the snapshot: it is no longer the file its layer-table record "
+                        "vouched for", man.files[f].rel.c_str());
+    }
+    return VMIG_OK;
+}
+
 // The passes of a tree call after its manifest is walked and checked: plan, (prune), data, metadata, (verify), table,
 // (move).  expect: the snapshot table's hashes in the manifest's block order (a checked restore), else empty.
 // snapshot non-null: vmig_snapshot_tree -- unchanged files and blocks come from the base (FileIO::finish_from_base).
@@ -790,10 +860,11 @@ int tree_passes(CallScope& call, const std::string& src, const std::string& dst,
     BlockTable prior;
     const bool has_prior = prior_path && *prior_path && !hash_only;
     if (has_prior && (rc = load_table(prior_path, "prior", o.block_bytes, &prior))) return rc;
-    BlockTable base; bool has_base = false;
+    const BlockTable* layer = snapshot ? snapshot->layer : nullptr;
+    BlockTable base_own; bool has_base = false;
+    const BlockTable& base = snapshot && snapshot->base_loaded ? *snapshot->base_loaded : base_own;
     if (base_path) {
-        rc = load_table(base_path, "base", o.block_bytes, &base);
-        if (rc) return rc;
+        if (!snapshot->base_loaded && (rc = load_table(base_path, "base", o.block_bytes, &base_own))) return rc;
         // a hard link cannot cross devices, and a base on another filesystem shares nothing with the snapshot
         struct stat bst, dst_st;
         has_base = stat(base_dir, &bst) == 0 && stat(dst.c_str(), &dst_st) == 0 && bst.st_dev == dst_st.st_dev;
@@ -813,16 +884,19 @@ int tree_passes(CallScope& call, const std::string& src, const std::string& dst,
     if (io.cufile) { rc = cufile_open(); if (rc) return rc; }
     rc = io.open_root(); if (rc) return rc;
     TreePlan plan;
-    rc = plan_tree(man, o.block_bytes, dst, has_prior ? &prior : nullptr, has_base ? base_dir : "", has_base ? &base : nullptr, cancel, &plan);
+    rc = plan_tree(man, o.block_bytes, dst, has_prior ? &prior : nullptr, has_base ? base_dir : "", has_base ? &base : nullptr, cancel, &plan,
+                   src, layer);
     if (rc) return rc;
     st.files_untrusted = plan.files_untrusted;
     io.init_files(man, plan);
-    std::vector<uint64_t> hashes(man.n_blocks, 0);
-    if (has_base) { io.base_root = base_dir; io.bidx.build(base, plan.base_trusted); io.hashes = hashes.data(); }
+    // a trusted layer file's hashes are its record's: the unread blocks keep them, K1 must return them for the rest
+    std::vector<uint64_t> hashes = layer ? plan.layer_hashes : std::vector<uint64_t>(man.n_blocks, 0);
+    if (has_base) { io.base_root = base_dir; io.bidx = &plan.bidx; io.hashes = hashes.data(); }
     // skip mode whenever the base can supply a block, also when no source path has a same-path record (a layer whose
     // files were all moved): without it the submitter streams every block back with its hash (DESIGN.md §3)
-    const bool skip_mode = has_prior || plan.any_base || !io.bidx.empty();
-    if (plan.any_base || !io.bidx.empty()) io.skipped.assign(man.n_blocks, 0);
+    const bool skip_mode = has_prior || plan.any_base || !plan.bidx.empty();
+    if ((plan.any_base || !plan.bidx.empty()) && io.skipped.empty()) io.skipped.assign(man.n_blocks, 0);
+    if (layer) { call.ctl->bytes_total.store(plan.bytes_read); call.ctl->blocks_total.store(plan.blocks.size()); }
     st.ns_plan += now_ns() - t0;
     const std::vector<std::string>* prune_scope = sel ? &sel->chosen_dirs : nullptr;
 
@@ -839,7 +913,12 @@ int tree_passes(CallScope& call, const std::string& src, const std::string& dst,
     if (!hash_only) { rc = make_dirs(dst, man); if (rc) return rc; }
 
     t0 = now_ns();
-    rc = run_blocks(plan.blocks, &io, skip_mode, hash_only, o, hashes.data(), &st, call.ctl, false, expect.empty() ? nullptr : expect.data());
+    BlockExpect bexp;
+    if (!expect.empty()) bexp.hashes = expect.data();
+    if (layer) { bexp.hashes = plan.layer_hashes.data(); bexp.valid = plan.expect.data(); bexp.code = VMIG_ESRCCHANGED; }
+    if (layer) rc = finish_unread(call, o, io, plan.unread);
+    if (!rc) rc = run_blocks(plan.blocks, &io, skip_mode, hash_only, o, hashes.data(), &st, call.ctl, false, bexp.hashes ? &bexp : nullptr);
+    if (!rc && layer) rc = recheck_trusted(src, man, plan);
     st.ns_data = now_ns() - t0;
     if (rc) return rc;
 
@@ -851,7 +930,12 @@ int tree_passes(CallScope& call, const std::string& src, const std::string& dst,
 
     if ((o.flags & VMIG_F_VERIFY) && !hash_only) {
         call.phase(VMIG_PHASE_VERIFY);
-        rc = verify_pass(call, o, io, hashes, &st, prune_scope);
+        std::vector<uint32_t> files = data_files(man);
+        if (layer) {            // vmig_snapshot_layer does not re-read what it linked: the base table already vouches for it
+            std::unordered_set<uint32_t> linked(io.linked_files.begin(), io.linked_files.end());
+            files.erase(std::remove_if(files.begin(), files.end(), [&](uint32_t f) { return linked.count(f) != 0; }), files.end());
+        }
+        rc = verify_pass(call, o, io, hashes, &st, prune_scope, files);
         if (rc) return rc;
     }
 
@@ -870,6 +954,7 @@ int tree_passes(CallScope& call, const std::string& src, const std::string& dst,
 
     st.files_direct = io.n_direct.load();
     st.bytes_total = man.bytes_total; st.blocks_total = man.n_blocks;
+    if (layer) { st.bytes_total = call.ctl->bytes_total.load(); st.blocks_total = call.ctl->blocks_total.load(); }
     st.files = man.files.size(); st.dirs = man.dirs.size() - (sel ? 1 : 0);
     st.ns_total = now_ns() - t_begin;
     if (stats_out) *stats_out = st;
@@ -879,6 +964,15 @@ int tree_passes(CallScope& call, const std::string& src, const std::string& dst,
         ss.files_linked = io.n_linked.load(); ss.bytes_linked = io.b_linked.load();
         ss.files_backfilled = io.n_backfilled.load(); ss.bytes_backfilled = io.b_backfilled.load();
         *snapshot->out = ss;
+    }
+    if (snapshot && snapshot->layer_out) {
+        vmig_layer_snapshot_stats ls; memset(&ls, 0, sizeof ls);
+        ls.files_linked = io.n_linked.load(); ls.bytes_linked = io.b_linked.load();
+        ls.files_backfilled = io.n_backfilled.load(); ls.bytes_backfilled = io.b_backfilled.load();
+        ls.files_base_untrusted = plan.files_base_untrusted;
+        ls.files_trusted = plan.files_trusted; ls.bytes_trusted = plan.bytes_trusted;
+        ls.files_read = plan.files_read; ls.bytes_read = plan.bytes_read;
+        *snapshot->layer_out = ls;
     }
     return VMIG_OK;
 }
@@ -1626,7 +1720,8 @@ int rollback_body(CallScope& call, const char* layer_dir, const char* layer_tabl
         if (rc) return rc;
     }
     std::vector<uint64_t> fetched(snap.n_blocks, 0);
-    rc = run_blocks(rp.fetch, &rio, false, false, o, fetched.data(), &st, call.ctl, false, snap_hashes.data());
+    BlockExpect fetch_expect; fetch_expect.hashes = snap_hashes.data();
+    rc = run_blocks(rp.fetch, &rio, false, false, o, fetched.data(), &st, call.ctl, false, &fetch_expect);
     st.ns_data += now_ns() - t0;
     if (rc) return rc;
 
@@ -1665,7 +1760,7 @@ int rollback_body(CallScope& call, const char* layer_dir, const char* layer_tabl
     vo.flags |= VMIG_F_PRUNE;                        // the verify's entry-set check is the pruning restore's
     if (o.flags & VMIG_F_VERIFY) {
         call.phase(VMIG_PHASE_VERIFY);
-        rc = verify_pass(call, vo, io, hashes, &st, nullptr);
+        rc = verify_pass(call, vo, io, hashes, &st, nullptr, data_files(snap));
         if (rc) return rc;
     }
 
@@ -1697,6 +1792,38 @@ int rollback_body(CallScope& call, const char* layer_dir, const char* layer_tabl
         *rs_out = rs;
     }
     return VMIG_OK;
+}
+
+// vmig_snapshot_layer: the refusals after the arguments, the layer's walk, then the snapshot's passes with the layer table
+int snapshot_layer_body(CallScope& call, const char* layer_dir, const char* layer_table, const char* dst_dir, const char* base_dir,
+                        const char* base_table, const char* out_table, const vmig_opts& o, vmig_stats* stats_out,
+                        vmig_layer_snapshot_stats* ls_out)
+{
+    const std::atomic<int>* cancel = call.cancel();
+    vmig_stats st; memset(&st, 0, sizeof st);
+    const uint64_t t_begin = now_ns();
+    if (cancel->load()) return fail(VMIG_ECANCELED, "the control was cancelled before the call started");
+    for (const char* d : {layer_dir, dst_dir, base_dir}) {
+        struct stat sb;
+        if (stat(d, &sb) != 0 || !S_ISDIR(sb.st_mode)) return fail(VMIG_ENOTDIR, "%s is missing or not a directory", d);
+    }
+    BlockTable base, layer;
+    int rc = load_table(base_table, "base", o.block_bytes, &base);
+    if (!rc) rc = load_table(layer_table, "layer", o.block_bytes, &layer);
+    if (rc) return rc;
+    std::vector<DeviceInfo> devs;                    // no CPU fallback: the GPU is there before anything is read
+    rc = ctx_select(o.gpu_mask, &devs);
+    if (rc) return rc;
+
+    Manifest man;
+    const uint64_t t0 = now_ns();
+    call.phase(VMIG_PHASE_WALK);
+    rc = walk_tree(layer_dir, o.block_bytes, (o.flags & VMIG_F_SKIP_HIDDEN_TOPDIRS) != 0, &man, cancel);
+    if (rc) return rc;
+    st.ns_walk = now_ns() - t0;
+    SnapshotArgs sa{base_dir, base_table, nullptr};
+    sa.base_loaded = &base; sa.layer = &layer; sa.layer_out = ls_out;
+    return tree_passes(call, layer_dir, dst_dir, man, {}, nullptr, out_table, o, st, &sa, nullptr, t_begin, stats_out);
 }
 
 }  // namespace
@@ -1834,6 +1961,40 @@ int vmig_snapshot_tree(const char* src_dir, const char* dst_dir, const char* bas
     if (snap_stats) memset(snap_stats, 0, sizeof *snap_stats);
     const SnapshotArgs sa{has_dir ? base_dir : nullptr, has_table ? base_table : nullptr, snap_stats};
     return migrate_tree_impl(src_dir, dst_dir, nullptr, out_table, opts, stats, nullptr, &sa);
+}
+int vmig_snapshot_layer(const char* layer_dir, const char* layer_table, const char* dst_dir, const char* base_dir,
+                        const char* base_table, const char* out_table, const vmig_opts* opts, vmig_stats* stats,
+                        vmig_layer_snapshot_stats* ls_stats)
+{
+    const char* const names[] = {"layer_dir", "layer_table", "dst_dir", "base_dir", "base_table", "out_table"};
+    const char* const paths[] = {layer_dir, layer_table, dst_dir, base_dir, base_table, out_table};
+    for (int i = 0; i < 6; i++)
+        if (!paths[i] || !*paths[i])
+            return fail(VMIG_EINVAL, "%s is NULL/empty: a layer snapshot takes the layer's table and a base (without them vmig_snapshot_tree is the call)", names[i]);
+    const vmig_opts o = norm_opts(opts);                     // VMIG_CUFILE=1 in the environment is refused too
+    const uint32_t allowed = VMIG_F_VERIFY | VMIG_F_PRUNE | VMIG_F_DIRECT_IO | VMIG_F_MTIME_NS | VMIG_F_NO_METADATA | VMIG_F_SKIP_HIDDEN_TOPDIRS;
+    if (o.flags & ~allowed)
+        return fail(VMIG_EINVAL, "flags 0x%x: a layer snapshot takes only VMIG_F_VERIFY, VMIG_F_PRUNE, VMIG_F_DIRECT_IO, VMIG_F_MTIME_NS, "
+                    "VMIG_F_NO_METADATA and VMIG_F_SKIP_HIDDEN_TOPDIRS", o.flags & ~allowed);
+    int rc = check_block_bytes(o);
+    if (rc) return rc;
+    std::string rd, rb, rl, x, y;
+    if (real_paths_overlap(dst_dir, base_dir, &rd, &rb))
+        return fail(VMIG_EINVAL, "dst_dir %s and base_dir %s are the same directory or one is inside the other", rd.c_str(), rb.c_str());
+    if (real_paths_overlap(dst_dir, layer_dir, &x, &rl))
+        return fail(VMIG_EINVAL, "dst_dir %s and layer_dir %s are the same directory or one is inside the other", x.c_str(), rl.c_str());
+    if (real_paths_overlap(base_dir, layer_dir, &x, &y))
+        return fail(VMIG_EINVAL, "base_dir %s and layer_dir %s are the same directory or one is inside the other", x.c_str(), y.c_str());
+    std::string ro, rt;
+    rc = real_parent_path(out_table, &ro);
+    if (!rc) rc = real_parent_path(base_table, &rt);
+    if (rc) return rc;
+    if (ro == rt || (!rb.empty() && path_inside(ro, rb)) || (!rl.empty() && path_inside(ro, rl)))
+        return fail(VMIG_EINVAL, "out_table %s is the base's table or lies inside base_dir or layer_dir: neither is ever written", out_table);
+    if (ls_stats) memset(ls_stats, 0, sizeof *ls_stats);
+    return in_call(o.ctl, [&](CallScope& call) {
+        return snapshot_layer_body(call, layer_dir, layer_table, dst_dir, base_dir, base_table, out_table, o, stats, ls_stats);
+    });
 }
 int vmig_scrub_store(uint32_t n, const char* const* snap_dirs, const char* const* snap_tables, const char* report_path,
                      int32_t* verdicts, const vmig_opts* opts, vmig_stats* stats, vmig_scrub_stats* scrub_stats)

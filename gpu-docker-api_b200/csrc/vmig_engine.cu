@@ -506,7 +506,7 @@ static void bind_thread(const DeviceInfo& d) {
 }
 
 int run_lane(Pipe* pipe, const std::vector<BlockRef>& blocks, BlockIO* io, bool has_prior, bool hash_only,
-             uint32_t n_readers, uint32_t n_writers, uint32_t max_slots, const uint64_t* expect, uint64_t* hashes_out,
+             uint32_t n_readers, uint32_t n_writers, uint32_t max_slots, const BlockExpect* expect, uint64_t* hashes_out,
              LaneStats* stats, std::atomic<int>* err, std::string* err_msg, std::mutex* err_mu, LaneProgress prog)
 {
     if (blocks.empty()) return VMIG_OK;
@@ -711,9 +711,13 @@ int run_lane(Pipe* pipe, const std::vector<BlockRef>& blocks, BlockIO* io, bool 
             if (fail_block >= 0 && (uint64_t)fail_block == r.table_idx) return fail(VMIG_EFAULT, "injected fault at block %ld (VMIG_FAIL_BLOCK)", fail_block);
             // restore: checked before the prior-table skip below, so a block the destination already has cannot hide
             // corruption; nothing of this batch has been written yet
-            if (expect && expect[r.table_idx] != h_hash[i])
-                return fail(VMIG_ECORRUPT, "%s hashes %016llx, its block table says %016llx", io->block_name(r).c_str(),
-                            (unsigned long long)h_hash[i], (unsigned long long)expect[r.table_idx]);
+            if (expect && (!expect->valid || expect->valid[r.table_idx]) && expect->hashes[r.table_idx] != h_hash[i]) {
+                if (expect->code == VMIG_ECORRUPT)
+                    return fail(VMIG_ECORRUPT, "%s hashes %016llx, its block table says %016llx", io->block_name(r).c_str(),
+                                (unsigned long long)h_hash[i], (unsigned long long)expect->hashes[r.table_idx]);
+                return fail(expect->code, "%s hashes %016llx, the table that vouched for it says %016llx: it changed since the table was written",
+                            io->block_name(r).c_str(), (unsigned long long)h_hash[i], (unsigned long long)expect->hashes[r.table_idx]);
+            }
             if (has_prior && (!h_changed[i] || (!hash_only && io->reusable(r, h_hash[i])))) { b->survive[i] = 0; skipped++; }
         }
         if (dev_dst) {

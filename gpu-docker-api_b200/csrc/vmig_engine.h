@@ -62,6 +62,16 @@ public:
     virtual std::string block_name(const BlockRef& b) { return "block at offset " + std::to_string(b.file_off); }
 };
 
+// The hashes blocks must have (nullable in run_lane): hashes[b.table_idx], for every block or, with a mask, for the blocks
+// with valid[b.table_idx] != 0.  A block that hashes otherwise fails the call with `code` before any block of its batch
+// is written: VMIG_ECORRUPT when the table speaks for the source (a checked restore), VMIG_ESRCCHANGED when it speaks for
+// a file that may have been written since (vmig_snapshot_layer).
+struct BlockExpect {
+    const uint64_t* hashes = nullptr;
+    const uint8_t* valid = nullptr;
+    int code = VMIG_ECORRUPT;
+};
+
 struct LaneStats {
     uint64_t bytes_h2d = 0, bytes_d2h = 0, bytes_written = 0, blocks_skipped = 0, kernel_launches = 0;
     double   ms_kernel = 0;
@@ -111,11 +121,11 @@ int  io_threads_default(uint32_t* readers, uint32_t* writers, uint32_t requested
 
 // Run blocks[] through one GPU.  hashes_out[b.table_idx] receives every block's hash.
 //   hash_only : no D2H of data, no writes (block_done(b,false) is still called).
-//   expect    : nullable; expect[b.table_idx] is the hash block b must have.  A block that hashes otherwise fails
-//               the call with VMIG_ECORRUPT before any block of its batch is written (skipped ones included).
+//   expect    : nullable; the hash block b must have (BlockExpect).  Checked before any block of its batch is written
+//               (skipped ones included).
 //   err       : call-wide first-error latch shared by all lanes (0 = fine); a cancel sets it from outside.
 int run_lane(Pipe* pipe, const std::vector<BlockRef>& blocks, BlockIO* io, bool has_prior, bool hash_only,
-             uint32_t readers, uint32_t writers, uint32_t max_slots, const uint64_t* expect, uint64_t* hashes_out,
+             uint32_t readers, uint32_t writers, uint32_t max_slots, const BlockExpect* expect, uint64_t* hashes_out,
              LaneStats* stats, std::atomic<int>* err, std::string* err_msg, std::mutex* err_mu, LaneProgress prog = LaneProgress());
 
 }  // namespace vmig

@@ -25,7 +25,8 @@ void interleave_blocks(const std::vector<BlockSpan>& spans, uint32_t block_bytes
 }
 
 int plan_tree(const Manifest& man, uint32_t block_bytes, const std::string& dst_root, const BlockTable* prior,
-              const std::string& base_root, const BlockTable* base, const std::atomic<int>* cancel, TreePlan* out)
+              const std::string& base_root, const BlockTable* base, const std::atomic<int>* cancel, TreePlan* out,
+              const std::string& src_root, const BlockTable* layer)
 {
     *out = TreePlan();
     out->files.resize(man.files.size());
@@ -38,6 +39,10 @@ int plan_tree(const Manifest& man, uint32_t block_bytes, const std::string& dst_
             struct stat bs;
             out->base_trusted[i] = bf.ino != 0 && lstat(pjoin(base_root, bf.rel).c_str(), &bs) == 0 && is_recorded_file(bs, bf);
         }
+        out->bidx.build(*base, out->base_trusted);
+    }
+    if (layer) {
+        out->layer_hashes.assign(man.n_blocks, 0); out->skipped.assign(man.n_blocks, 0); out->expect.assign(man.n_blocks, 0);
     }
     for (const Entry& e : man.files) if (e.hardlink_of >= 0) out->files[(size_t)e.hardlink_of].solo = false;
     std::vector<BlockSpan> spans;
@@ -62,10 +67,36 @@ int plan_tree(const Manifest& man, uint32_t block_bytes, const std::string& dst_
                 else out->files_untrusted++;
             }
         }
+        if (layer) {
+            // the same skip a snapshot makes after reading: every block whose (hash, length) a trusted base file holds,
+            // the same-path one included (base_rec is only set for a trusted base file)
+            auto it = layer->index.find(e.rel);
+            struct stat ls;
+            if (it != layer->index.end() && lstat(pjoin(src_root, e.rel).c_str(), &ls) == 0 && (uint64_t)ls.st_ino == e.ino &&
+                (uint64_t)ls.st_size == e.size && is_recorded_file(ls, layer->files[it->second])) {
+                p.layer_rec = &layer->files[it->second];
+                out->files_trusted++; out->bytes_trusted += e.size;
+                uint64_t n_read = 0, b_read = 0;
+                for (uint64_t r = 0; r < e.n_blocks; r++) {
+                    const uint64_t h = layer->hashes[p.layer_rec->first_block + r];
+                    const uint32_t len = (uint32_t)std::min<uint64_t>(block_bytes, e.size - r * block_bytes);
+                    out->layer_hashes[e.first_block + r] = h;
+                    if (out->bidx.contains(h, len)) out->skipped[e.first_block + r] = 1;
+                    else { out->expect[e.first_block + r] = 1; n_read++; b_read += len; }
+                }
+                if (!n_read) { out->unread.push_back(f); continue; }
+                out->files_read++; out->bytes_read += b_read;
+                spans.push_back({f, e.size, e.first_block, e.n_blocks});
+                continue;
+            }
+            out->files_read++; out->bytes_read += e.size;
+        }
         spans.push_back({f, e.size, e.first_block, e.n_blocks});
     }
     out->blocks.reserve(man.n_blocks);
     interleave_blocks(spans, block_bytes, &out->blocks);
+    if (layer) out->blocks.erase(std::remove_if(out->blocks.begin(), out->blocks.end(), [&](const BlockRef& b) { return out->skipped[b.table_idx] != 0; }),
+                                 out->blocks.end());
     // the same rule for a file patched in place and for a snapshot file whose base is trusted
     for (BlockRef& b : out->blocks) {
         const FilePlan& p = out->files[b.file];

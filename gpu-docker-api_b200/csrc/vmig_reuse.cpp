@@ -6,41 +6,6 @@
 
 namespace vmig {
 
-void BaseIndex::build(const BlockTable& table, const std::vector<uint8_t>& trusted)
-{
-    t = &table; trust = trusted; locs.clear(); first.clear();
-    for (uint32_t f = 0; f < table.files.size(); f++) {
-        if (!trusted[f]) continue;
-        const uint64_t nb = table.blocks_of(table.files[f]);
-        for (uint64_t r = 0; r < nb; r++) locs.push_back({hash_of(f, r), block_len(f, r), f, r});
-    }
-    std::sort(locs.begin(), locs.end(), [](const Loc& a, const Loc& b) {
-        if (a.hash != b.hash) return a.hash < b.hash;
-        if (a.len != b.len) return a.len < b.len;
-        return a.file != b.file ? a.file < b.file : a.block < b.block;
-    });
-    first.reserve(locs.size());
-    for (uint32_t i = 0; i < locs.size(); i++) first.emplace(std::make_pair(locs[i].hash, locs[i].len), i);   // keeps the first
-}
-
-const BaseIndex::Loc* BaseIndex::find(uint64_t hash, uint32_t len, size_t* n) const
-{
-    *n = 0;
-    auto it = first.find(std::make_pair(hash, len));
-    if (it == first.end()) return nullptr;
-    size_t j = it->second;
-    while (j < locs.size() && locs[j].hash == hash && locs[j].len == len) j++;
-    *n = j - it->second;
-    return &locs[it->second];
-}
-
-uint32_t BaseIndex::block_len(uint32_t file, uint64_t block) const
-{
-    const TableFile& f = t->files[file];
-    const uint64_t off = block * (uint64_t)t->block_bytes;
-    return off < f.size ? (uint32_t)std::min<uint64_t>(t->block_bytes, f.size - off) : 0;
-}
-
 int plan_backfill(const BaseIndex& idx, int same, uint64_t size, uint32_t block_bytes, const uint64_t* hashes,
                   const uint8_t* skipped, const std::string& what, std::vector<ReuseRun>* out)
 {

@@ -23,7 +23,7 @@ import threading
 
 from . import (F_PRUNE, F_VERIFY, VMIG_ECANCELED, Ctl, GetContainerMergedLayer, GetVolumeMountPoint, VmigError,
                compare_snapshot, manifest, migrate_tree, restore_paths, restore_tree, retire_versions, rollback_layer,
-               scrub_store, snapshot_tree)
+               scrub_store, snapshot_layer, snapshot_tree)
 
 log = logging.getLogger("vmig.handoff")
 _root: dict = {"cwd": None}
@@ -120,6 +120,28 @@ def SnapshotVersionIncremental(ctrVersionName: str) -> dict:
         return SnapshotDirVerified(upper, data, table)
     baseData, baseTable = snapshotPaths(base)
     return SnapshotDirIncrementalVerified(upper, data, baseData, baseTable, table)
+
+
+def SnapshotDirFromLayerVerified(src, dest, baseDir, baseTable, outTable, layerTable) -> dict:
+    """utils.SnapshotDirFromLayerVerified of the cgo shim: SnapshotDirIncrementalVerified with the layer's own block table
+    (vmig_snapshot_layer): of a file the table still vouches for only the blocks the base lacks are read.  The re-read
+    covers what was written or backfilled; linked files are the base table's own record and are left to the scrub."""
+    return snapshot_layer(src, dest, baseDir, baseTable, outTable, layerTable, flags=F_VERIFY)
+
+
+def SnapshotVersionFromLayer(ctrVersionName: str) -> dict:
+    """N1: the snapshot SnapshotVersionIncremental writes, at the cost of what the tenant changed since the hand-off.  When
+    the version's directory has no diff/ yet, its blocks.vmig is the table HandoffCopy (or RollbackInPlace) wrote for the
+    running layer: it is the layer's table, and the snapshot's table replaces it (the rule of CompareWithVersion).  Without
+    that table or an earlier snapshot to share with, it is SnapshotVersionIncremental."""
+    data, table = snapshotPaths(ctrVersionName)
+    base = baseVersion(ctrVersionName)
+    if data.exists() or not table.is_file() or base is None:
+        return SnapshotVersionIncremental(ctrVersionName)
+    upper = GetContainerMergedLayer(ctrVersionName)
+    data.mkdir(parents=True, exist_ok=True)
+    baseData, baseTable = snapshotPaths(base)
+    return SnapshotDirFromLayerVerified(upper, data, baseData, baseTable, table, table)
 
 
 def ScrubReplicaSet(rs: str) -> dict:

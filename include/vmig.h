@@ -567,6 +567,62 @@ int vmig_rollback_layer(const char* layer_dir, const char* layer_table /*nullabl
                         const vmig_opts* opts /*nullable*/, vmig_stats* stats /*nullable*/,
                         vmig_rollback_stats* rb_stats /*nullable*/);
 
+/* A version snapshot taken through the layer's own block table: what vmig_snapshot_layer took from the base and read. */
+typedef struct vmig_layer_snapshot_stats {
+    uint64_t files_linked, bytes_linked;          /* as vmig_snapshot_stats                                              */
+    uint64_t files_backfilled, bytes_backfilled;
+    uint64_t files_base_untrusted;
+    uint64_t files_trusted, bytes_trusted;        /* layer files whose hashes came from layer_table                      */
+    uint64_t files_read, bytes_read;              /* layer files with >= 1 block read; layer bytes read (H2D)            */
+    uint64_t reserved[4];
+} vmig_layer_snapshot_stats;
+
+/* Write the version snapshot of the layer layer_dir that vmig_snapshot_tree(layer_dir, dst_dir, base_dir, base_table,
+ * out_table, ...) writes, reading from the layer only the blocks the base does not already hold.  layer_table is the
+ * block table written for the layer's files (vmig_migrate_tree into the layer, or vmig_rollback_layer's out_table); the
+ * hashes of a file it still vouches for are taken from it instead of from a read.  Its cost is what changed in the
+ * layer since that table was written, where vmig_snapshot_tree reads the whole layer.
+ *   - Result: compared with the snapshot vmig_snapshot_tree writes with the same arguments and flags, these are equal:
+ *     the tree (entry kinds, contents, permission bits, owners, mtimes, symlink targets, device numbers, in-tree
+ *     hard-link grouping); which paths are hard links to which base inode; the bytes backfilled; and out_table's paths,
+ *     sizes and hashes.  Inode identities differ only where a file is a new inode.  Why: the blocks vmig_snapshot_tree
+ *     does not write are exactly those whose (XXH64, length) is among the blocks of the trusted base files (a same-path
+ *     match is one of them, since only a trusted base file is compared by path), so taking the hashes from a record
+ *     that still describes the file yields the same skipped blocks, and so the same links and backfills, without a read.
+ *   - Layer side: a layer regular file is trusted when layer_table records it with an inode and it is still the walked
+ *     regular file with that record's inode, size and ctime (the in-place diff path's rule).  Format-01 tables,
+ *     hard-linked paths (no identity) and a table written for another directory trust nothing.  Of a trusted file, a
+ *     block whose recorded (XXH64, length) a trusted base file holds is not read; every other block is read through the
+ *     block pipeline and K1's hash must equal the record's before its batch is written, else VMIG_ESRCCHANGED naming the
+ *     path and block.  A trusted file with no block to read is linked or backfilled from the base without entering the
+ *     pipeline.  An untrusted file is read and handled exactly as vmig_snapshot_tree handles it.  After the data pass
+ *     every trusted file must still be its record (lstat), else VMIG_ESRCCHANGED.  Nothing under layer_dir is written
+ *     and no layer ctime moves.  The layer must not be in use, as for vmig_rollback_layer.
+ *   - VMIG_F_VERIFY re-reads every snapshot file this call wrote from the ring or backfilled, and not the files it
+ *     linked -- the one place where this call deliberately differs from vmig_snapshot_tree.  A linked path's hashes in
+ *     out_table are the base table's record of that same inode, so the new table claims nothing the base table did not;
+ *     re-reading them would put the whole layer back into the call's cost.  Rot in shared inodes is vmig_scrub_store's
+ *     job, as it is for the snapshot blocks vmig_compare_snapshot and vmig_rollback_layer do not read.
+ *   - Refusals, in this order, each before anything is read or written: VMIG_EINVAL (any of the six paths NULL or
+ *     empty; flags other than VMIG_F_VERIFY | VMIG_F_PRUNE | VMIG_F_DIRECT_IO | VMIG_F_MTIME_NS | VMIG_F_NO_METADATA |
+ *     VMIG_F_SKIP_HIDDEN_TOPDIRS; bad block_bytes; two of dst_dir, base_dir and layer_dir the same directory or one
+ *     inside the other, by real path; out_table equal to base_table, or inside base_dir or layer_dir -- out_table ==
+ *     layer_table is allowed, it is one blocks.vmig in the hand-off layout); a control cancelled before the call:
+ *     VMIG_ECANCELED; VMIG_ENOTDIR (any of the three directories missing or not a directory); VMIG_ETABLE (either table
+ *     does not load, or its block_bytes differs from the call's); VMIG_ENOGPU (no CPU fallback, even when nothing needs
+ *     reading).
+ *   - Control: vmig_opts.ctl as for the tree calls; phases WALK, (PRUNE), DATA, META, (VERIFY), TABLE, DONE.
+ *     bytes_total / blocks_total are the layer bytes and blocks to read.  A cancel is honoured where vmig_snapshot_tree
+ *     honours it and per file of the unread trusted files.  A failed or cancelled call leaves what a failed snapshot
+ *     leaves: no out_table and no .tmp, both input tables untouched, the layer untouched.
+ *   - stats (nullable): as for vmig_snapshot_tree, with bytes_total / blocks_total as above; without VMIG_F_VERIFY,
+ *     bytes_h2d == ls_stats.bytes_read.  ls_stats (nullable): the counters above, written on success; the first five
+ *     are vmig_snapshot_stats' and equal what vmig_snapshot_tree counts. */
+int vmig_snapshot_layer(const char* layer_dir, const char* layer_table,
+                        const char* dst_dir, const char* base_dir, const char* base_table,
+                        const char* out_table, const vmig_opts* opts /*nullable*/, vmig_stats* stats /*nullable*/,
+                        vmig_layer_snapshot_stats* ls_stats /*nullable*/);
+
 /* utils.CopyDir(src, dest) (reference utils/copy.go:21-27) == vmig_migrate_tree with defaults. */
 int vmig_copy_dir(const char* src_dir, const char* dst_dir);
 
@@ -589,7 +645,7 @@ void vmig_host_free(void* p);
 
 /* ---- cancellation and progress ------------------------------------------------------------------
  * A control is a numeric id (cgo passes it in vmig_opts.ctl without any pointer rules).  It serves the entry points
- * that take vmig_opts: vmig_migrate_tree, vmig_restore_tree, vmig_restore_paths, vmig_snapshot_tree, vmig_scrub_store, vmig_retire_versions, vmig_compare_snapshot, vmig_rollback_layer and vmig_migrate_buffer (a caller that
+ * that take vmig_opts: vmig_migrate_tree, vmig_restore_tree, vmig_restore_paths, vmig_snapshot_tree, vmig_scrub_store, vmig_retire_versions, vmig_compare_snapshot, vmig_rollback_layer, vmig_snapshot_layer and vmig_migrate_buffer (a caller that
  * wants to cancel a copy or a move calls vmig_migrate_tree with the flags vmig_copy_dir / vmig_move_dir use).  One
  * control serves one call at a time: attaching it to a second concurrent call fails with VMIG_EINVAL.  The engine has
  * no deadline of its own; a deadline is the caller's timer calling vmig_ctl_cancel.

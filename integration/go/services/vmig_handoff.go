@@ -115,6 +115,30 @@ func SnapshotVersionIncremental(ctrVersionName string) error {
 		"snapshot of %s against %s failed", ctrVersionName, base)
 }
 
+// N1 -- SnapshotVersionFromLayer is the snapshot SnapshotVersionIncremental writes, at the cost of what the tenant
+// changed since the hand-off.  While the version's directory has no diff/ yet, its blocks.vmig is the table HandoffCopy
+// (or RollbackInPlace) wrote for the running layer: it is the layer's table, and the snapshot's table replaces it (the
+// rule of CompareWithVersion).  Without that table or an earlier snapshot it is SnapshotVersionIncremental.
+func SnapshotVersionFromLayer(ctrVersionName string) error {
+	data, table := snapshotPaths(ctrVersionName)
+	base, ok := baseVersion(ctrVersionName)
+	_, dataErr := os.Stat(data)
+	tableInfo, tableErr := os.Stat(table)
+	if dataErr == nil || tableErr != nil || !tableInfo.Mode().IsRegular() || !ok {
+		return SnapshotVersionIncremental(ctrVersionName)
+	}
+	upper, err := utils.GetContainerMergedLayer(ctrVersionName)
+	if err != nil {
+		return errors.WithMessagef(err, "utils.GetContainerMergedLayer failed, container: %s", ctrVersionName)
+	}
+	if err := os.MkdirAll(data, 0755); err != nil {
+		return errors.Wrapf(err, "mkdir %s", data)
+	}
+	baseData, baseTable := snapshotPaths(base)
+	return errors.WithMessagef(utils.SnapshotDirFromLayerVerified(upper, data, baseData, baseTable, table, table),
+		"snapshot of %s from its layer against %s failed", ctrVersionName, base)
+}
+
 // N1 -- ScrubReplicaSet checks every snapshot of the ReplicaSet against its block table in one pass that reads each
 // inode the versions share once.  The versions are the merges/<rs>/<rs>-<k> that hold diff/ (the rule of baseVersion;
 // a missing blocks.vmig is that version's VMIG_ETABLE).  It returns each version's verdict by name and the report,

@@ -154,6 +154,29 @@ func SnapshotDirIncrementalVerifiedContext(ctx context.Context, src, dest, baseD
 		})
 }
 
+// SnapshotDirFromLayerVerified is SnapshotDirIncrementalVerified with the layer's own block table layerTable
+// (vmig_snapshot_layer): of a file the table still vouches for, only the blocks the base does not hold are read.  The
+// snapshot, its links and its table are the ones SnapshotDirIncrementalVerified writes.  The re-read (VMIG_F_VERIFY)
+// covers what was written or backfilled, not what was linked: a linked file's hashes are the base table's own record,
+// and rot in shared inodes is ScrubSnapshots' job.  outTable may be layerTable.
+func SnapshotDirFromLayerVerified(src, dest, baseDir, baseTable, outTable, layerTable string) error {
+	return SnapshotDirFromLayerVerifiedContext(context.Background(), src, dest, baseDir, baseTable, outTable, layerTable)
+}
+
+// SnapshotDirFromLayerVerifiedContext is SnapshotDirFromLayerVerified that stops when ctx is done (see
+// CopyDirDiffContext); the layer, both tables and the base snapshot's contents are unchanged either way.
+func SnapshotDirFromLayerVerifiedContext(ctx context.Context, src, dest, baseDir, baseTable, outTable, layerTable string) error {
+	cb, ct, cl := C.CString(baseDir), C.CString(baseTable), C.CString(layerTable)
+	defer C.free(unsafe.Pointer(cb))
+	defer C.free(unsafe.Pointer(ct))
+	defer C.free(unsafe.Pointer(cl))
+	return runDiff(ctx, "vmig_snapshot_layer", src, dest, "", outTable, C.VMIG_F_VERIFY,
+		func(cs, cd, _, co *C.char, o *C.vmig_opts, st *C.vmig_stats, _ *C.vmig_snapshot_stats) C.int {
+			var ls C.vmig_layer_snapshot_stats
+			return C.vmig_snapshot_layer(cs, cl, cd, cb, ct, co, o, st, &ls)
+		})
+}
+
 // ScrubSnapshots checks every snapshot snapDirs[i] against its block table snapTables[i] in one pass that reads each
 // inode the snapshots share once (vmig_scrub_store), and writes every finding to report.  verdicts[i] is the VMIG_*
 // code a hash-only restore of that snapshot would return (VMIG_OK, VMIG_ECORRUPT, VMIG_ETABLE, VMIG_ENOTDIR); a

@@ -124,35 +124,44 @@ struct LatchLink {
 };
 
 // ---------------------------------------------------------------------------------------------
-// file-backed BlockIO
-class FileIO : public BlockIO {
-public:
-    // the call's mutable state of one file; what was decided about it before the data pass is in plan->files
-    struct FS {
-        std::atomic<int> sfd{-1}, dfd{-1};
-        std::atomic<uint32_t> reads_left{0}, blocks_left{0};
-        uint64_t id_ino = 0; int64_t id_ctime_ns = 0;   // identity of the file the table will speak for (vmig_table.h)
-        bool s_direct = false, d_direct = false;         // this file's descriptor was opened with O_DIRECT
-        std::atomic<void*> s_cfh{nullptr}, d_cfh{nullptr};   // cuFile handles of sfd / dfd (VMIG_F_CUFILE)
-        std::atomic<bool> wrote{false};                  // at least one block of the file was written in this call
-        std::atomic<bool> reused{false};                 // vmig_snapshot_tree: a changed block was found elsewhere in the base
-        int lent_mode = -1;                              // >= 0: open_dst lent the file a write bit; its mode before that
-        void identify(const struct stat& st) { id_ino = (uint64_t)st.st_ino; id_ctime_ns = ctime_ns(st); }
-    };
-    std::string src_root, dst_root;
-    int src_root_fd = -1;                // source files are opened beneath this descriptor, never by absolute path
+// The identity a block table records for a file (vmig_table.h)
+struct FileId { uint64_t ino = 0; int64_t ctime_ns = 0; };
+FileId file_id(const struct stat& st) { return {(uint64_t)st.st_ino, ctime_ns(st)}; }
+
+// A tree as a call leaves it in its destination: what the metadata, verify and table passes need of it
+struct DstTree {
     const Manifest* m = nullptr;
-    const TreePlan* plan = nullptr;
+    std::string dst_root;
     MetaPolicy pol;
     bool hash_only = false;
     bool direct = false;                 // VMIG_F_DIRECT_IO: O_DIRECT into / out of the pinned rings
     bool cufile = false;                 // VMIG_F_CUFILE: file <-> HBM slot through libcufile (GPUDirect Storage)
-    std::atomic<uint64_t> n_direct{0};   // descriptors that really were opened O_DIRECT
+    uint32_t block_bytes = 4u << 20;
+    std::vector<FileId> ids;             // per manifest file, the identity its table record carries; a writer sets only its file's
+};
+
+// file-backed BlockIO
+class FileIO : public BlockIO, public DstTree {
+public:
+    // the call's mutable state of one file; what was decided about it before the data pass is in plan->files
+    struct FS {
+        std::atomic<int> dfd{-1};
+        std::atomic<uint32_t> blocks_left{0};
+        bool d_direct = false;                           // dfd was opened with O_DIRECT
+        std::atomic<void*> s_cfh{nullptr}, d_cfh{nullptr};   // cuFile handles of the source descriptor / dfd (VMIG_F_CUFILE)
+        std::atomic<bool> wrote{false};                  // at least one block of the file was written in this call
+        std::atomic<bool> reused{false};                 // vmig_snapshot_tree: a changed block was found elsewhere in the base
+        int lent_mode = -1;                              // >= 0: open_dst lent the file a write bit; its mode before that
+    };
+    std::string src_root;
+    int src_root_fd = -1;                // source files are opened beneath this descriptor, never by absolute path
+    const TreePlan* plan = nullptr;
+    ReadFds src;                         // source descriptors, per manifest file
+    std::atomic<uint64_t> n_direct{0};   // destination descriptors that really were opened O_DIRECT (source: src.n_direct)
     uint32_t slot_align() override { return direct || cufile ? kSector : 512; }
     bool device_reads() override { return cufile; }
     bool device_writes() override { return cufile && !hash_only; }
     long corrupt_block = -1;             // VMIG_CORRUPT_BLOCK test hook: flip one bit of this block on its way to disk
-    uint32_t block_bytes = 4u << 20;
     std::string block_name(const BlockRef& b) override {
         return m->files[b.file].rel + " block " + std::to_string(b.file_off / block_bytes);
     }
@@ -163,7 +172,9 @@ public:
     void init_files(const Manifest& man, const TreePlan& p) {
         m = &man; plan = &p;
         fs.reset(new FS[man.files.size() ? man.files.size() : 1]);
-        for (const BlockRef& b : p.blocks) { fs[b.file].reads_left.fetch_add(1, std::memory_order_relaxed); fs[b.file].blocks_left.fetch_add(1, std::memory_order_relaxed); }
+        src.init(man.files.size());
+        ids.assign(man.files.size(), FileId{});
+        for (const BlockRef& b : p.blocks) { src.add_reads(b.file, 1); fs[b.file].blocks_left.fetch_add(1, std::memory_order_relaxed); }
         if (!p.skipped.empty()) {
             skipped = p.skipped;
             for (uint32_t f = 0; f < man.files.size(); f++)
@@ -283,46 +294,29 @@ public:
     // libcufile refuses descriptors whose open flags include O_NOFOLLOW / O_NONBLOCK ("unsupported file open flags"),
     // which is exactly how the safe opens below are made, and F_SETFL cannot clear O_NOFOLLOW.  The descriptor already
     // refers to the checked regular file, so it is re-opened through /proc/self/fd with plain flags and registered.
-    // *fd is replaced by the new descriptor, or closed on failure.
+    // *fd is replaced by the new descriptor; on failure *fd (the old or the new one) is left for the caller to close.
     static int attach_cufile(int* fd, int flags, const char* what, void** handle) {
         char p[64]; snprintf(p, sizeof p, "/proc/self/fd/%d", *fd);
         const int nfd = open(p, flags | O_CLOEXEC);
-        if (nfd < 0) { const int e = errno; close(*fd); return fail(VMIG_EIO, "reopen %s for cuFile: %s", what, errno_str(e).c_str()); }
+        if (nfd < 0) return fail(VMIG_EIO, "reopen %s for cuFile: %s", what, errno_str(errno).c_str());
         close(*fd); *fd = nfd;
-        const int rc = cufile_handle_open(nfd, handle);
-        if (rc) close(nfd);
-        return rc;
+        return cufile_handle_open(nfd, handle);
     }
     int open_src(uint32_t f, int* out) {
-        FS& s = fs[f];
-        int fd = s.sfd.load(std::memory_order_acquire);
-        if (fd < 0) {
-            std::lock_guard<std::mutex> lk(stripes[f & 63]);
-            fd = s.sfd.load(std::memory_order_acquire);
-            if (fd < 0) {
-                // the tenant may still be running on this layer: no symlink is followed and the root is never
-                // left (vmig_tree.h open_beneath); O_NONBLOCK so a FIFO swapped in cannot park a reader thread
-                int rc = VMIG_EIO;
-                if (direct) { rc = open_beneath(src_root_fd, m->files[f].rel, O_RDONLY | O_NONBLOCK | O_DIRECT, &fd); s.s_direct = rc == VMIG_OK; }
-                if (rc) rc = open_beneath(src_root_fd, m->files[f].rel, O_RDONLY | O_NONBLOCK, &fd);     // the filesystem may refuse O_DIRECT
-                if (rc) return rc;
-                struct stat st;
-                if (fstat(fd, &st) != 0 || !S_ISREG(st.st_mode)) {
-                    close(fd);
-                    return fail(VMIG_ESRCCHANGED, "%s is not a regular file any more", m->files[f].rel.c_str());
-                }
-                if (hash_only && st.st_nlink == 1) s.identify(st);
-                if (s.s_direct) n_direct++;
-                if (cufile) {
-                    void* h = nullptr;
-                    rc = attach_cufile(&fd, O_RDONLY | (s.s_direct ? O_DIRECT : 0), m->files[f].rel.c_str(), &h);
-                    if (rc) return rc;
-                    s.s_cfh.store(h, std::memory_order_release);
-                }
-                s.sfd.store(fd, std::memory_order_release);
-            }
-        }
-        *out = fd; return VMIG_OK;
+        const char* rel = m->files[f].rel.c_str();
+        return src.get(f, src_root_fd, m->files[f].rel, direct, [&](int* fd, const struct stat* st, bool is_direct) {
+            if (!st || !S_ISREG(st->st_mode)) return fail(VMIG_ESRCCHANGED, "%s is not a regular file any more", rel);
+            if (hash_only && st->st_nlink == 1) ids[f] = file_id(*st);
+            if (!cufile) return VMIG_OK;
+            void* h = nullptr;
+            const int rc = attach_cufile(fd, O_RDONLY | (is_direct ? O_DIRECT : 0), rel, &h);
+            if (!rc) fs[f].s_cfh.store(h, std::memory_order_release);
+            return rc;
+        }, out);
+    }
+    // one counted read of file f is done: after its last, the cuFile handle goes before the descriptor closes
+    void read_done(uint32_t f) {
+        src.read_done(f, [&](int) { void* h = fs[f].s_cfh.exchange(nullptr); if (h) cufile_handle_close(h); });
     }
     int open_dst(uint32_t f, int* out) {
         FS& s = fs[f];
@@ -332,9 +326,9 @@ public:
             fd = s.dfd.load(std::memory_order_acquire);
             if (fd < 0) {
                 const std::string p = pjoin(dst_root, m->files[f].rel);
-                const int dflag = direct && corrupt_block < 0 ? O_DIRECT : 0;
+                const bool want_direct = direct && corrupt_block < 0;
                 if (plan->files[f].prior_rec) {
-                    fd = open(p.c_str(), O_WRONLY | O_CLOEXEC | O_NOFOLLOW | dflag);
+                    fd = open_for_write(p, false, want_direct, &s.d_direct);
                     // an ordinary user's own read-only file (tar would replace it): made writable for the patch; its mode no
                     // longer matches the source's, so block_done puts the source's back whether a block was written or not
                     // (under VMIG_F_NO_METADATA the mode it had before the lend)
@@ -342,21 +336,19 @@ public:
                     if (fd < 0 && errno == EACCES && lstat(p.c_str(), &ws) == 0 && S_ISREG(ws.st_mode) &&
                         chmod(p.c_str(), (ws.st_mode & 07777) | S_IWUSR) == 0) {
                         s.lent_mode = (int)(ws.st_mode & 07777);
-                        fd = open(p.c_str(), O_WRONLY | O_CLOEXEC | O_NOFOLLOW | dflag);
+                        fd = open_for_write(p, false, want_direct, &s.d_direct);
                     }
-                    if (fd < 0 && dflag && errno == EINVAL) fd = open(p.c_str(), O_WRONLY | O_CLOEXEC | O_NOFOLLOW); else s.d_direct = dflag != 0 && fd >= 0;
                 } else {
                     int rc = clear_path(p, "a regular file");     // tar replaces what is there
                     if (rc) return rc;
-                    fd = open(p.c_str(), O_WRONLY | O_CREAT | O_EXCL | O_CLOEXEC | O_NOFOLLOW | dflag, 0600);
-                    if (fd < 0 && dflag && errno == EINVAL) fd = open(p.c_str(), O_WRONLY | O_CREAT | O_CLOEXEC | O_NOFOLLOW, 0600); else s.d_direct = dflag != 0 && fd >= 0;
+                    fd = open_for_write(p, true, want_direct, &s.d_direct);
                 }
                 if (fd < 0) return fail(VMIG_EIO, "open %s for writing: %s", p.c_str(), errno_str(errno).c_str());
                 if (s.d_direct) n_direct++;
                 if (cufile && !hash_only) {
                     void* h = nullptr;
                     const int rc = attach_cufile(&fd, O_WRONLY | (s.d_direct ? O_DIRECT : 0), p.c_str(), &h);
-                    if (rc) return rc;
+                    if (rc) { close(fd); return rc; }
                     s.d_cfh.store(h, std::memory_order_release);
                 }
                 s.dfd.store(fd, std::memory_order_release);
@@ -367,35 +359,28 @@ public:
     int read_block(const BlockRef& b, uint8_t* dst) override {
         int fd; int rc = open_src(b.file, &fd);
         if (rc) return rc;
-        FS& s = fs[b.file];
         // O_DIRECT: the device DMAs straight into the pinned ring; the file's last block is short, the read past EOF simply
         // returns fewer bytes
         size_t got;
-        rc = xfer_block(s.s_direct, true, b.len, &got, [&](size_t pos, size_t n) { return pread(fd, dst + pos, n, (off_t)(b.file_off + pos)); });
+        rc = xfer_block(src.direct(b.file), true, b.len, &got, [&](size_t pos, size_t n) { return pread(fd, dst + pos, n, (off_t)(b.file_off + pos)); });
         if (rc < 0) return fail(VMIG_EIO, "pread %s: %s", m->files[b.file].rel.c_str(), errno_str(errno).c_str());
         if (rc) return shrank(b, got);
-        if (s.reads_left.fetch_sub(1) == 1) { close_src(s, fd); }
+        read_done(b.file);
         return VMIG_OK;
     }
     int shrank(const BlockRef& b, size_t got) {
         return fail(VMIG_ESRCCHANGED, "%s shrank while being migrated (wanted %u bytes at %llu, got %zu)", m->files[b.file].rel.c_str(), b.len, (unsigned long long)b.file_off, got);
     }
-    void close_src(FS& s, int fd) {
-        void* h = s.s_cfh.exchange(nullptr);
-        if (h) cufile_handle_close(h);
-        close(fd); s.sfd.store(-1);
-    }
     // GPUDirect Storage: file -> HBM slot
     int read_block_dev(const BlockRef& b, uint8_t* d_base, size_t d_off) override {
         int fd; int rc = open_src(b.file, &fd);
         if (rc) return rc;
-        FS& s = fs[b.file];
-        void* h = s.s_cfh.load(std::memory_order_acquire);
+        void* h = fs[b.file].s_cfh.load(std::memory_order_acquire);
         size_t got;
-        rc = xfer_block(s.s_direct, false, b.len, &got, [&](size_t pos, size_t n) { return cufile_read(h, d_base, n, (off_t)(b.file_off + pos), (off_t)(d_off + pos)); });
+        rc = xfer_block(src.direct(b.file), false, b.len, &got, [&](size_t pos, size_t n) { return cufile_read(h, d_base, n, (off_t)(b.file_off + pos), (off_t)(d_off + pos)); });
         if (rc < 0) return rc;
         if (rc) return shrank(b, got);
-        if (s.reads_left.fetch_sub(1) == 1) close_src(s, fd);
+        read_done(b.file);
         return VMIG_OK;
     }
     // GPUDirect Storage: HBM slot -> file (surviving blocks only)
@@ -457,19 +442,17 @@ public:
         // O_DIRECT writes whole sectors: cut the padding of the last one.  A file patched in place that took no write has
         // none, and a truncate would move its mtime and ctime and so the identity its table records
         const bool padded = s.d_direct && (e.size & (kSector - 1)) && (s.wrote.load() || !inplace);
-        if (((inplace && fp.prior_rec->size != e.size) || padded) && ftruncate(fd, (off_t)e.size) != 0) {
-            close(fd); return fail(VMIG_EIO, "ftruncate %s: %s", p.c_str(), errno_str(errno).c_str());
-        }
+        if ((inplace && fp.prior_rec->size != e.size) || padded) rc = cut_to_size(fd, e.size, p);
         // a patched-in-place file none of whose blocks changed and whose metadata is already right is not touched at all:
         // its ctime -- by which the block table knows it -- stays what the table recorded
         const bool untouched = inplace && !s.wrote.load() && fp.prior_rec->size == e.size && file_meta_matches(fd, e, pol);
-        rc = untouched ? VMIG_OK : apply_file_meta(fd, p, e, pol);
+        if (!rc && !untouched) rc = apply_file_meta(fd, p, e, pol);
         if (!rc && pol.no_metadata && s.lent_mode >= 0 && fchmod(fd, (mode_t)s.lent_mode) != 0)
             rc = fail(VMIG_EIO, "fchmod %s (mode lent for the patch): %s", p.c_str(), errno_str(errno).c_str());
-        struct stat ids;                            // nothing touches the file after this point: its ctime is final
-        if (!rc && fstat(fd, &ids) == 0) s.identify(ids);
+        struct stat fst;                            // nothing touches the file after this point: its ctime is final
+        if (!rc && fstat(fd, &fst) == 0) ids[f] = file_id(fst);
         { void* h = s.d_cfh.exchange(nullptr); if (h) cufile_handle_close(h); }
-        if (close(fd) != 0 && !rc) rc = fail(VMIG_EIO, "close %s: %s", p.c_str(), errno_str(errno).c_str());
+        rc = close_written(fd, rc, p);
         s.dfd.store(-1);
         return rc;
     }
@@ -479,11 +462,10 @@ public:
         return VMIG_OK;
     }
     ~FileIO() {
-        for (size_t i = 0; m && i < m->files.size(); i++) {     // what a failed data pass left open
+        for (size_t i = 0; m && i < m->files.size(); i++) {     // what a failed data pass left open (src closes its own after)
             void* h = fs[i].s_cfh.exchange(nullptr); if (h) cufile_handle_close(h);
             h = fs[i].d_cfh.exchange(nullptr); if (h) cufile_handle_close(h);
-            int a = fs[i].sfd.exchange(-1); if (a >= 0) close(a);
-            int b = fs[i].dfd.exchange(-1); if (b >= 0) close(b);
+            const int d = fs[i].dfd.exchange(-1); if (d >= 0) close(d);
         }
         if (src_root_fd >= 0) close(src_root_fd);
     }
@@ -659,10 +641,10 @@ struct SnapshotArgs {
 // the tree's metadata is replayed (vmig_tree.h replay_metadata).
 // make_empty == false: the caller has already put every empty regular file in place (vmig_rollback_layer keeps one
 // that is already right).
-int meta_pass(CallScope& call, FileIO& io, const std::vector<uint64_t>& expect, std::vector<uint64_t>* hashes, vmig_stats* st,
+int meta_pass(CallScope& call, DstTree& t, const std::vector<uint64_t>& expect, std::vector<uint64_t>* hashes, vmig_stats* st,
               size_t first_dir, bool make_empty = true)
 {
-    const Manifest& man = *io.m;
+    const Manifest& man = *t.m;
     const std::atomic<int>* cancel = call.cancel();
     std::vector<uint64_t>& h = *hashes;
     if (cancel->load()) return fail(VMIG_ECANCELED, "after the data pass, before any metadata step");
@@ -679,22 +661,22 @@ int meta_pass(CallScope& call, FileIO& io, const std::vector<uint64_t>& expect, 
                                 (unsigned long long)expect[e.first_block + r]);
             }
         }
-    if (io.hash_only) return VMIG_OK;
+    if (t.hash_only) return VMIG_OK;
     size_t steps = 0;
     for (auto& e : man.files) {                    // empty regular files carry no blocks
         if (e.hardlink_of >= 0 || e.n_blocks || !make_empty) continue;
         if (steps++ % kMetaCheckEvery == 0 && cancel->load()) return fail(VMIG_ECANCELED, "before creating %s", e.rel.c_str());
-        const std::string p = pjoin(io.dst_root, e.rel);
+        const std::string p = pjoin(t.dst_root, e.rel);
         int rc = clear_path(p, "an empty regular file"); if (rc) return rc;
         int fd = open(p.c_str(), O_WRONLY | O_CREAT | O_EXCL | O_CLOEXEC | O_NOFOLLOW, 0600);
         if (fd < 0) return fail(VMIG_EIO, "create %s: %s", p.c_str(), errno_str(errno).c_str());
-        rc = apply_file_meta(fd, p, e, io.pol);
-        struct stat ids;
-        if (!rc && fstat(fd, &ids) == 0) io.fs[&e - &man.files[0]].identify(ids);
+        rc = apply_file_meta(fd, p, e, t.pol);
+        struct stat fst;
+        if (!rc && fstat(fd, &fst) == 0) t.ids[&e - &man.files[0]] = file_id(fst);
         close(fd);
         if (rc) return rc;
     }
-    return replay_metadata(io.dst_root, man, io.pol, &st->symlinks, &st->hardlinks, &st->specials, cancel, first_dir);
+    return replay_metadata(t.dst_root, man, t.pol, &st->symlinks, &st->hardlinks, &st->specials, cancel, first_dir);
 }
 
 // The manifest files that carry blocks (a hard-link group's first path): what VMIG_F_VERIFY re-reads, except
@@ -707,14 +689,14 @@ std::vector<uint32_t> data_files(const Manifest& man)
 }
 
 // VMIG_F_VERIFY: read the given destination files back through the same GPU path (hash only) and compare block tables
-int verify_pass(CallScope& call, const vmig_opts& o, const FileIO& io, const std::vector<uint64_t>& hashes, vmig_stats* st,
+int verify_pass(CallScope& call, const vmig_opts& o, const DstTree& t, const std::vector<uint64_t>& hashes, vmig_stats* st,
                 const std::vector<std::string>* prune_scope, const std::vector<uint32_t>& files)
 {
-    const Manifest& man = *io.m;
+    const Manifest& man = *t.m;
     FileIO vio;
-    vio.src_root = io.dst_root; vio.dst_root = io.dst_root; vio.pol = io.pol; vio.hash_only = true;
-    vio.direct = io.direct;          // O_DIRECT re-read: what is verified is what the device holds, not the page cache
-    vio.cufile = io.cufile;
+    vio.src_root = t.dst_root; vio.dst_root = t.dst_root; vio.pol = t.pol; vio.hash_only = true;
+    vio.direct = t.direct;           // O_DIRECT re-read: what is verified is what the device holds, not the page cache
+    vio.cufile = t.cufile;
     TreePlan blank;                  // nothing patched in place or taken from a base: every block is read back
     blank.files.resize(man.files.size());
     {
@@ -737,38 +719,39 @@ int verify_pass(CallScope& call, const vmig_opts& o, const FileIO& io, const std
                         (unsigned long long)vh[b.table_idx], (unsigned long long)hashes[b.table_idx]);
     if (o.flags & VMIG_F_PRUNE) {               // the destination's entry set must now equal the source's
         uint64_t extras = 0;
-        rc = prune_extras(io.dst_root, man, true, &extras, call.cancel(), prune_scope); if (rc) return rc;
+        rc = prune_extras(t.dst_root, man, true, &extras, call.cancel(), prune_scope); if (rc) return rc;
         if (extras) return fail(VMIG_EVERIFY, "verify: %llu destination entries are not in the source after pruning", (unsigned long long)extras);
     }
     return VMIG_OK;
 }
 
-// The table records each file as the call leaves it.  A snapshot's must let the next increment trust it: a linked
-// path's ctime moved with this call's link to the base inode, and a hard-linked file's with replay_metadata's link (both
-// after block_done recorded it), so they are read again.  Nothing later in the call touches these inodes.
-int write_table(FileIO& io, bool snapshot, const char* out_path, const std::vector<uint64_t>& hashes, const std::atomic<int>* cancel)
+// Record the identity the given files have now, each by an lstat of its destination path: for those whose ctime moved
+// after their writer recorded it.  Nothing later in the call touches these inodes.
+int record_ids(DstTree& t, const std::vector<uint32_t>& files)
 {
-    const Manifest& man = *io.m;
-    if (snapshot) {
-        std::vector<uint32_t> refresh = io.linked_files;
-        for (uint32_t f = 0; f < man.files.size(); f++) if (!io.plan->files[f].solo && man.files[f].n_blocks) refresh.push_back(f);
-        for (uint32_t f : refresh) {
-            const std::string p = pjoin(io.dst_root, man.files[f].rel);
-            struct stat ls;
-            if (lstat(p.c_str(), &ls) != 0) return fail(VMIG_EIO, "lstat %s: %s", p.c_str(), errno_str(errno).c_str());
-            io.fs[f].identify(ls);
-        }
+    for (uint32_t f : files) {
+        const std::string p = pjoin(t.dst_root, t.m->files[f].rel);
+        struct stat ls;
+        if (lstat(p.c_str(), &ls) != 0) return fail(VMIG_EIO, "lstat %s: %s", p.c_str(), errno_str(errno).c_str());
+        t.ids[f] = file_id(ls);
     }
+    return VMIG_OK;
+}
+
+// The table records each file as the call leaves it
+int write_table(const DstTree& t, const char* out_path, const std::vector<uint64_t>& hashes, const std::atomic<int>* cancel)
+{
+    const Manifest& man = *t.m;
     if (!out_path || !*out_path) return VMIG_OK;
-    BlockTable t; t.block_bytes = io.block_bytes; t.algo = 1;
-    t.files.reserve(man.files.size());
+    BlockTable tab; tab.block_bytes = t.block_bytes; tab.algo = 1;
+    tab.files.reserve(man.files.size());
     for (uint32_t f = 0; f < man.files.size(); f++) {
         const Entry& e = man.files[f];
-        const bool own = e.hardlink_of < 0 && (e.n_blocks || !io.hash_only);      // hard-linked paths are never patched in place
-        t.files.push_back({e.rel, e.size, e.first_block, own ? io.fs[f].id_ino : 0, own ? io.fs[f].id_ctime_ns : 0});
+        const bool own = e.hardlink_of < 0 && (e.n_blocks || !t.hash_only);      // hard-linked paths are never patched in place
+        tab.files.push_back({e.rel, e.size, e.first_block, own ? t.ids[f].ino : 0, own ? t.ids[f].ctime_ns : 0});
     }
-    t.hashes = hashes;
-    return table_store(out_path, t, cancel);
+    tab.hashes = hashes;
+    return table_store(out_path, tab, cancel);
 }
 
 // VMIG_F_MOVE_SRC: the old volume's data is about to be unlinked, so deferred write-back errors (ENOSPC / EIO on delayed
@@ -942,7 +925,14 @@ int tree_passes(CallScope& call, const std::string& src, const std::string& dst,
     if (!sel) {
         t0 = now_ns();
         call.phase(VMIG_PHASE_TABLE);
-        rc = write_table(io, snapshot != nullptr, out_path, hashes, cancel);
+        if (snapshot) {
+            // a snapshot's table must let the next increment trust it: a linked path's ctime moved with this call's link to
+            // the base inode, and a hard-linked file's with replay_metadata's link, both after block_done recorded it
+            std::vector<uint32_t> moved = io.linked_files;
+            for (uint32_t f = 0; f < man.files.size(); f++) if (!plan.files[f].solo && man.files[f].n_blocks) moved.push_back(f);
+            rc = record_ids(io, moved);
+        }
+        if (!rc) rc = write_table(io, out_path, hashes, cancel);
         if (rc) return rc;
         st.ns_table = now_ns() - t0;
     }
@@ -952,7 +942,7 @@ int tree_passes(CallScope& call, const std::string& src, const std::string& dst,
         if (rc) return rc;
     }
 
-    st.files_direct = io.n_direct.load();
+    st.files_direct = io.src.n_direct.load() + io.n_direct.load();
     st.bytes_total = man.bytes_total; st.blocks_total = man.n_blocks;
     if (layer) { st.bytes_total = call.ctl->bytes_total.load(); st.blocks_total = call.ctl->blocks_total.load(); }
     st.files = man.files.size(); st.dirs = man.dirs.size() - (sel ? 1 : 0);
@@ -1153,7 +1143,7 @@ int inode_pass(CallScope& call, const vmig_opts& o, const std::vector<int>& root
     const int rc = run_blocks(blocks, reader, false, true, o, hashes->data(), st, call.ctl, false);
     reader->close_all();
     st->ns_data = now_ns() - t0;
-    st->files_direct = reader->n_direct.load();
+    st->files_direct = reader->fds.n_direct.load();
     st->bytes_total = bytes; st->blocks_total = n_blocks; st->files = inodes.size();
     return rc;
 }
@@ -1519,14 +1509,14 @@ public:
     bool direct = false;                            // VMIG_F_DIRECT_IO
     uint32_t block_bytes = 4u << 20;
     const std::atomic<int>* cancel = nullptr;       // checked per copy chunk of a rebuilt file
-    std::atomic<uint64_t> n_direct{0}, b_copied{0};      // descriptors opened O_DIRECT; bytes copied from old inodes
+    ReadFds src;                                    // per plan file: its snapshot file
+    std::atomic<uint64_t> n_direct{0}, b_copied{0};      // layer descriptors opened O_DIRECT; bytes copied from old inodes
     RebuildGuard rebuild_guard;                          // the call's own unlinks of rebuilt paths
 
     void init() {
         fs.reset(new FS[plan->files.size() ? plan->files.size() : 1]);
-        for (size_t i = 0; i < plan->files.size(); i++) {
-            fs[i].reads_left.store(plan->files[i].n_fetch); fs[i].blocks_left.store(plan->files[i].n_fetch);
-        }
+        src.init(plan->files.size());
+        for (size_t i = 0; i < plan->files.size(); i++) { src.add_reads(i, plan->files[i].n_fetch); fs[i].blocks_left.store(plan->files[i].n_fetch); }
     }
     uint32_t slot_align() override { return direct ? kSector : 512; }
     std::string block_name(const BlockRef& b) override {
@@ -1541,15 +1531,13 @@ public:
         const Entry& s = snap->files[rf.snap];
         const std::string p = pjoin(layer_root, s.rel);
         FS& f = fs[i];
-        const int dflag = direct ? O_DIRECT : 0;
         int fd = -1, rc = VMIG_OK;
         if (rf.action == kRbPatch) {
-            fd = open(p.c_str(), O_WRONLY | O_CLOEXEC | O_NOFOLLOW | dflag);
-            if (fd < 0 && dflag && errno == EINVAL) fd = open(p.c_str(), O_WRONLY | O_CLOEXEC | O_NOFOLLOW); else f.d_direct = dflag && fd >= 0;
+            fd = open_for_write(p, false, direct, &f.d_direct);
             if (fd < 0) return fail(VMIG_EIO, "open %s for writing: %s", p.c_str(), errno_str(errno).c_str());
             const LayerId& id = (*ids)[(size_t)rf.layer];
             rc = rollback_check_fd(fd, id, p);
-            if (!rc && id.size != s.size && ftruncate(fd, (off_t)s.size) != 0) rc = fail(VMIG_EIO, "ftruncate %s: %s", p.c_str(), errno_str(errno).c_str());
+            if (!rc && id.size != s.size) rc = cut_to_size(fd, s.size, p);
         } else {
             int old = -1;
             if (rf.action == kRbRebuild) {
@@ -1561,11 +1549,7 @@ public:
             } else {
                 rc = clear_path(p, "a regular file");           // tar replaces what is there
             }
-            if (!rc) {
-                fd = open(p.c_str(), O_WRONLY | O_CREAT | O_EXCL | O_CLOEXEC | O_NOFOLLOW | dflag, 0600);
-                if (fd < 0 && dflag && errno == EINVAL) fd = open(p.c_str(), O_WRONLY | O_CREAT | O_EXCL | O_CLOEXEC | O_NOFOLLOW, 0600); else f.d_direct = dflag && fd >= 0;
-                if (fd < 0) rc = fail(VMIG_EIO, "create %s: %s", p.c_str(), errno_str(errno).c_str());
-            }
+            if (!rc && (fd = open_for_write(p, true, direct, &f.d_direct)) < 0) rc = fail(VMIG_EIO, "create %s: %s", p.c_str(), errno_str(errno).c_str());
             for (uint64_t k = 0; !rc && k < rf.n_runs; k++) {
                 const CopyRun& u = plan->runs[rf.first_run + k];
                 rc = copy_range_at(old, u.off, fd, u.off, u.len, f.d_direct, false, p, cancel);
@@ -1581,39 +1565,24 @@ public:
     // O_DIRECT writes whole sectors: cut the padding of the last one
     int finish(uint32_t i, int fd) {
         const Entry& s = snap->files[plan->files[i].snap];
-        int rc = VMIG_OK;
-        if (fs[i].d_direct && (s.size & (kSector - 1)) && ftruncate(fd, (off_t)s.size) != 0)
-            rc = fail(VMIG_EIO, "ftruncate %s/%s: %s", layer_root.c_str(), s.rel.c_str(), errno_str(errno).c_str());
-        if (close(fd) != 0 && !rc) rc = fail(VMIG_EIO, "close %s/%s: %s", layer_root.c_str(), s.rel.c_str(), errno_str(errno).c_str());
-        return rc;
+        const std::string p = pjoin(layer_root, s.rel);
+        return close_written(fd, fs[i].d_direct && (s.size & (kSector - 1)) ? cut_to_size(fd, s.size, p) : VMIG_OK, p);
     }
 
     int read_block(const BlockRef& b, uint8_t* dst) override {
-        FS& f = fs[b.file];
         const Entry& s = snap->files[plan->files[b.file].snap];
-        int fd = f.sfd.load(std::memory_order_acquire);
-        if (fd < 0) {
-            std::lock_guard<std::mutex> lk(stripes[b.file & 63]);
-            fd = f.sfd.load(std::memory_order_acquire);
-            if (fd < 0) {
-                int rc = VMIG_EIO;
-                if (direct) { rc = open_beneath(snap_fd, s.rel, O_RDONLY | O_NONBLOCK | O_DIRECT, &fd); f.s_direct = rc == VMIG_OK; }
-                if (rc) rc = open_beneath(snap_fd, s.rel, O_RDONLY | O_NONBLOCK, &fd);
-                if (rc) return rc;
-                struct stat st;
-                if (fstat(fd, &st) != 0 || !S_ISREG(st.st_mode) || (uint64_t)st.st_size != s.size) {
-                    close(fd);
-                    return fail(VMIG_ESRCCHANGED, "snapshot file %s is not the walked file any more", s.rel.c_str());
-                }
-                if (f.s_direct) n_direct++;
-                f.sfd.store(fd, std::memory_order_release);
-            }
-        }
+        int fd;
+        int rc = src.get(b.file, snap_fd, s.rel, direct, [&](int*, const struct stat* st, bool) {
+            if (!st || !S_ISREG(st->st_mode) || (uint64_t)st->st_size != s.size)
+                return fail(VMIG_ESRCCHANGED, "snapshot file %s is not the walked file any more", s.rel.c_str());
+            return VMIG_OK;
+        }, &fd);
+        if (rc) return rc;
         size_t got;
-        const int rc = xfer_block(f.s_direct, true, b.len, &got, [&](size_t pos, size_t n) { return pread(fd, dst + pos, n, (off_t)(b.file_off + pos)); });
+        rc = xfer_block(src.direct(b.file), true, b.len, &got, [&](size_t pos, size_t n) { return pread(fd, dst + pos, n, (off_t)(b.file_off + pos)); });
         if (rc < 0) return fail(VMIG_EIO, "pread %s: %s", s.rel.c_str(), errno_str(errno).c_str());
         if (rc) return fail(VMIG_ESRCCHANGED, "snapshot file %s shrank (wanted %u bytes at %llu, got %zu)", s.rel.c_str(), b.len, (unsigned long long)b.file_off, got);
-        if (f.reads_left.fetch_sub(1) == 1) close(f.sfd.exchange(-1));
+        src.read_done(b.file);
         return VMIG_OK;
     }
     int write_block(const BlockRef& b, const uint8_t* src) override {
@@ -1636,21 +1605,13 @@ public:
         const int fd = fs[b.file].dfd.exchange(-1);
         return fd >= 0 ? finish(b.file, fd) : VMIG_OK;
     }
-    ~RollbackIO() {
-        for (size_t i = 0; fs && i < plan->files.size(); i++) {     // what a failed pass left open
-            const int a = fs[i].sfd.exchange(-1); if (a >= 0) close(a);
-            const int d = fs[i].dfd.exchange(-1); if (d >= 0) close(d);
-        }
+    ~RollbackIO() {                                 // what a failed pass left open (src closes its own)
+        for (size_t i = 0; fs && i < plan->files.size(); i++) { const int d = fs[i].dfd.exchange(-1); if (d >= 0) close(d); }
     }
 
 private:
-    struct FS {
-        std::atomic<int> sfd{-1}, dfd{-1};
-        std::atomic<uint64_t> reads_left{0}, blocks_left{0};
-        bool s_direct = false, d_direct = false;
-    };
+    struct FS { std::atomic<int> dfd{-1}; std::atomic<uint64_t> blocks_left{0}; bool d_direct = false; };
     std::unique_ptr<FS[]> fs;
-    std::mutex stripes[64];
 };
 
 int rollback_body(CallScope& call, const char* layer_dir, const char* layer_table, const char* snap_dir, const char* snap_table,
@@ -1728,31 +1689,23 @@ int rollback_body(CallScope& call, const char* layer_dir, const char* layer_tabl
     // ---- metadata: each regular file's where it differs, then the restore's replay; the layer now holds the table's bytes
     t0 = now_ns();
     call.phase(VMIG_PHASE_META);
-    FileIO io;
-    io.src_root = snap_dir; io.dst_root = layer; io.pol = default_meta_policy(o.flags); io.block_bytes = o.block_bytes;
-    io.direct = (o.flags & VMIG_F_DIRECT_IO) != 0;
-    TreePlan whole;                                  // every block of the snapshot's files: what VMIG_F_VERIFY re-reads
-    whole.files.resize(snap.files.size());
-    {
-        std::vector<BlockSpan> spans;
-        for (uint32_t f = 0; f < snap.files.size(); f++)
-            if (snap.files[f].hardlink_of < 0 && snap.files[f].n_blocks) spans.push_back({f, snap.files[f].size, snap.files[f].first_block, snap.files[f].n_blocks});
-        interleave_blocks(spans, o.block_bytes, &whole.blocks);
-    }
-    io.init_files(snap, whole);
+    DstTree tree;
+    tree.m = &snap; tree.dst_root = layer; tree.pol = default_meta_policy(o.flags); tree.block_bytes = o.block_bytes;
+    tree.direct = (o.flags & VMIG_F_DIRECT_IO) != 0;
+    tree.ids.resize(snap.files.size());
     for (size_t i = 0; i < rp.files.size(); i++) {
         if (i % kMetaCheckEvery == 0 && cancel->load()) return fail(VMIG_ECANCELED, "before the metadata of %s", snap.files[rp.files[i].snap].rel.c_str());
         const Entry& e = snap.files[rp.files[i].snap];
         const std::string p = pjoin(layer, e.rel);
         const int fd = open(p.c_str(), O_RDONLY | O_CLOEXEC | O_NOFOLLOW | O_NONBLOCK);
         if (fd < 0 && errno != EACCES) return fail(VMIG_EIO, "open %s: %s", p.c_str(), errno_str(errno).c_str());
-        if (fd < 0) rc = apply_file_meta(-1, p, e, io.pol);          // an ordinary user's unreadable file: by path
-        else rc = file_meta_matches(fd, e, io.pol) ? VMIG_OK : apply_file_meta(fd, p, e, io.pol);     // a kept file's ctime stays
+        if (fd < 0) rc = apply_file_meta(-1, p, e, tree.pol);        // an ordinary user's unreadable file: by path
+        else rc = file_meta_matches(fd, e, tree.pol) ? VMIG_OK : apply_file_meta(fd, p, e, tree.pol);     // a kept file's ctime stays
         if (fd >= 0) close(fd);
         if (rc) return rc;
     }
     std::vector<uint64_t> hashes(snap_hashes);
-    rc = meta_pass(call, io, snap_hashes, &hashes, &st, 0, false);
+    rc = meta_pass(call, tree, snap_hashes, &hashes, &st, 0, false);
     if (rc) return rc;
     st.ns_meta = now_ns() - t0;
 
@@ -1760,25 +1713,21 @@ int rollback_body(CallScope& call, const char* layer_dir, const char* layer_tabl
     vo.flags |= VMIG_F_PRUNE;                        // the verify's entry-set check is the pruning restore's
     if (o.flags & VMIG_F_VERIFY) {
         call.phase(VMIG_PHASE_VERIFY);
-        rc = verify_pass(call, vo, io, hashes, &st, nullptr, data_files(snap));
+        rc = verify_pass(call, vo, tree, hashes, &st, nullptr, data_files(snap));
         if (rc) return rc;
     }
 
     // ---- the table: the snapshot's hashes, and each layer file's identity as the call leaves it
     t0 = now_ns();
     call.phase(VMIG_PHASE_TABLE);
-    for (uint32_t f = 0; f < snap.files.size(); f++) {
-        if (snap.files[f].hardlink_of >= 0) continue;
-        const std::string p = pjoin(layer, snap.files[f].rel);
-        struct stat ls;
-        if (lstat(p.c_str(), &ls) != 0) return fail(VMIG_EIO, "lstat %s: %s", p.c_str(), errno_str(errno).c_str());
-        io.fs[f].identify(ls);
-    }
-    rc = write_table(io, false, out_table, hashes, cancel);
+    std::vector<uint32_t> own;
+    for (uint32_t f = 0; f < snap.files.size(); f++) if (snap.files[f].hardlink_of < 0) own.push_back(f);
+    rc = record_ids(tree, own);
+    if (!rc) rc = write_table(tree, out_table, hashes, cancel);
     if (rc) return rc;
     st.ns_table = now_ns() - t0;
 
-    st.files_direct += rio.n_direct.load();
+    st.files_direct += rio.src.n_direct.load() + rio.n_direct.load();
     st.bytes_total = hashed_bytes + rp.bytes_fetched; st.blocks_total = hashed_blocks + rp.blocks_fetched;
     st.files = snap.files.size(); st.dirs = snap.dirs.size();
     st.ns_total = now_ns() - t_begin;

@@ -153,9 +153,10 @@ int scrub_report_store(const std::string& path, const std::vector<ScrubFinding>&
 // ---------------------------------------------------------------------------------------------
 void ScrubReader::init()
 {
-    n_st = inodes->size();
-    st.reset(new State[n_st ? n_st : 1]);
-    for (size_t u = 0; u < n_st; u++) st[u].reads_left.store((uint32_t)(*inodes)[u].n_blocks);
+    const size_t n = inodes->size();
+    st.reset(new State[n ? n : 1]);
+    fds.init(n);
+    for (size_t u = 0; u < n; u++) fds.add_reads(u, (*inodes)[u].n_blocks);
 }
 
 std::string ScrubReader::block_name(const BlockRef& b)
@@ -164,80 +165,43 @@ std::string ScrubReader::block_name(const BlockRef& b)
     return I.rel + " (version " + std::to_string(I.version) + ") block " + std::to_string(b.file_off / block_bytes);
 }
 
-void ScrubReader::adopt(uint32_t u, int fd, bool is_direct)
-{
-    st[u].s_direct = is_direct;
-    st[u].fd.store(fd, std::memory_order_release);
-}
-
 std::string ScrubReader::why(uint32_t u)
 {
-    std::lock_guard<std::mutex> lk(stripes[u & 63]);
+    std::lock_guard<std::mutex> lk(why_mu);
     return st[u].why;
 }
 
 void ScrubReader::mark_bad(uint32_t u, const std::string& why)
 {
-    std::lock_guard<std::mutex> lk(stripes[u & 63]);
+    std::lock_guard<std::mutex> lk(why_mu);
     if (!st[u].bad.load()) st[u].why = why;
     st[u].bad.store(true);
-}
-
-void ScrubReader::done_one(uint32_t u)
-{
-    if (st[u].reads_left.fetch_sub(1) != 1) return;
-    const int fd = st[u].fd.exchange(-1);
-    if (fd >= 0) close(fd);
-}
-
-void ScrubReader::close_all()
-{
-    for (size_t u = 0; u < n_st; u++) {
-        const int fd = st[u].fd.exchange(-1);
-        if (fd >= 0) close(fd);
-    }
 }
 
 // VMIG_OK with *out; VMIG_ESRCCHANGED: not the walked inode any more; any other code: the inode cannot be opened
 int ScrubReader::open_inode(uint32_t u, int* out)
 {
-    State& s = st[u];
-    int fd = s.fd.load(std::memory_order_acquire);
-    if (fd >= 0) { *out = fd; return VMIG_OK; }
-    std::lock_guard<std::mutex> lk(stripes[u & 63]);
-    fd = s.fd.load(std::memory_order_acquire);
-    if (fd >= 0) { *out = fd; return VMIG_OK; }
     const ScrubInode& I = (*inodes)[u];
-    const int root = root_fds[I.version];
-    int rc = VMIG_EIO;
-    if (direct) { rc = open_beneath(root, I.rel, O_RDONLY | O_NONBLOCK | O_DIRECT, &fd); s.s_direct = rc == VMIG_OK; }
-    if (rc) rc = open_beneath(root, I.rel, O_RDONLY | O_NONBLOCK, &fd);        // the filesystem may refuse O_DIRECT
-    if (rc) return rc;
-    struct stat sb;
-    if (fstat(fd, &sb) != 0) { const int e = errno; close(fd); return fail(VMIG_EIO, "fstat %s: %s", I.rel.c_str(), errno_str(e).c_str()); }
-    if (!S_ISREG(sb.st_mode) || (uint64_t)sb.st_dev != I.dev || (uint64_t)sb.st_ino != I.ino || (uint64_t)sb.st_size != I.size) {
-        close(fd);
-        return fail(VMIG_ESRCCHANGED, "%s (version %u) is no longer the %llu-byte regular file the walk saw: the store changed during the scrub",
-                    I.rel.c_str(), I.version, (unsigned long long)I.size);
-    }
-    if (s.s_direct) n_direct++;
-    s.fd.store(fd, std::memory_order_release);
-    *out = fd;
-    return VMIG_OK;
+    return fds.get(u, root_fds[I.version], I.rel, direct, [&](int*, const struct stat* sb, bool) {
+        if (!sb) return fail(VMIG_EIO, "fstat %s: %s", I.rel.c_str(), errno_str(errno).c_str());
+        if (!S_ISREG(sb->st_mode) || (uint64_t)sb->st_dev != I.dev || (uint64_t)sb->st_ino != I.ino || (uint64_t)sb->st_size != I.size)
+            return fail(VMIG_ESRCCHANGED, "%s (version %u) is no longer the %llu-byte regular file the walk saw: the store changed during the scrub",
+                        I.rel.c_str(), I.version, (unsigned long long)I.size);
+        return VMIG_OK;
+    }, out);
 }
 
 int ScrubReader::read(uint32_t u, uint64_t off, uint32_t len, uint8_t* dst)
 {
-    State& s = st[u];
-    if (s.bad.load()) { done_one(u); return VMIG_OK; }             // the rest of an unreadable inode is not read
+    if (st[u].bad.load()) { fds.read_done(u); return VMIG_OK; }    // the rest of an unreadable inode is not read
     int fd;
     int rc = open_inode(u, &fd);
     if (rc == VMIG_ESRCCHANGED) return rc;
-    if (rc) { mark_bad(u, last_error_cstr()); done_one(u); return VMIG_OK; }
+    if (rc) { mark_bad(u, last_error_cstr()); fds.read_done(u); return VMIG_OK; }
     const ScrubInode& I = (*inodes)[u];
     // O_DIRECT: buffer, offset and length in whole sectors (the pipeline's slot layout leaves the room), as FileIO reads
     size_t got, at = 0;
-    rc = xfer_block(s.s_direct, true, len, &got, [&](size_t pos, size_t n) { at = pos; return pread(fd, dst + pos, n, (off_t)(off + pos)); });
+    rc = xfer_block(fds.direct(u), true, len, &got, [&](size_t pos, size_t n) { at = pos; return pread(fd, dst + pos, n, (off_t)(off + pos)); });
     if (rc < 0) {
         char b[64]; snprintf(b, sizeof b, " at offset %llu: ", (unsigned long long)(off + at));
         mark_bad(u, "pread " + I.rel + b + errno_str(errno));
@@ -245,7 +209,7 @@ int ScrubReader::read(uint32_t u, uint64_t off, uint32_t len, uint8_t* dst)
         return fail(VMIG_ESRCCHANGED, "%s (version %u) shrank during the scrub (wanted %u bytes at %llu, got %zu)", I.rel.c_str(), I.version,
                     len, (unsigned long long)off, got);
     }
-    done_one(u);
+    fds.read_done(u);
     return VMIG_OK;
 }
 

@@ -93,34 +93,28 @@ public:
     const std::vector<ScrubInode>* inodes = nullptr;
     bool direct = false;                       // VMIG_F_DIRECT_IO
     uint32_t block_bytes = 4u << 20;           // numbers the blocks in block_name
-    std::atomic<uint64_t> n_direct{0};         // descriptors really opened O_DIRECT
+    ReadFds fds;                               // one slot per inode; fds.n_direct: descriptors really opened O_DIRECT
 
-    void init();                               // after inodes is set: one reads_left per block
+    void init();                               // after inodes is set: one counted read per block
     int read(uint32_t u, uint64_t off, uint32_t len, uint8_t* dst);
     int read_block(const BlockRef& b, uint8_t* dst) override { return read(b.file, b.file_off, b.len, dst); }
     int write_block(const BlockRef&, const uint8_t*) override { return fail(VMIG_EINVAL, "a scrub writes nothing"); }
     uint32_t slot_align() override { return direct ? kSector : 512; }
     std::string block_name(const BlockRef& b) override;   // "<rel> (version N) block K"
-    void adopt(uint32_t u, int fd, bool is_direct);   // use this open descriptor for inode u (tests/scrub_unit.cpp)
+    void adopt(uint32_t u, int fd, bool is_direct) { fds.adopt(u, fd, is_direct); }   // use this open descriptor for inode u (tests/scrub_unit.cpp)
     bool unreadable(uint32_t u) const { return st[u].bad.load(); }
     std::string why(uint32_t u);               // the error that made u unreadable
-    void close_all();
-    ~ScrubReader() { close_all(); }
+    void close_all() { fds.close_all(); }
 
 private:
     struct State {
-        std::atomic<int> fd{-1};
-        std::atomic<uint32_t> reads_left{0};
         std::atomic<bool> bad{false};
-        bool s_direct = false;
-        std::string why;                       // under the inode's stripe
+        std::string why;                       // under why_mu
     };
     std::unique_ptr<State[]> st;
-    size_t n_st = 0;
-    std::mutex stripes[64];
+    std::mutex why_mu;
     int open_inode(uint32_t u, int* out);
     void mark_bad(uint32_t u, const std::string& why);
-    void done_one(uint32_t u);
 };
 
 }  // namespace vmig

@@ -370,6 +370,27 @@ int copy_range_at(int in_fd, uint64_t off, int out_fd, uint64_t out_off, uint64_
     return rc;
 }
 
+int open_for_write(const std::string& path, bool create, bool want_direct, bool* direct)
+{
+    const int flags = O_WRONLY | O_CLOEXEC | O_NOFOLLOW | (create ? O_CREAT | O_EXCL : 0);
+    int fd = want_direct ? open(path.c_str(), flags | O_DIRECT, 0600) : -1;
+    *direct = fd >= 0;
+    // a create the filesystem refused for O_DIRECT has already made the file: take it without O_EXCL
+    if (fd < 0 && (!want_direct || errno == EINVAL)) fd = open(path.c_str(), want_direct ? flags & ~O_EXCL : flags, 0600);
+    return fd;
+}
+
+int cut_to_size(int fd, uint64_t size, const std::string& path)
+{
+    return ftruncate(fd, (off_t)size) == 0 ? VMIG_OK : fail(VMIG_EIO, "ftruncate %s: %s", path.c_str(), errno_str(errno).c_str());
+}
+
+int close_written(int fd, int rc, const std::string& path)
+{
+    if (close(fd) != 0 && !rc) rc = fail(VMIG_EIO, "close %s: %s", path.c_str(), errno_str(errno).c_str());
+    return rc;
+}
+
 int make_dirs(const std::string& dst_root, const Manifest& m)
 {
     for (size_t i = 1; i < m.dirs.size(); i++) {

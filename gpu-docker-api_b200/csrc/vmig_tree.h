@@ -7,12 +7,17 @@
 // skipped ("socket ignored"); xattrs/ACLs are dropped; existing destination entries are
 // replaced, extras are kept.
 #pragma once
+#include <fcntl.h>
 #include <stdint.h>
 #include <atomic>
+#include <memory>
+#include <mutex>
 #include <string>
 #include <vector>
 #include <sys/stat.h>
 #include <sys/types.h>
+#include <unistd.h>
+#include "../../include/vmig.h"
 
 namespace vmig {
 
@@ -121,5 +126,69 @@ int copy_range(int in_fd, int out_fd, uint64_t off, uint64_t len, bool out_direc
 // offset, or in another file, of the base snapshot).  out_direct: out_off must be a multiple of 4096.
 int copy_range_at(int in_fd, uint64_t in_off, int out_fd, uint64_t out_off, uint64_t len, bool out_direct, bool rw_only,
                   const std::string& what, const std::atomic<int>* cancel = nullptr);
+
+// The read descriptors of a file backend: one slot per file (or inode) of the call, opened by the first reader thread
+// that needs it and closed after its last counted read.  The source may be a running tenant's layer: a file is opened
+// with open_beneath (no symlink followed, the root never left), O_RDONLY | O_NONBLOCK so a FIFO swapped in cannot park
+// a reader, and O_DIRECT first when asked (the filesystem may refuse it).  Per block a reader pays one acquire load in
+// get and one fetch_sub in read_done.
+class ReadFds {
+public:
+    std::atomic<uint64_t> n_direct{0};         // descriptors published that really were opened O_DIRECT
+
+    void init(size_t n) { close_all(); n_ = n; slots_.reset(new Slot[n ? n : 1]); }     // n empty slots, no reads counted
+    void add_reads(size_t i, uint64_t n) { slots_[i].reads_left.fetch_add(n, std::memory_order_relaxed); }
+    bool direct(size_t i) const { return slots_[i].direct; }     // once get() has returned slot i's descriptor
+    // *out: slot i's descriptor, opened if it is not yet (rel beneath root_fd).  A new descriptor is first given to
+    // hook(int* fd, const struct stat* st, bool direct), st its fstat (nullptr when fstat failed; errno says why).  The
+    // hook may replace *fd; a non-zero return is the call's code, and the table closes *fd and leaves the slot empty.
+    template <class Hook> int get(size_t i, int root_fd, const std::string& rel, bool want_direct, Hook hook, int* out) {
+        Slot& s = slots_[i];
+        int fd = s.fd.load(std::memory_order_acquire);
+        if (fd < 0) {
+            std::lock_guard<std::mutex> lk(stripes_[i & 63]);
+            fd = s.fd.load(std::memory_order_acquire);
+            if (fd < 0) {
+                int rc = want_direct ? open_beneath(root_fd, rel, O_RDONLY | O_NONBLOCK | O_DIRECT, &fd) : VMIG_EIO;
+                const bool direct = rc == VMIG_OK;
+                if (rc) rc = open_beneath(root_fd, rel, O_RDONLY | O_NONBLOCK, &fd);
+                struct stat st;
+                if (!rc && (rc = hook(&fd, fstat(fd, &st) == 0 ? &st : nullptr, direct))) close(fd);
+                if (rc) return rc;
+                s.direct = direct;
+                if (direct) n_direct++;
+                s.fd.store(fd, std::memory_order_release);
+            }
+        }
+        *out = fd;
+        return VMIG_OK;
+    }
+    // One counted read of slot i is done; after the last one the descriptor is closed, before_close(fd) first
+    template <class BeforeClose> void read_done(size_t i, BeforeClose before_close) {
+        if (slots_[i].reads_left.fetch_sub(1) != 1) return;
+        const int fd = slots_[i].fd.exchange(-1);
+        if (fd >= 0) { before_close(fd); close(fd); }
+    }
+    void read_done(size_t i) { read_done(i, [](int) {}); }
+    void adopt(size_t i, int fd, bool direct) { slots_[i].direct = direct; slots_[i].fd.store(fd, std::memory_order_release); }
+    void close_all() { for (size_t i = 0; i < n_; i++) { const int fd = slots_[i].fd.exchange(-1); if (fd >= 0) close(fd); } }
+    ~ReadFds() { close_all(); }
+
+private:
+    struct Slot { std::atomic<int> fd{-1}; std::atomic<uint64_t> reads_left{0}; bool direct = false; };
+    std::unique_ptr<Slot[]> slots_;
+    size_t n_ = 0;
+    std::mutex stripes_[64];
+};
+
+// Open path for writing, never through a symlink: in place, or as a new file (O_CREAT | O_EXCL, mode 0600).
+// want_direct: O_DIRECT, and without it where the filesystem refuses it (EINVAL); *direct tells whether it held.
+// Returns the descriptor, or -1 with errno.
+int open_for_write(const std::string& path, bool create, bool want_direct, bool* direct);
+// O_DIRECT writes whole sectors, so the last one of a file written that way is padded past the file's size: cut it back
+// (ftruncate to size).  Also a patched file's resize.
+int cut_to_size(int fd, uint64_t size, const std::string& path);
+// Close a written file; its close error (deferred write-back) is the call's only when rc holds none yet.  Returns rc.
+int close_written(int fd, int rc, const std::string& path);
 
 }  // namespace vmig

@@ -81,7 +81,9 @@ def test_source_side_path_safety_unit(shm_tmp):
     descend through symlinked directories, remove_source cannot be steered out of the tree; prune_extras (VMIG_F_PRUNE)
     removes exactly the entries the manifest lacks and never follows a symlink; the walk gives the same manifest with
     one thread and with eight (hard-link pair across two sub-walks included); the metadata policy reads the umask without
-    changing it, so a call running at the same time never sees umask 0."""
+    changing it, so a call running at the same time never sees umask 0.  The file backends' descriptor table opens a slot
+    once however many threads ask, closes it after its last counted read, and handles a hook's refusal or replacement;
+    the destination open creates with O_EXCL or opens in place, never through a symlink, and reports O_DIRECT as it is."""
     import subprocess
     exe = shm_tmp / "tree_unit"
     csrc = ROOT / "gpu-docker-api_b200" / "csrc"

@@ -1,6 +1,8 @@
 // tree_unit.cpp -- CPU unit test of the source-side path safety in csrc/vmig_tree.cpp (compiled and run by
 // tests/test_host.py).  The source layer may belong to a running tenant: open_beneath() must refuse symlinks and
-// escapes, the walk must not descend through a symlinked directory, remove_source() must not leave the tree.
+// escapes, the walk must not descend through a symlinked directory, remove_source() must not leave the tree.  The file
+// backends' shared descriptor code: ReadFds opens a slot once, runs the caller's hook before publishing, and closes it
+// after its last counted read; open_for_write / cut_to_size / close_written on the destination side.
 //   g++ -std=c++17 -I gpu-docker-api_b200/csrc tests/tree_unit.cpp gpu-docker-api_b200/csrc/vmig_tree.cpp -o tree_unit
 #include "vmig_tree.h"
 #include "vmig_common.h"
@@ -11,6 +13,7 @@
 #include <atomic>
 #include <thread>
 #include <string>
+#include <vector>
 #include <sys/stat.h>
 
 namespace vmig {   // the three error-channel functions normally provided by vmig_engine.cu
@@ -22,13 +25,123 @@ long env_long(const char* name, long d) { const char* v = getenv(name); return v
 }
 using namespace vmig;
 
+#define CHECK_VOID(c) do { if (!(c)) { printf("FAIL line %d: %s\n", __LINE__, #c); exit(1); } } while (0)
 #define CHECK(c) do { if (!(c)) { printf("FAIL line %d: %s   [last error: %s]\n", __LINE__, #c, last_error_cstr()); return 1; } } while (0)
 static void put(const std::string& p, const char* s) { FILE* f = fopen(p.c_str(), "w"); fputs(s, f); fclose(f); }
 static std::string get(int fd) { char b[64] = {0}; ssize_t n = read(fd, b, 63); close(fd); return std::string(b, n > 0 ? (size_t)n : 0); }
+static bool is_open(int fd) { return fcntl(fd, F_GETFD) != -1; }
+static std::string pget(int fd) { char b[64] = {0}; ssize_t n = pread(fd, b, 63, 0); return std::string(b, n > 0 ? (size_t)n : 0); }
+
+static int read_fds(const std::string& base) {
+    const std::string root = base + "/rfd";
+    CHECK(system(("mkdir -p " + root).c_str()) == 0);
+    put(root + "/a", "alpha"); put(root + "/b", "bravo");
+    const int rfd = open(root.c_str(), O_RDONLY | O_DIRECTORY);
+    CHECK(rfd >= 0);
+    auto accept = [](int*, const struct stat* st, bool) { return st ? VMIG_OK : VMIG_EIO; };
+    {   // eight threads ask for one slot at once: one open, one hook call, one descriptor for all
+        ReadFds t; t.init(1); t.add_reads(0, 8);
+        std::atomic<int> hooks{0}, go{0};
+        std::vector<int> got(8, -1);
+        std::vector<std::thread> th;
+        for (int i = 0; i < 8; i++)
+            th.emplace_back([&, i] {
+                while (!go.load()) {}
+                t.get(0, rfd, "a", false, [&](int*, const struct stat*, bool) { hooks++; std::this_thread::sleep_for(std::chrono::milliseconds(20)); return VMIG_OK; }, &got[i]);
+            });
+        go = 1;
+        for (auto& x : th) x.join();
+        CHECK(hooks.load() == 1 && got[0] >= 0 && pget(got[0]) == "alpha");
+        for (int fd : got) CHECK(fd == got[0]);
+        CHECK(t.n_direct.load() == 0 && !t.direct(0));
+    }
+    {   // closed exactly after the last counted read, before_close first and only then
+        ReadFds t; t.init(2); t.add_reads(1, 3);
+        int fd = -1, before = 0;
+        CHECK(t.get(1, rfd, "b", false, accept, &fd) == VMIG_OK && pget(fd) == "bravo");
+        for (int r = 0; r < 3; r++) {
+            CHECK(is_open(fd));
+            t.read_done(1, [&](int c) { before++; CHECK_VOID(c == fd && is_open(c)); });
+        }
+        CHECK(before == 1 && !is_open(fd));
+    }
+    {   // a refusal closes the new descriptor and leaves the slot empty: the next get opens again
+        ReadFds t; t.init(1); t.add_reads(0, 1);
+        int seen = -1, fd = -1, hooks = 0;
+        CHECK(t.get(0, rfd, "a", false, [&](int* f, const struct stat*, bool) { hooks++; seen = *f; return VMIG_ESRCCHANGED; }, &fd) == VMIG_ESRCCHANGED);
+        CHECK(seen >= 0 && !is_open(seen) && fd == -1);
+        CHECK(t.get(0, rfd, "a", false, [&](int*, const struct stat*, bool) { hooks++; return VMIG_OK; }, &fd) == VMIG_OK);
+        CHECK(hooks == 2 && pget(fd) == "alpha");
+        t.read_done(0);
+        CHECK(!is_open(fd));
+    }
+    {   // a hook that replaces the descriptor has the replacement published, and later closed
+        ReadFds t; t.init(1); t.add_reads(0, 2);
+        int orig = -1, repl = -1, fd = -1;
+        CHECK(t.get(0, rfd, "a", false, [&](int* f, const struct stat* st, bool) {
+            struct stat bs;
+            if (!st || stat((root + "/a").c_str(), &bs) != 0 || st->st_ino != bs.st_ino) return VMIG_EIO;    // st is the opened file's
+            orig = *f; repl = open((root + "/b").c_str(), O_RDONLY); close(*f); *f = repl;
+            return VMIG_OK;
+        }, &fd) == VMIG_OK);
+        CHECK(fd == repl && fd != orig && pget(fd) == "bravo");
+        int again = -1;
+        CHECK(t.get(0, rfd, "a", false, [](int*, const struct stat*, bool) { return VMIG_EIO; }, &again) == VMIG_OK && again == repl);
+        t.read_done(0); CHECK(is_open(repl));
+        t.read_done(0); CHECK(!is_open(repl));
+    }
+    {   // close_all closes what is still open (a failed pass), and the direct flag is what the open really got
+        ReadFds t; t.init(3);
+        for (size_t i = 0; i < 3; i++) t.add_reads(i, 5);
+        int a = -1, b = -1;
+        bool hook_direct = false;
+        CHECK(t.get(0, rfd, "a", false, accept, &a) == VMIG_OK && !t.direct(0));
+        CHECK(t.get(2, rfd, "b", true, [&](int*, const struct stat*, bool d) { hook_direct = d; return VMIG_OK; }, &b) == VMIG_OK);
+        CHECK(t.direct(2) == hook_direct && t.direct(2) == ((fcntl(b, F_GETFL) & O_DIRECT) != 0) && t.n_direct.load() == (t.direct(2) ? 1u : 0u));
+        t.close_all();
+        CHECK(!is_open(a) && !is_open(b));
+    }
+    close(rfd);
+    return 0;
+}
+
+static int dst_open(const std::string& base) {
+    const std::string dir = base + "/dst";
+    CHECK(system(("mkdir -p " + dir).c_str()) == 0);
+    const std::string p = dir + "/new";
+    bool direct = true;
+    int fd = open_for_write(p, true, false, &direct);                  // create: a new 0600 file, no O_DIRECT unless asked
+    struct stat st;
+    CHECK(fd >= 0 && !direct && (fcntl(fd, F_GETFL) & O_DIRECT) == 0);
+    CHECK(fstat(fd, &st) == 0 && (st.st_mode & 07777) == 0600 && st.st_size == 0);
+    CHECK(pwrite(fd, "0123456789", 10, 0) == 10);
+    CHECK(close_written(fd, VMIG_OK, p) == VMIG_OK);
+    direct = true;
+    CHECK(open_for_write(p, true, false, &direct) == -1 && errno == EEXIST && !direct);    // O_EXCL: an existing path is not taken
+    CHECK(open_for_write(p, true, true, &direct) == -1 && errno == EEXIST && !direct);
+    fd = open_for_write(p, false, false, &direct);                      // in place: no truncate
+    CHECK(fd >= 0 && !direct && get(open(p.c_str(), O_RDONLY)) == "0123456789");
+    CHECK(pwrite(fd, "ab", 2, 0) == 2);
+    CHECK(cut_to_size(fd, 4, p) == VMIG_OK && fstat(fd, &st) == 0 && st.st_size == 4);
+    CHECK(close_written(fd, VMIG_OK, p) == VMIG_OK);
+    FILE* f = fopen(p.c_str(), "r"); char b[16] = {0}; CHECK(f && fread(b, 1, sizeof b, f) == 4); fclose(f);
+    CHECK(std::string(b) == "ab23");
+    CHECK(open_for_write(dir + "/missing", false, false, &direct) == -1 && errno == ENOENT);
+    CHECK(symlink("new", (dir + "/sl").c_str()) == 0);
+    CHECK(open_for_write(dir + "/sl", false, false, &direct) == -1);   // never through a symlink
+    fd = open_for_write(dir + "/d", true, true, &direct);               // asked: reported as the descriptor really is
+    CHECK(fd >= 0 && direct == ((fcntl(fd, F_GETFL) & O_DIRECT) != 0));
+    CHECK(close_written(fd, VMIG_OK, dir + "/d") == VMIG_OK);
+    // a failed close is the call's error only when it has none yet
+    CHECK(close_written(fd, VMIG_OK, dir + "/d") == VMIG_EIO && std::string(last_error_cstr()).find("close " + dir + "/d") == 0);
+    CHECK(close_written(fd, VMIG_ESRCCHANGED, dir + "/d") == VMIG_ESRCCHANGED);
+    return 0;
+}
 
 int main(int argc, char** argv) {
     if (argc < 2) return 2;
     const std::string base = argv[1], root = base + "/root", outside = base + "/outside";
+    if (read_fds(base) || dst_open(base)) return 1;
     CHECK(system(("mkdir -p " + root + "/a/b " + root + "/victim " + outside).c_str()) == 0);
     put(root + "/a/b/file", "inside"); put(root + "/victim/f", "inside2"); put(outside + "/f", "SECRET"); put(outside + "/secret", "SECRET");
     CHECK(symlink(outside.c_str(), (root + "/a/link").c_str()) == 0);

@@ -751,6 +751,7 @@ int write_table(const DstTree& t, const char* out_path, const std::vector<uint64
         tab.files.push_back({e.rel, e.size, e.first_block, own ? t.ids[f].ino : 0, own ? t.ids[f].ctime_ns : 0});
     }
     tab.hashes = hashes;
+    wait_past_recorded_ctimes(tab);
     return table_store(out_path, tab, cancel);
 }
 
@@ -1378,6 +1379,7 @@ int retire_body(CallScope& call, const RetireArgs& a, const vmig_opts& o, vmig_s
     t0 = now_ns();
     for (uint32_t k = 0; k < n_keep; k++) {
         if (!retire_patch(k, stale, chosen, inodes, inode_of, &tab[k])) continue;
+        wait_past_recorded_ctimes(tab[k]);
         rc = table_store(a.keep_tables[k], tab[k], cancel);
         if (rc) return rc;
         rs.tables_rewritten++;
@@ -1588,10 +1590,16 @@ public:
     int write_block(const BlockRef& b, const uint8_t* src) override {
         FS& f = fs[b.file];
         int fd = f.dfd.load(std::memory_order_acquire);
-        if (fd < 0) {                               // one writer per file (write_key): no other thread opens it
-            const int rc = prepare(b.file, &fd);
-            if (rc) return rc;
-            f.dfd.store(fd, std::memory_order_release);
+        if (fd < 0) {
+            // a file with few fetched siblings may have its blocks cut across lanes (run_blocks): the first writer to
+            // get here makes it ready, the others wait for that and write into the same descriptor
+            std::lock_guard<std::mutex> lk(f.open_mu);
+            fd = f.dfd.load(std::memory_order_acquire);
+            if (fd < 0) {
+                const int rc = prepare(b.file, &fd);
+                if (rc) return rc;
+                f.dfd.store(fd, std::memory_order_release);
+            }
         }
         size_t put;
         const int rc = xfer_block(f.d_direct, true, b.len, &put, [&](size_t pos, size_t n) { return pwrite(fd, src + pos, n, (off_t)(b.file_off + pos)); });
@@ -1610,7 +1618,7 @@ public:
     }
 
 private:
-    struct FS { std::atomic<int> dfd{-1}; std::atomic<uint64_t> blocks_left{0}; bool d_direct = false; };
+    struct FS { std::atomic<int> dfd{-1}; std::atomic<uint64_t> blocks_left{0}; bool d_direct = false; std::mutex open_mu; };
     std::unique_ptr<FS[]> fs;
 };
 

@@ -6,6 +6,8 @@
 #include <unistd.h>
 #include <sys/stat.h>
 #include <sys/syscall.h>
+#include <time.h>
+#include <algorithm>
 
 namespace vmig {
 
@@ -91,6 +93,19 @@ int table_store(const std::string& path, const BlockTable& t, const std::atomic<
     if (cancel && cancel->load()) { unlink(tmp.c_str()); return fail(VMIG_ECANCELED, "cancelled before the block table %s was renamed into place", path.c_str()); }
     if (rename(tmp.c_str(), path.c_str()) != 0) { unlink(tmp.c_str()); return fail(VMIG_EIO, "rename %s: %s", path.c_str(), errno_str(errno).c_str()); }
     return VMIG_OK;
+}
+
+void wait_past_recorded_ctimes(const BlockTable& t)
+{
+    int64_t newest = 0;
+    for (auto& f : t.files) if (f.ino) newest = std::max(newest, f.ctime_ns);
+    auto coarse = [] { struct timespec ts; clock_gettime(CLOCK_REALTIME_COARSE, &ts); return (int64_t)ts.tv_sec * 1000000000ll + ts.tv_nsec; };
+    if (!newest || newest - coarse() > 1000000000ll) return;
+    const uint64_t give_up = now_ns() + 1100000000ull;           // the realtime clock may be stepped back meanwhile
+    while (coarse() <= newest && now_ns() < give_up) {
+        const struct timespec nap = {0, 200000};
+        nanosleep(&nap, nullptr);
+    }
 }
 
 }  // namespace vmig

@@ -40,5 +40,11 @@ int table_load(const std::string& path, BlockTable* out);
 // Atomic: writes path.tmp.<pid>.<tid>, fsyncs, renames over path.  A non-zero *cancel (nullable) before the rename
 // removes the .tmp and returns VMIG_ECANCELED: no table at all.
 int table_store(const std::string& path, const BlockTable& t, const std::atomic<int>* cancel = nullptr);
+// Called before table_store by every call that records identities.  A kernel without multigrain timestamps (Linux
+// < 6.13) stamps ctime from CLOCK_REALTIME_COARSE, so a same-size write in the timer tick of a recorded ctime leaves
+// inode, size and ctime as recorded, and is_recorded_file would vouch for stale hashes.  Returns once that clock is past
+// the newest ctime t records: every later write then moves the ctime of any file it records.  At most one tick; a
+// ctime more than a second ahead of the clock (another host's, on a network filesystem) is not waited for.
+void wait_past_recorded_ctimes(const BlockTable& t);
 
 }  // namespace vmig

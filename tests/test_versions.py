@@ -34,10 +34,10 @@ def _fresh(p: Path) -> Path:
     return p
 
 
-def _frozen(orc, root: Path) -> dict:
+def _frozen(orc, root: Path, mtime_ns: bool = False) -> dict:
     """The manifest a copy of the frozen version `root` must have.  As root that is the version itself; an ordinary
     user's tar, and so the engine, applies the umask and keeps no set-id or sticky bit."""
-    man = L.tree_in_itself(orc, root)
+    man = L.tree_in_itself(orc, root, mtime_ns)
     if os.geteuid() != 0:
         um = os.umask(0)
         os.umask(um)

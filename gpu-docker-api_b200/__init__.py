@@ -49,7 +49,7 @@ EXPORTS = [
     "vmig_table_hashes", "vmig_dir_size", "vmig_to_bytes", "vmig_datagen_files", "vmig_manifest", "vmig_link_probe", "vmig_thread_plan",
     "vmig_ctl_open", "vmig_ctl_cancel", "vmig_ctl_progress", "vmig_ctl_close", "vmig_scrub_store",
     "vmig_retire_versions", "vmig_restore_paths", "vmig_compare_snapshot", "vmig_rollback_layer",
-    "vmig_snapshot_layer",
+    "vmig_snapshot_layer", "vmig_migrate_layer",
 ]
 SCRUB_KINDS = ("missing", "extra", "resized", "block", "hardlink", "unreadable", "table", "dir")
 COMPARE_KINDS = ("added", "removed", "type", "resized", "block", "target", "rdev", "hardlink", "mode", "owner", "mtime")
@@ -133,6 +133,15 @@ class LayerSnapshotStats(C.Structure):
         return {n: getattr(self, n) for n, _ in self._fields_ if n != "reserved"}
 
 
+class LayerMigrateStats(C.Structure):
+    _fields_ = [(n, C.c_uint64) for n in ("files_trusted", "bytes_trusted", "files_read", "bytes_read", "files_unread",
+                                          "files_verified", "bytes_verified", "src_recorded", "src_unrecorded")] + \
+        [("reserved", C.c_uint64 * 4)]
+
+    def as_dict(self) -> dict:
+        return {n: getattr(self, n) for n, _ in self._fields_ if n != "reserved"}
+
+
 class TableInfo(C.Structure):
     _fields_ = [("block_bytes", C.c_uint32), ("algo", C.c_uint32), ("n_files", C.c_uint64),
                 ("n_blocks", C.c_uint64), ("bytes_total", C.c_uint64)]
@@ -194,6 +203,8 @@ _sig = {
                                       C.POINTER(Stats), C.POINTER(RollbackStats)]),
     "vmig_snapshot_layer": (C.c_int, [C.c_char_p, C.c_char_p, C.c_char_p, C.c_char_p, C.c_char_p, C.c_char_p,
                                       C.POINTER(Opts), C.POINTER(Stats), C.POINTER(LayerSnapshotStats)]),
+    "vmig_migrate_layer": (C.c_int, [C.c_char_p, C.c_char_p, C.c_char_p, C.c_char_p, C.c_char_p, C.c_char_p,
+                                     C.POINTER(Opts), C.POINTER(Stats), C.POINTER(LayerMigrateStats)]),
 }
 for _n, (_r, _a) in _sig.items():
     _f = getattr(_lib, _n)
@@ -242,7 +253,7 @@ def _b(p) -> Optional[bytes]:
 
 class Ctl:
     """A call control (vmig_ctl_*): pass it as ``ctl=`` to migrate_tree, restore_tree, restore_paths, snapshot_tree,
-    scrub_store, retire_versions, compare_snapshot, rollback_layer, snapshot_layer or migrate_buffer,
+    scrub_store, retire_versions, compare_snapshot, rollback_layer, snapshot_layer, migrate_layer or migrate_buffer,
     then cancel() from any thread (the call raises VmigError(VMIG_ECANCELED)) or read progress() while it runs.  ctypes
     releases the GIL during the call.  One control serves one call at a time; a deadline is a threading.Timer."""
 
@@ -412,6 +423,23 @@ def snapshot_layer(layer, dst, base, base_table, out_table, layer_table, *, flag
     _check(_lib.vmig_snapshot_layer(_b(layer), _b(layer_table), _b(dst), _b(base), _b(base_table), _b(out_table), C.byref(o),
                                     C.byref(st), C.byref(ls)), f"vmig_snapshot_layer({layer} -> {dst}, base {base})")
     return {**st.as_dict(), **ls.as_dict()}
+
+
+def migrate_layer(src, src_table, dst, prior_table=None, out_table=None, src_out_table=None, *, flags: int = 0,
+                  gpu_mask: int = 0, block_bytes: int = 0, io_threads: int = 0, streams_per_gpu: int = 0,
+                  lanes_per_gpu: int = 0, ctl: Optional[Ctl] = None) -> dict:
+    """What migrate_tree(src, dst, prior_table, out_table) leaves, with the source's hashes taken from `src_table` (a table
+    written for the source's files, None: none) wherever it still vouches for a file: of such a file only the blocks that
+    differ from the prior record at the same index are read.  src_out_table: the same table with the source's identities,
+    for the next call's src_table; a file written while it was read is recorded without one.  F_VERIFY re-reads only the
+    destination files the call created, wrote into or resized.  Returns the migrate_tree counters plus the
+    vmig_layer_migrate_stats fields."""
+    o = Opts(gpu_mask=gpu_mask, block_bytes=block_bytes, flags=flags, io_threads=io_threads,
+             streams_per_gpu=streams_per_gpu, lanes_per_gpu=lanes_per_gpu, ctl=_ctl_id(ctl))
+    st, ms = Stats(), LayerMigrateStats()
+    _check(_lib.vmig_migrate_layer(_b(src), _b(src_table), _b(dst), _b(prior_table), _b(out_table), _b(src_out_table),
+                                   C.byref(o), C.byref(st), C.byref(ms)), f"vmig_migrate_layer({src} -> {dst})")
+    return {**st.as_dict(), **ms.as_dict()}
 
 
 def unescape_report_path(s: str) -> bytes:

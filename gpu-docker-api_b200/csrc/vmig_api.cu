@@ -152,6 +152,8 @@ public:
         std::atomic<bool> wrote{false};                  // at least one block of the file was written in this call
         std::atomic<bool> reused{false};                 // vmig_snapshot_tree: a changed block was found elsewhere in the base
         int lent_mode = -1;                              // >= 0: open_dst lent the file a write bit; its mode before that
+        struct stat src_before;                          // record_src: the source's fstat before its first read, and the
+        int64_t src_clock = 0;                           // CLOCK_REALTIME_COARSE reading taken just before that fstat
     };
     std::string src_root;
     int src_root_fd = -1;                // source files are opened beneath this descriptor, never by absolute path
@@ -178,7 +180,7 @@ public:
         if (!p.skipped.empty()) {
             skipped = p.skipped;
             for (uint32_t f = 0; f < man.files.size(); f++)
-                if (p.files[f].layer_rec)
+                if (p.files[f].layer_rec && !p.bidx.empty())       // (vmig_migrate_layer's skipped blocks are the destination's)
                     for (uint64_t r = 0; r < man.files[f].n_blocks; r++) if (p.skipped[man.files[f].first_block + r]) { fs[f].reused.store(true); break; }
         }
     }
@@ -302,11 +304,34 @@ public:
         close(*fd); *fd = nfd;
         return cufile_handle_open(nfd, handle);
     }
+    // vmig_migrate_layer's src_out_table: the identity each source file may be recorded with (live_identity_holds).  A
+    // listed file's descriptor is held open past its last read, until its last block's hash is back (note_source).
+    bool record_src = false;
+    std::vector<FileId> src_ids;                           // per manifest file; 0/0: the next call reads the file
+    void hold_sources() {
+        record_src = true;
+        src_ids.assign(m->files.size(), FileId{});
+        for (uint32_t f = 0; f < m->files.size(); f++) if (fs[f].blocks_left.load(std::memory_order_relaxed)) src.add_reads(f, 1);
+    }
+    void note_source(uint32_t f) {
+        int fd;
+        if (open_src(f, &fd) != VMIG_OK) return;           // (the held descriptor: nothing is opened here)
+        struct stat after;
+        if (plan->files[f].solo && fstat(fd, &after) == 0 && (uint64_t)after.st_size == m->files[f].size &&
+            live_identity_holds(fs[f].src_before, fs[f].src_clock, after))
+            src_ids[f] = file_id(after);
+        read_done(f);
+    }
     int open_src(uint32_t f, int* out) {
         const char* rel = m->files[f].rel.c_str();
         return src.get(f, src_root_fd, m->files[f].rel, direct, [&](int* fd, const struct stat* st, bool is_direct) {
             if (!st || !S_ISREG(st->st_mode)) return fail(VMIG_ESRCCHANGED, "%s is not a regular file any more", rel);
             if (hash_only && st->st_nlink == 1) ids[f] = file_id(*st);
+            if (record_src) {                               // the clock first: a write after the fstat stamps a later ctime
+                struct timespec ts;
+                clock_gettime(CLOCK_REALTIME_COARSE, &ts);
+                fs[f].src_clock = fstat(*fd, &fs[f].src_before) == 0 ? (int64_t)ts.tv_sec * 1000000000ll + ts.tv_nsec : 0;
+            }
             if (!cufile) return VMIG_OK;
             void* h = nullptr;
             const int rc = attach_cufile(fd, O_RDONLY | (is_direct ? O_DIRECT : 0), rel, &h);
@@ -422,9 +447,10 @@ public:
         if (!written && fp.base_rec) skipped[b.table_idx] = 1;          // (a reused block was marked by reusable())
         if (s.blocks_left.fetch_sub(1) != 1) return VMIG_OK;
         if (hash_only) return VMIG_OK;
+        if (record_src) note_source(b.file);
         return finish_file(b.file);
     }
-    // The file's last block passed (or none is read: vmig_snapshot_layer's unread files): link or backfill from the base,
+    // The file's last block passed (or none is read: the layer calls' unread files): link or backfill from the base,
     // else cut and apply metadata, and take the identity the table records
     int finish_file(uint32_t f) {
         FS& s = fs[f];
@@ -637,6 +663,14 @@ struct SnapshotArgs {
     vmig_layer_snapshot_stats* layer_out = nullptr;    // nullable
 };
 
+// vmig_migrate_layer: the loaded tables, and what the call writes besides the tree call's results
+struct LayerMigrateArgs {
+    const BlockTable* src_table;       // an empty table when none is given: nothing is trusted
+    const BlockTable* prior;           // nullable
+    const char* src_out;               // nullable
+    vmig_layer_migrate_stats* out;     // nullable
+};
+
 // After the data pass: hard-linked paths take their primary's hashes, empty regular files are created, then the rest of
 // the tree's metadata is replayed (vmig_tree.h replay_metadata).
 // make_empty == false: the caller has already put every empty regular file in place (vmig_rollback_layer keeps one
@@ -782,8 +816,9 @@ bool path_inside(const std::string& a, const std::string& root)
     return a == root || (a.size() > root.size() && a.compare(0, root.size(), root) == 0 && (root == "/" || a[root.size()] == '/'));
 }
 
-// vmig_snapshot_layer: the trusted layer files none of whose blocks is read are linked or backfilled from the base, then
-// finished, as their last block's writer finishes a file that was read; spread over as many threads as a lane has writers
+// The layer calls: the trusted source files none of whose blocks is read are linked or backfilled from the base
+// (vmig_snapshot_layer) or left as the prior record they are (vmig_migrate_layer), then finished, as their last block's
+// writer finishes a file that was read; spread over as many threads as a lane has writers
 int finish_unread(CallScope& call, const vmig_opts& o, FileIO& io, const std::vector<uint32_t>& files)
 {
     if (files.empty()) return VMIG_OK;
@@ -796,7 +831,7 @@ int finish_unread(CallScope& call, const vmig_opts& o, FileIO& io, const std::ve
     auto work = [&] {
         for (size_t i = next++; i < files.size() && !err.load(); i = next++) {
             const uint32_t f = files[i];
-            const int rc = call.cancel()->load() ? fail(VMIG_ECANCELED, "before %s was finished from the base", io.m->files[f].rel.c_str())
+            const int rc = call.cancel()->load() ? fail(VMIG_ECANCELED, "before the unread file %s was finished", io.m->files[f].rel.c_str())
                                                  : io.finish_file(f);
             int none = 0;
             if (rc && err.compare_exchange_strong(none, rc)) { std::lock_guard<std::mutex> lk(err_mu); err_msg = last_error_cstr(); }
@@ -810,8 +845,8 @@ int finish_unread(CallScope& call, const vmig_opts& o, FileIO& io, const std::ve
     return err.load();
 }
 
-// vmig_snapshot_layer, after the data pass: every trusted layer file must still be its record, or the hashes the
-// snapshot took from the record may not be the bytes the layer holds
+// The layer calls, after the data pass: every trusted source file must still be its record, or the hashes the call took
+// from the record may not be the bytes the source holds
 int recheck_trusted(const std::string& src, const Manifest& man, const TreePlan& plan)
 {
     for (uint32_t f = 0; f < man.files.size(); f++) {
@@ -819,7 +854,7 @@ int recheck_trusted(const std::string& src, const Manifest& man, const TreePlan&
         if (!rec) continue;
         struct stat ls;
         if (lstat(pjoin(src, man.files[f].rel).c_str(), &ls) != 0 || !is_recorded_file(ls, *rec))
-            return fail(VMIG_ESRCCHANGED, "layer file %s changed during the snapshot: it is no longer the file its layer-table record "
+            return fail(VMIG_ESRCCHANGED, "source file %s changed during the call: it is no longer the file its table record "
                         "vouched for", man.files[f].rel.c_str());
     }
     return VMIG_OK;
@@ -831,9 +866,11 @@ int recheck_trusted(const std::string& src, const Manifest& man, const TreePlan&
 // sel non-null: vmig_restore_paths -- the parent chains are made real directories before the plan looks at the
 // destination, the prune and its verify stay beneath the chosen directories, the destination root's metadata ("."
 // here stands for it) is not replayed, and no table is written.
+// lm non-null: vmig_migrate_layer -- a migration with the source's own table (the layer branch of plan_tree against the
+// prior), src_out_table, and a verify of only what the call wrote.
 int tree_passes(CallScope& call, const std::string& src, const std::string& dst, Manifest& man, const std::vector<uint64_t>& expect,
                 const char* prior_path, const char* out_path, const vmig_opts& o, vmig_stats& st, const SnapshotArgs* snapshot,
-                Selection* sel, uint64_t t_begin, vmig_stats* stats_out)
+                Selection* sel, uint64_t t_begin, vmig_stats* stats_out, const LayerMigrateArgs* lm = nullptr)
 {
     const char* base_dir = snapshot ? snapshot->base_dir : nullptr;
     const char* base_path = snapshot ? snapshot->base_table : nullptr;
@@ -841,10 +878,11 @@ int tree_passes(CallScope& call, const std::string& src, const std::string& dst,
     const bool hash_only = (o.flags & VMIG_F_HASH_ONLY) != 0;
     int rc;
     uint64_t t0 = now_ns();
-    BlockTable prior;
+    BlockTable prior_own;
     const bool has_prior = prior_path && *prior_path && !hash_only;
-    if (has_prior && (rc = load_table(prior_path, "prior", o.block_bytes, &prior))) return rc;
-    const BlockTable* layer = snapshot ? snapshot->layer : nullptr;
+    const BlockTable& prior = lm && lm->prior ? *lm->prior : prior_own;
+    if (has_prior && !(lm && lm->prior) && (rc = load_table(prior_path, "prior", o.block_bytes, &prior_own))) return rc;
+    const BlockTable* layer = snapshot ? snapshot->layer : lm ? lm->src_table : nullptr;
     BlockTable base_own; bool has_base = false;
     const BlockTable& base = snapshot && snapshot->base_loaded ? *snapshot->base_loaded : base_own;
     if (base_path) {
@@ -873,6 +911,12 @@ int tree_passes(CallScope& call, const std::string& src, const std::string& dst,
     if (rc) return rc;
     st.files_untrusted = plan.files_untrusted;
     io.init_files(man, plan);
+    const bool src_out = lm && lm->src_out && *lm->src_out;
+    if (src_out) {
+        io.hold_sources();
+        for (uint32_t f : plan.unread)                     // a trusted unread file keeps its record's identity
+            if (plan.files[f].solo) io.src_ids[f] = {plan.files[f].layer_rec->ino, plan.files[f].layer_rec->ctime_ns};
+    }
     // a trusted layer file's hashes are its record's: the unread blocks keep them, K1 must return them for the rest
     std::vector<uint64_t> hashes = layer ? plan.layer_hashes : std::vector<uint64_t>(man.n_blocks, 0);
     if (has_base) { io.base_root = base_dir; io.bidx = &plan.bidx; io.hashes = hashes.data(); }
@@ -912,13 +956,21 @@ int tree_passes(CallScope& call, const std::string& src, const std::string& dst,
     if (rc) return rc;
     st.ns_meta = now_ns() - t0;
 
+    uint64_t n_verified = 0, b_verified = 0;
     if ((o.flags & VMIG_F_VERIFY) && !hash_only) {
         call.phase(VMIG_PHASE_VERIFY);
         std::vector<uint32_t> files = data_files(man);
-        if (layer) {            // vmig_snapshot_layer does not re-read what it linked: the base table already vouches for it
+        if (snapshot && layer) {    // vmig_snapshot_layer does not re-read what it linked: the base table already vouches for it
             std::unordered_set<uint32_t> linked(io.linked_files.begin(), io.linked_files.end());
             files.erase(std::remove_if(files.begin(), files.end(), [&](uint32_t f) { return linked.count(f) != 0; }), files.end());
         }
+        if (lm) {                   // vmig_migrate_layer does not re-read what it left alone: it still is its prior record
+            files.erase(std::remove_if(files.begin(), files.end(), [&](uint32_t f) {
+                const TableFile* pr = plan.files[f].prior_rec;
+                return pr && !io.fs[f].wrote.load() && pr->size == man.files[f].size;
+            }), files.end());
+        }
+        for (uint32_t f : files) { n_verified++; b_verified += man.files[f].size; }
         rc = verify_pass(call, o, io, hashes, &st, prune_scope, files);
         if (rc) return rc;
     }
@@ -933,7 +985,16 @@ int tree_passes(CallScope& call, const std::string& src, const std::string& dst,
             for (uint32_t f = 0; f < man.files.size(); f++) if (!plan.files[f].solo && man.files[f].n_blocks) moved.push_back(f);
             rc = record_ids(io, moved);
         }
-        if (!rc) rc = write_table(io, out_path, hashes, cancel);
+        if (!rc && src_out) {
+            // the source's table first, under the cancel; once it is in place the call commits, and a failure to store
+            // out_table takes it away again
+            DstTree sv = static_cast<const DstTree&>(io);
+            sv.ids = io.src_ids;
+            rc = write_table(sv, lm->src_out, hashes, cancel);
+            if (!rc && (rc = write_table(io, out_path, hashes, nullptr))) unlink(lm->src_out);
+        } else if (!rc) {
+            rc = write_table(io, out_path, hashes, cancel);
+        }
         if (rc) return rc;
         st.ns_table = now_ns() - t0;
     }
@@ -964,6 +1025,16 @@ int tree_passes(CallScope& call, const std::string& src, const std::string& dst,
         ls.files_trusted = plan.files_trusted; ls.bytes_trusted = plan.bytes_trusted;
         ls.files_read = plan.files_read; ls.bytes_read = plan.bytes_read;
         *snapshot->layer_out = ls;
+    }
+    if (lm && lm->out) {
+        vmig_layer_migrate_stats ms; memset(&ms, 0, sizeof ms);
+        ms.files_trusted = plan.files_trusted; ms.bytes_trusted = plan.bytes_trusted;
+        ms.files_read = plan.files_read; ms.bytes_read = plan.bytes_read;
+        ms.files_unread = plan.unread.size();
+        ms.files_verified = n_verified; ms.bytes_verified = b_verified;
+        if (src_out)
+            for (const FileId& id : io.src_ids) (id.ino ? ms.src_recorded : ms.src_unrecorded)++;
+        *lm->out = ms;
     }
     return VMIG_OK;
 }
@@ -1783,6 +1854,41 @@ int snapshot_layer_body(CallScope& call, const char* layer_dir, const char* laye
     return tree_passes(call, layer_dir, dst_dir, man, {}, nullptr, out_table, o, st, &sa, nullptr, t_begin, stats_out);
 }
 
+// vmig_migrate_layer: the refusals after the arguments, the source's walk, then the migration's passes with the
+// source's table
+int migrate_layer_body(CallScope& call, const char* src_dir, const char* src_table, const char* dst_dir, const char* prior_table,
+                       const char* out_table, const char* src_out_table, const vmig_opts& o, vmig_stats* stats_out,
+                       vmig_layer_migrate_stats* lm_out)
+{
+    const std::atomic<int>* cancel = call.cancel();
+    vmig_stats st; memset(&st, 0, sizeof st);
+    const uint64_t t_begin = now_ns();
+    if (cancel->load()) return fail(VMIG_ECANCELED, "the control was cancelled before the call started");
+    for (const char* d : {src_dir, dst_dir}) {
+        struct stat sb;
+        if (stat(d, &sb) != 0 || !S_ISDIR(sb.st_mode)) return fail(VMIG_ENOTDIR, "%s is missing or not a directory", d);
+    }
+    BlockTable src_tab, prior;
+    src_tab.block_bytes = o.block_bytes;
+    const bool has_prior = prior_table && *prior_table;
+    int rc = src_table && *src_table ? load_table(src_table, "source", o.block_bytes, &src_tab) : VMIG_OK;
+    if (!rc && has_prior) rc = load_table(prior_table, "prior", o.block_bytes, &prior);
+    if (rc) return rc;
+    std::vector<DeviceInfo> devs;                    // no CPU fallback: the GPU is there before anything is read
+    rc = ctx_select(o.gpu_mask, &devs);
+    if (rc) return rc;
+
+    Manifest man;
+    const uint64_t t0 = now_ns();
+    call.phase(VMIG_PHASE_WALK);
+    rc = walk_tree(src_dir, o.block_bytes, (o.flags & VMIG_F_SKIP_HIDDEN_TOPDIRS) != 0, &man, cancel);
+    if (rc) return rc;
+    st.ns_walk = now_ns() - t0;
+    const LayerMigrateArgs lma{&src_tab, has_prior ? &prior : nullptr, src_out_table, lm_out};
+    return tree_passes(call, src_dir, dst_dir, man, {}, has_prior ? prior_table : nullptr, out_table, o, st, nullptr, nullptr,
+                       t_begin, stats_out, &lma);
+}
+
 }  // namespace
 
 // =============================================================================================
@@ -1951,6 +2057,37 @@ int vmig_snapshot_layer(const char* layer_dir, const char* layer_table, const ch
     if (ls_stats) memset(ls_stats, 0, sizeof *ls_stats);
     return in_call(o.ctl, [&](CallScope& call) {
         return snapshot_layer_body(call, layer_dir, layer_table, dst_dir, base_dir, base_table, out_table, o, stats, ls_stats);
+    });
+}
+int vmig_migrate_layer(const char* src_dir, const char* src_table, const char* dst_dir, const char* prior_table,
+                       const char* out_table, const char* src_out_table, const vmig_opts* opts, vmig_stats* stats,
+                       vmig_layer_migrate_stats* lm_stats)
+{
+    if (!src_dir || !*src_dir) return fail(VMIG_EINVAL, "src_dir is NULL/empty");
+    if (!dst_dir || !*dst_dir) return fail(VMIG_EINVAL, "dst_dir is NULL/empty");
+    const vmig_opts o = norm_opts(opts);                     // VMIG_CUFILE=1 in the environment is refused too
+    const uint32_t allowed = VMIG_F_VERIFY | VMIG_F_PRUNE | VMIG_F_DIRECT_IO | VMIG_F_MTIME_NS | VMIG_F_NO_METADATA | VMIG_F_SKIP_HIDDEN_TOPDIRS;
+    if (o.flags & ~allowed)
+        return fail(VMIG_EINVAL, "flags 0x%x: a layer migration takes only VMIG_F_VERIFY, VMIG_F_PRUNE, VMIG_F_DIRECT_IO, VMIG_F_MTIME_NS, "
+                    "VMIG_F_NO_METADATA and VMIG_F_SKIP_HIDDEN_TOPDIRS", o.flags & ~allowed);
+    int rc = check_block_bytes(o);
+    if (rc) return rc;
+    std::string rs, rd;
+    if (real_paths_overlap(src_dir, dst_dir, &rs, &rd))
+        return fail(VMIG_EINVAL, "src_dir %s and dst_dir %s are the same directory or one is inside the other", rs.c_str(), rd.c_str());
+    const bool has_out = out_table && *out_table, has_src_out = src_out_table && *src_out_table;
+    std::string ro, rso;
+    if (has_out && (rc = real_parent_path(out_table, &ro))) return rc;
+    if (has_src_out && (rc = real_parent_path(src_out_table, &rso))) return rc;
+    if (has_out && has_src_out && ro == rso)
+        return fail(VMIG_EINVAL, "out_table and src_out_table are the same file %s: one table records the destination, the other the source", ro.c_str());
+    if (!rs.empty() && ((has_out && path_inside(ro, rs)) || (has_src_out && path_inside(rso, rs))))
+        return fail(VMIG_EINVAL, "out_table or src_out_table lies inside src_dir %s: the source is never written", rs.c_str());
+    if (has_src_out && !rd.empty() && path_inside(rso, rd))
+        return fail(VMIG_EINVAL, "src_out_table %s lies inside dst_dir %s: it would be part of the tree it describes the source of", rso.c_str(), rd.c_str());
+    if (lm_stats) memset(lm_stats, 0, sizeof *lm_stats);
+    return in_call(o.ctl, [&](CallScope& call) {
+        return migrate_layer_body(call, src_dir, src_table, dst_dir, prior_table, out_table, src_out_table, o, stats, lm_stats);
     });
 }
 int vmig_scrub_store(uint32_t n, const char* const* snap_dirs, const char* const* snap_tables, const char* report_path,

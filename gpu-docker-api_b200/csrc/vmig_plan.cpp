@@ -68,8 +68,9 @@ int plan_tree(const Manifest& man, uint32_t block_bytes, const std::string& dst_
             }
         }
         if (layer) {
-            // the same skip a snapshot makes after reading: every block whose (hash, length) a trusted base file holds,
-            // the same-path one included (base_rec is only set for a trusted base file)
+            // the same skip the tree call makes after reading: a snapshot's, every block whose (hash, length) a trusted
+            // base file holds, the same-path one included (base_rec is only set for a trusted base file); a migration's
+            // (vmig_migrate_layer, no base), every block whose (hash, length) is the prior record's at the same index
             auto it = layer->index.find(e.rel);
             struct stat ls;
             if (it != layer->index.end() && lstat(pjoin(src_root, e.rel).c_str(), &ls) == 0 && (uint64_t)ls.st_ino == e.ino &&
@@ -81,7 +82,11 @@ int plan_tree(const Manifest& man, uint32_t block_bytes, const std::string& dst_
                     const uint64_t h = layer->hashes[p.layer_rec->first_block + r];
                     const uint32_t len = (uint32_t)std::min<uint64_t>(block_bytes, e.size - r * block_bytes);
                     out->layer_hashes[e.first_block + r] = h;
-                    if (out->bidx.contains(h, len)) out->skipped[e.first_block + r] = 1;
+                    const uint64_t off = r * (uint64_t)block_bytes;
+                    const bool same_prior = p.prior_rec && off < p.prior_rec->size &&
+                                            std::min<uint64_t>(block_bytes, p.prior_rec->size - off) == len &&
+                                            prior->hashes[p.prior_rec->first_block + r] == h;
+                    if (same_prior || out->bidx.contains(h, len)) out->skipped[e.first_block + r] = 1;
                     else { out->expect[e.first_block + r] = 1; n_read++; b_read += len; }
                 }
                 if (!n_read) { out->unread.push_back(f); continue; }
@@ -107,6 +112,12 @@ int plan_tree(const Manifest& man, uint32_t block_bytes, const std::string& dst_
         if (plen == b.len) { b.prior_hash = t.hashes[rec->first_block + b.file_off / block_bytes]; b.prior_valid = 1; }
     }
     return VMIG_OK;
+}
+
+bool live_identity_holds(const struct stat& before, int64_t clock_ns, const struct stat& after)
+{
+    return S_ISREG(before.st_mode) && before.st_nlink == 1 && ctime_ns(before) < clock_ns &&
+           after.st_ino == before.st_ino && after.st_size == before.st_size && ctime_ns(after) == ctime_ns(before);
 }
 
 }  // namespace vmig

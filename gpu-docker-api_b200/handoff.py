@@ -22,8 +22,8 @@ from typing import Callable, Optional
 import threading
 
 from . import (F_PRUNE, F_VERIFY, VMIG_ECANCELED, Ctl, GetContainerMergedLayer, GetVolumeMountPoint, VmigError,
-               compare_snapshot, manifest, migrate_tree, restore_paths, restore_tree, retire_versions, rollback_layer,
-               scrub_store, snapshot_layer, snapshot_tree)
+               compare_snapshot, manifest, migrate_layer, migrate_tree, restore_paths, restore_tree, retire_versions,
+               rollback_layer, scrub_store, snapshot_layer, snapshot_tree)
 
 log = logging.getLogger("vmig.handoff")
 _root: dict = {"cwd": None}
@@ -56,6 +56,17 @@ def CopyDirDiffVerified(src, dest, priorTable, outTable, ctl: Optional[Ctl] = No
     """The pass after which the old container is deleted: the destination is re-read through the GPU and must hash
     like the source (VMIG_F_VERIFY), and holds nothing the source does not (VMIG_F_PRUNE)."""
     return CopyDirDiff(src, dest, priorTable, outTable, F_VERIFY | F_PRUNE, ctl)
+
+
+def CopyDirFromLayerVerified(src, srcTable, dest, priorTable, outTable, srcOutTable, prune: bool = True,
+                             ctl: Optional[Ctl] = None) -> dict:
+    """utils.CopyDirFromLayerVerified of the cgo shim: CopyDirDiffVerified through the source's own block table
+    (vmig_migrate_layer).  Of a source file srcTable still vouches for, only the blocks that differ from the destination's
+    priorTable record are read; the re-read covers only the destination files the call created, wrote into or resized.
+    srcOutTable receives the table the next call trusts as srcTable.  prune False: no F_PRUNE (the hand-off's live
+    pass).  ctl: the mirror of the shim's ...Context variant."""
+    return migrate_layer(src, srcTable or None, dest, priorTable or None, outTable or None, srcOutTable or None,
+                         flags=F_VERIFY | (F_PRUNE if prune else 0), ctl=ctl)
 
 
 def SnapshotDirVerified(src, dest, outTable) -> dict:
@@ -309,6 +320,63 @@ def HandoffCopy(oldContainer: str, newContainer: str, pause: Callable[[str], Non
     finally:
         if pass1 is not None and pass1.exists():
             pass1.unlink()
+
+
+def HandoffCopyFromLayer(oldContainer: str, newContainer: str, pause: Callable[[str], None],
+                         resume: Callable[[str], None], pauseBudget: float = 0.0, ctl: Optional[Ctl] = None) -> dict:
+    """N2: HandoffCopy whose paused pass costs what the tenant changed during the live pass, not two reads of the layer.
+    Pass 1 (live) is verified and also leaves a table of the SOURCE's files (<table>.pass1src; a file written while it
+    was read is recorded without an identity).  Pass 2 (paused) trusts that table: a source file still as it recorded
+    it is not read where the destination still is pass 1's record (<table>.pass1), and only what pass 2 wrote is
+    re-read.  Pause budget, resume-on-error and ctl as in HandoffCopy; a failed live pass falls back to HandoffCopy's
+    single paused pass.  Both .pass1 tables are removed at the end."""
+    src = GetContainerMergedLayer(oldContainer)
+    dst = GetContainerMergedLayer(newContainer)
+    _, table = snapshotPaths(newContainer)
+    table.parent.mkdir(parents=True, exist_ok=True)
+    pass1, pass1src = Path(str(table) + ".pass1"), Path(str(table) + ".pass1src")
+    out = {"pass1": None, "pass1_error": None}
+    try:
+        fallback = False
+        try:
+            out["pass1"] = CopyDirFromLayerVerified(src, None, dst, None, pass1, pass1src, prune=False, ctl=ctl)
+        except VmigError as e:      # live source: a file that shrinks under the reader, a directory swapped for a symlink
+            if e.code == VMIG_ECANCELED:
+                raise
+            log.warning("vmig: live pass of %s failed (%s); falling back to one paused pass", oldContainer, e)
+            out["pass1_error"] = e.code
+            fallback = True
+        pause(oldContainer)
+        with Ctl() as budget:
+            expired = threading.Event()
+
+            def expire():
+                expired.set()
+                budget.cancel()
+            timer = threading.Timer(pauseBudget, expire) if pauseBudget > 0 else None
+            if timer is not None:
+                timer.start()
+            try:
+                if fallback:
+                    out["pass2"] = CopyDirDiffVerified(src, dst, None, table, ctl=budget)
+                else:
+                    out["pass2"] = CopyDirFromLayerVerified(src, pass1src, dst, pass1, table, None, ctl=budget)
+            except VmigError as e:
+                resume(oldContainer)
+                if e.code == VMIG_ECANCELED and expired.is_set():
+                    e.pause_budget_exceeded = True
+                    log.warning("vmig: final pass of %s exceeded its pause budget of %.3f s; old container resumed",
+                                oldContainer, pauseBudget)
+                raise
+            finally:
+                if timer is not None:
+                    timer.cancel()
+                    timer.join()
+        return out
+    finally:
+        for p in (pass1, pass1src):
+            if p.exists():
+                p.unlink()
 
 
 def UsedBytes(volVersionName: str) -> int:

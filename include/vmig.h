@@ -623,6 +623,66 @@ int vmig_snapshot_layer(const char* layer_dir, const char* layer_table,
                         const char* out_table, const vmig_opts* opts /*nullable*/, vmig_stats* stats /*nullable*/,
                         vmig_layer_snapshot_stats* ls_stats /*nullable*/);
 
+/* A migration through the source's own block table: what vmig_migrate_layer trusted, read, verified and recorded. */
+typedef struct vmig_layer_migrate_stats {
+    uint64_t files_trusted, bytes_trusted;        /* source files whose hashes came from src_table                       */
+    uint64_t files_read, bytes_read;              /* source files with >= 1 block read; source bytes read (H2D)          */
+    uint64_t files_unread;                        /* trusted files with nothing to read: every block is the prior's      */
+    uint64_t files_verified, bytes_verified;      /* VMIG_F_VERIFY: destination files re-read, and their bytes           */
+    uint64_t src_recorded, src_unrecorded;        /* src_out_table records with / without an identity                    */
+    uint64_t reserved[4];
+} vmig_layer_migrate_stats;
+
+/* Migrate src_dir into dst_dir as vmig_migrate_tree(src_dir, dst_dir, prior_table, out_table, ...) does, reading from
+ * the source only the blocks the destination does not already hold.  src_table is a block table written for the
+ * source's files (src_out_table of an earlier call of this function, typically the hand-off's live pass); the hashes of
+ * a file it still vouches for are taken from it instead of from a read.  The paused pass of a hand-off then costs what
+ * the tenant changed since the live pass, where vmig_migrate_tree reads the whole layer and VMIG_F_VERIFY re-reads all
+ * of the destination.
+ *   - Result: with truthful records, dst_dir, out_table's paths, sizes and hashes, and bytes_written equal what
+ *     vmig_migrate_tree leaves with the same prior_table and flags (prune, metadata, hard links and kind changes
+ *     included).  Why: a block that is not read is one whose source record (XXH64, length) equals the prior record's at
+ *     the same index of a destination file the prior table still vouches for; K1 would return that hash, and
+ *     vmig_migrate_tree would skip that block too.
+ *   - Source side: a source regular file is trusted when src_table records it with an inode, an lstat still shows the
+ *     walked inode and size, and it still is its record (inode, size, ctime: the in-place diff path's rule).  Format-01
+ *     tables, hard-linked paths and a table written for another directory trust nothing.  Of a trusted file whose
+ *     destination prior_table trusts, a block whose recorded (XXH64, length) equals the prior record's at the same index
+ *     is neither read nor written; every other block of a trusted file is read and K1 must return the record's hash
+ *     before its batch is written, else VMIG_ESRCCHANGED naming the path and block.  A trusted file with nothing to read
+ *     is finished (size, metadata) without entering the pipeline.  An untrusted file is handled exactly as
+ *     vmig_migrate_tree handles it.  After the data pass every trusted file must still be its record (lstat), else
+ *     VMIG_ESRCCHANGED.  Nothing under src_dir is written.
+ *   - src_out_table (nullable): out_table's paths, sizes and hashes with the SOURCE files' identities, for the next call
+ *     to trust.  The source may be written while it is read, so a read file's identity is recorded only when its fstat
+ *     before the first block was read shows a ctime strictly older than a CLOCK_REALTIME_COARSE reading taken just
+ *     before that fstat, and an fstat once its last block's hash is back shows the same inode, size and ctime; else the
+ *     record carries 0/0 and the next call reads the file (not an error).  A trusted unread file carries its src_table
+ *     record forward; hard-linked paths carry 0/0.  The rule is the ctime rule of every table: a write that moves no
+ *     ctime (a shared-mmap store on a filesystem that does not stamp it) is invisible to it.
+ *   - VMIG_F_VERIFY re-reads every destination file this call created or replaced, wrote a block into, or resized, and
+ *     not the files it left alone: those still are their prior record, whose hashes the earlier pass computed (and, in
+ *     the hand-off, verified).  This is the one deliberate difference from vmig_migrate_tree.  With VMIG_F_PRUNE the
+ *     entry-set check runs as in a migration.
+ *   - Refusals, in this order, each before anything is read or written: VMIG_EINVAL (src_dir or dst_dir NULL or empty;
+ *     flags other than VMIG_F_VERIFY | VMIG_F_PRUNE | VMIG_F_DIRECT_IO | VMIG_F_MTIME_NS | VMIG_F_NO_METADATA |
+ *     VMIG_F_SKIP_HIDDEN_TOPDIRS; bad block_bytes; src_dir and dst_dir the same directory or one inside the other, by
+ *     real path; out_table equal to src_out_table; either output table inside src_dir; src_out_table inside dst_dir);
+ *     a control cancelled before the call: VMIG_ECANCELED; VMIG_ENOTDIR (either directory missing or not a directory);
+ *     VMIG_ETABLE (src_table or prior_table given and does not load, or its block_bytes differs from the call's);
+ *     VMIG_ENOGPU (no CPU fallback, even when nothing needs reading).
+ *   - Control: vmig_opts.ctl as for the tree calls; phases WALK, (PRUNE), DATA, META, (VERIFY), TABLE, DONE.
+ *     bytes_total / blocks_total are the source bytes and blocks to read.  A cancel is honoured where vmig_migrate_tree
+ *     honours it and per unread trusted file.  A failed or cancelled call leaves no new out_table or src_out_table and no
+ *     .tmp of either; src_table and prior_table are left byte-identical.
+ *   - stats (nullable): as for vmig_migrate_tree, with bytes_total / blocks_total as above; without VMIG_F_VERIFY,
+ *     bytes_h2d == lm_stats.bytes_read.  lm_stats (nullable): the counters above, written on success. */
+int vmig_migrate_layer(const char* src_dir, const char* src_table /*nullable*/,
+                       const char* dst_dir, const char* prior_table /*nullable*/,
+                       const char* out_table /*nullable*/, const char* src_out_table /*nullable*/,
+                       const vmig_opts* opts /*nullable*/, vmig_stats* stats /*nullable*/,
+                       vmig_layer_migrate_stats* lm_stats /*nullable*/);
+
 /* utils.CopyDir(src, dest) (reference utils/copy.go:21-27) == vmig_migrate_tree with defaults. */
 int vmig_copy_dir(const char* src_dir, const char* dst_dir);
 
@@ -645,7 +705,7 @@ void vmig_host_free(void* p);
 
 /* ---- cancellation and progress ------------------------------------------------------------------
  * A control is a numeric id (cgo passes it in vmig_opts.ctl without any pointer rules).  It serves the entry points
- * that take vmig_opts: vmig_migrate_tree, vmig_restore_tree, vmig_restore_paths, vmig_snapshot_tree, vmig_scrub_store, vmig_retire_versions, vmig_compare_snapshot, vmig_rollback_layer, vmig_snapshot_layer and vmig_migrate_buffer (a caller that
+ * that take vmig_opts: vmig_migrate_tree, vmig_restore_tree, vmig_restore_paths, vmig_snapshot_tree, vmig_scrub_store, vmig_retire_versions, vmig_compare_snapshot, vmig_rollback_layer, vmig_snapshot_layer, vmig_migrate_layer and vmig_migrate_buffer (a caller that
  * wants to cancel a copy or a move calls vmig_migrate_tree with the flags vmig_copy_dir / vmig_move_dir use).  One
  * control serves one call at a time: attaching it to a second concurrent call fails with VMIG_EINVAL.  The engine has
  * no deadline of its own; a deadline is the caller's timer calling vmig_ctl_cancel.

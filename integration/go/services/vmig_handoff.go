@@ -372,6 +372,60 @@ func HandoffCopy(ctx context.Context, oldContainer, newContainer string, pauseBu
 	return nil
 }
 
+// N2 -- HandoffCopyFromLayer is HandoffCopy whose paused pass costs what the tenant changed during the live pass, not
+// two reads of the layer.  Pass 1 (live) is verified and also leaves a table of the SOURCE's files (<table>.pass1src; a
+// file written while it was read is recorded without an identity).  Pass 2 (paused) trusts that table: a source file
+// still as it recorded it is not read where the destination still is pass 1's record (<table>.pass1), and only what
+// pass 2 wrote is re-read.  Pause budget, resume-on-error and ctx as in HandoffCopy; a failed live pass falls back to
+// HandoffCopy's single paused pass.  Both .pass1 tables are removed at the end.
+func HandoffCopyFromLayer(ctx context.Context, oldContainer, newContainer string, pauseBudget time.Duration, pause, resume func(name string) error) error {
+	src, err := utils.GetContainerMergedLayer(oldContainer)
+	if err != nil {
+		return errors.WithMessagef(err, "utils.GetContainerMergedLayer failed, container: %s", oldContainer)
+	}
+	dst, err := utils.GetContainerMergedLayer(newContainer)
+	if err != nil {
+		return errors.WithMessagef(err, "utils.GetContainerMergedLayer failed, container: %s", newContainer)
+	}
+	_, table := snapshotPaths(newContainer)
+	if err := os.MkdirAll(filepath.Dir(table), 0755); err != nil {
+		return errors.Wrapf(err, "mkdir %s", filepath.Dir(table))
+	}
+	pass1, pass1src := table+".pass1", table+".pass1src"
+	defer os.Remove(pass1)
+	defer os.Remove(pass1src)
+	fallback := false
+	if err := utils.CopyDirFromLayerVerifiedContext(ctx, src, "", dst, "", pass1, pass1src, false); err != nil {
+		if ctx.Err() != nil {
+			return errors.WithMessage(err, "hand-off cancelled during the live pass; old container untouched")
+		}
+		log.Warnf("vmig: live pass of %s failed (%v); falling back to one paused pass", oldContainer, err)
+		fallback = true
+	}
+	if err := pause(oldContainer); err != nil {
+		return errors.WithMessage(err, "pause before the final pass failed")
+	}
+	budget, cancel := context.Background(), context.CancelFunc(func() {})
+	if pauseBudget > 0 {
+		budget, cancel = context.WithTimeout(context.Background(), pauseBudget)
+	}
+	defer cancel()
+	if fallback {
+		err = utils.CopyDirDiffVerifiedContext(budget, src, dst, "", table)
+	} else {
+		err = utils.CopyDirFromLayerVerifiedContext(budget, src, pass1src, dst, pass1, table, "", true)
+	}
+	if err != nil {
+		_ = resume(oldContainer)
+		if errors.Is(err, context.DeadlineExceeded) {
+			log.Warnf("vmig: final pass of %s exceeded its pause budget of %v; old container resumed", oldContainer, pauseBudget)
+			return errors.WithMessagef(ErrPauseBudgetExceeded, "%v", err)
+		}
+		return errors.WithMessage(err, "final pass failed; old container resumed, nothing deleted")
+	}
+	return nil
+}
+
 // ErrPauseBudgetExceeded: HandoffCopy's final pass did not finish within its pause budget; the old container was
 // resumed and nothing was deleted.  Test with errors.Is.
 var ErrPauseBudgetExceeded = stderrors.New("vmig: final pass exceeded the pause budget")

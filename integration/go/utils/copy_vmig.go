@@ -177,6 +177,39 @@ func SnapshotDirFromLayerVerifiedContext(ctx context.Context, src, dest, baseDir
 		})
 }
 
+// CopyDirFromLayerVerified is CopyDirDiffVerified through the source's own block table srcTable (vmig_migrate_layer):
+// of a source file srcTable still vouches for, only the blocks that differ from dest's priorTable record at the same
+// index are read, and the re-read (VMIG_F_VERIFY) covers only the destination files the call created, wrote into or
+// resized.  dest and outTable are what CopyDirDiffVerified leaves.  srcOutTable (may be "") receives outTable's hashes
+// with the source files' identities, for the next call's srcTable; a file written while it was read is recorded without
+// one.  prune false: no VMIG_F_PRUNE (the hand-off's live pass).  srcTable and priorTable may be "".
+func CopyDirFromLayerVerified(src, srcTable, dest, priorTable, outTable, srcOutTable string, prune bool) error {
+	return CopyDirFromLayerVerifiedContext(context.Background(), src, srcTable, dest, priorTable, outTable, srcOutTable, prune)
+}
+
+// CopyDirFromLayerVerifiedContext is CopyDirFromLayerVerified that stops when ctx is done (see CopyDirDiffContext);
+// the source, srcTable and priorTable are untouched either way, and neither outTable nor srcOutTable is written.
+func CopyDirFromLayerVerifiedContext(ctx context.Context, src, srcTable, dest, priorTable, outTable, srcOutTable string, prune bool) error {
+	var ct, cso *C.char
+	if srcTable != "" {
+		ct = C.CString(srcTable)
+		defer C.free(unsafe.Pointer(ct))
+	}
+	if srcOutTable != "" {
+		cso = C.CString(srcOutTable)
+		defer C.free(unsafe.Pointer(cso))
+	}
+	flags := C.uint32_t(C.VMIG_F_VERIFY)
+	if prune {
+		flags |= C.VMIG_F_PRUNE
+	}
+	return runDiff(ctx, "vmig_migrate_layer", src, dest, priorTable, outTable, flags,
+		func(cs, cd, cp, co *C.char, o *C.vmig_opts, st *C.vmig_stats, _ *C.vmig_snapshot_stats) C.int {
+			var ms C.vmig_layer_migrate_stats
+			return C.vmig_migrate_layer(cs, ct, cd, cp, co, cso, o, st, &ms)
+		})
+}
+
 // ScrubSnapshots checks every snapshot snapDirs[i] against its block table snapTables[i] in one pass that reads each
 // inode the snapshots share once (vmig_scrub_store), and writes every finding to report.  verdicts[i] is the VMIG_*
 // code a hash-only restore of that snapshot would return (VMIG_OK, VMIG_ECORRUPT, VMIG_ETABLE, VMIG_ENOTDIR); a

@@ -653,22 +653,26 @@ int check_block_bytes(const vmig_opts& o)
     return VMIG_OK;
 }
 
-struct SnapshotArgs {
-    const char* base_dir;              // both NULL: a full snapshot
-    const char* base_table;
-    vmig_snapshot_stats* out;          // nullable
-    // vmig_snapshot_layer: both tables already loaded, and the source's own table
-    const BlockTable* base_loaded = nullptr;
-    const BlockTable* layer = nullptr;
-    vmig_layer_snapshot_stats* layer_out = nullptr;    // nullable
-};
-
-// vmig_migrate_layer: the loaded tables, and what the call writes besides the tree call's results
-struct LayerMigrateArgs {
-    const BlockTable* src_table;       // an empty table when none is given: nothing is trusted
-    const BlockTable* prior;           // nullable
-    const char* src_out;               // nullable
-    vmig_layer_migrate_stats* out;     // nullable
+// What the passes of a tree call consume (tree_passes).  Every table is loaded by the call before the passes start;
+// a null table is none.
+struct TreeCall {
+    std::string src, dst;
+    const Manifest* man = nullptr;
+    std::vector<uint64_t> expect;           // a checked restore: the snapshot table's hashes in the manifest's block order
+    const BlockTable* prior = nullptr;      // a destination file that still is its record is patched in place
+    const BlockTable* base = nullptr;       // the snapshots: unchanged files and blocks come from the base
+    std::string base_dir;                   //   (FileIO::finish_from_base), when base_dir is on the destination's device
+    const BlockTable* layer = nullptr;      // the layer calls: the source's own table (an empty one trusts nothing)
+    // vmig_restore_paths: the parent chains are made real directories before the plan looks at the destination, the
+    // prune and its verify stay beneath the chosen directories, the destination root's metadata ("." here stands for
+    // it) is not replayed, and no table is written
+    Selection* sel = nullptr;
+    const char* out_table = nullptr;
+    const char* src_out_table = nullptr;    // vmig_migrate_layer: out_table with the source files' identities
+    bool refresh_ids = false;               // the snapshots: record the identities the call's own links moved
+    vmig_snapshot_stats* snap_out = nullptr;                // the call-specific stats (nullable)
+    vmig_layer_snapshot_stats* layer_snap_out = nullptr;
+    vmig_layer_migrate_stats* layer_mig_out = nullptr;
 };
 
 // After the data pass: hard-linked paths take their primary's hashes, empty regular files are created, then the rest of
@@ -860,37 +864,22 @@ int recheck_trusted(const std::string& src, const Manifest& man, const TreePlan&
     return VMIG_OK;
 }
 
-// The passes of a tree call after its manifest is walked and checked: plan, (prune), data, metadata, (verify), table,
-// (move).  expect: the snapshot table's hashes in the manifest's block order (a checked restore), else empty.
-// snapshot non-null: vmig_snapshot_tree -- unchanged files and blocks come from the base (FileIO::finish_from_base).
-// sel non-null: vmig_restore_paths -- the parent chains are made real directories before the plan looks at the
-// destination, the prune and its verify stay beneath the chosen directories, the destination root's metadata ("."
-// here stands for it) is not replayed, and no table is written.
-// lm non-null: vmig_migrate_layer -- a migration with the source's own table (the layer branch of plan_tree against the
-// prior), src_out_table, and a verify of only what the call wrote.
-int tree_passes(CallScope& call, const std::string& src, const std::string& dst, Manifest& man, const std::vector<uint64_t>& expect,
-                const char* prior_path, const char* out_path, const vmig_opts& o, vmig_stats& st, const SnapshotArgs* snapshot,
-                Selection* sel, uint64_t t_begin, vmig_stats* stats_out, const LayerMigrateArgs* lm = nullptr)
+// The passes of a tree call after its manifest is walked and checked and its tables are loaded: plan, (prune), data,
+// metadata, (verify), table, (move).  st arrives with the walk's and the table loads' times.
+int tree_passes(CallScope& call, const TreeCall& c, const vmig_opts& o, vmig_stats& st, uint64_t t_begin, vmig_stats* stats_out)
 {
-    const char* base_dir = snapshot ? snapshot->base_dir : nullptr;
-    const char* base_path = snapshot ? snapshot->base_table : nullptr;
+    const std::string& src = c.src;
+    const std::string& dst = c.dst;
+    const Manifest& man = *c.man;
+    const BlockTable* layer = c.layer;
+    Selection* sel = c.sel;
     const std::atomic<int>* cancel = call.cancel();
     const bool hash_only = (o.flags & VMIG_F_HASH_ONLY) != 0;
     int rc;
     uint64_t t0 = now_ns();
-    BlockTable prior_own;
-    const bool has_prior = prior_path && *prior_path && !hash_only;
-    const BlockTable& prior = lm && lm->prior ? *lm->prior : prior_own;
-    if (has_prior && !(lm && lm->prior) && (rc = load_table(prior_path, "prior", o.block_bytes, &prior_own))) return rc;
-    const BlockTable* layer = snapshot ? snapshot->layer : lm ? lm->src_table : nullptr;
-    BlockTable base_own; bool has_base = false;
-    const BlockTable& base = snapshot && snapshot->base_loaded ? *snapshot->base_loaded : base_own;
-    if (base_path) {
-        if (!snapshot->base_loaded && (rc = load_table(base_path, "base", o.block_bytes, &base_own))) return rc;
-        // a hard link cannot cross devices, and a base on another filesystem shares nothing with the snapshot
-        struct stat bst, dst_st;
-        has_base = stat(base_dir, &bst) == 0 && stat(dst.c_str(), &dst_st) == 0 && bst.st_dev == dst_st.st_dev;
-    }
+    // a hard link cannot cross devices, and a base on another filesystem shares nothing with the snapshot
+    struct stat bst, dst_st;
+    const bool has_base = c.base && stat(c.base_dir.c_str(), &bst) == 0 && stat(dst.c_str(), &dst_st) == 0 && bst.st_dev == dst_st.st_dev;
     if (sel) {
         if (cancel->load()) return fail(VMIG_ECANCELED, "before the destination's parent directories were made");
         rc = prepare_parents(dst, sel, cancel);
@@ -906,12 +895,11 @@ int tree_passes(CallScope& call, const std::string& src, const std::string& dst,
     if (io.cufile) { rc = cufile_open(); if (rc) return rc; }
     rc = io.open_root(); if (rc) return rc;
     TreePlan plan;
-    rc = plan_tree(man, o.block_bytes, dst, has_prior ? &prior : nullptr, has_base ? base_dir : "", has_base ? &base : nullptr, cancel, &plan,
-                   src, layer);
+    rc = plan_tree(man, o.block_bytes, dst, c.prior, has_base ? c.base_dir : "", has_base ? c.base : nullptr, cancel, &plan, src, layer);
     if (rc) return rc;
     st.files_untrusted = plan.files_untrusted;
     io.init_files(man, plan);
-    const bool src_out = lm && lm->src_out && *lm->src_out;
+    const bool src_out = c.src_out_table && *c.src_out_table;
     if (src_out) {
         io.hold_sources();
         for (uint32_t f : plan.unread)                     // a trusted unread file keeps its record's identity
@@ -919,10 +907,10 @@ int tree_passes(CallScope& call, const std::string& src, const std::string& dst,
     }
     // a trusted layer file's hashes are its record's: the unread blocks keep them, K1 must return them for the rest
     std::vector<uint64_t> hashes = layer ? plan.layer_hashes : std::vector<uint64_t>(man.n_blocks, 0);
-    if (has_base) { io.base_root = base_dir; io.bidx = &plan.bidx; io.hashes = hashes.data(); }
+    if (has_base) { io.base_root = c.base_dir; io.bidx = &plan.bidx; io.hashes = hashes.data(); }
     // skip mode whenever the base can supply a block, also when no source path has a same-path record (a layer whose
     // files were all moved): without it the submitter streams every block back with its hash (DESIGN.md §3)
-    const bool skip_mode = has_prior || plan.any_base || !plan.bidx.empty();
+    const bool skip_mode = c.prior || plan.any_base || !plan.bidx.empty();
     if ((plan.any_base || !plan.bidx.empty()) && io.skipped.empty()) io.skipped.assign(man.n_blocks, 0);
     if (layer) { call.ctl->bytes_total.store(plan.bytes_read); call.ctl->blocks_total.store(plan.blocks.size()); }
     st.ns_plan += now_ns() - t0;
@@ -942,7 +930,7 @@ int tree_passes(CallScope& call, const std::string& src, const std::string& dst,
 
     t0 = now_ns();
     BlockExpect bexp;
-    if (!expect.empty()) bexp.hashes = expect.data();
+    if (!c.expect.empty()) bexp.hashes = c.expect.data();
     if (layer) { bexp.hashes = plan.layer_hashes.data(); bexp.valid = plan.expect.data(); bexp.code = VMIG_ESRCCHANGED; }
     if (layer) rc = finish_unread(call, o, io, plan.unread);
     if (!rc) rc = run_blocks(plan.blocks, &io, skip_mode, hash_only, o, hashes.data(), &st, call.ctl, false, bexp.hashes ? &bexp : nullptr);
@@ -952,7 +940,7 @@ int tree_passes(CallScope& call, const std::string& src, const std::string& dst,
 
     t0 = now_ns();
     call.phase(VMIG_PHASE_META);
-    rc = meta_pass(call, io, expect, &hashes, &st, sel ? 1 : 0);
+    rc = meta_pass(call, io, c.expect, &hashes, &st, sel ? 1 : 0);
     if (rc) return rc;
     st.ns_meta = now_ns() - t0;
 
@@ -960,14 +948,14 @@ int tree_passes(CallScope& call, const std::string& src, const std::string& dst,
     if ((o.flags & VMIG_F_VERIFY) && !hash_only) {
         call.phase(VMIG_PHASE_VERIFY);
         std::vector<uint32_t> files = data_files(man);
-        if (snapshot && layer) {    // vmig_snapshot_layer does not re-read what it linked: the base table already vouches for it
+        if (layer) {
+            // a layer call does not re-read what it linked (the base table already vouches for it) nor what it left alone
+            // (it still is its prior record).  vmig_snapshot_layer has no prior and vmig_migrate_layer no base, so in each
+            // call only one of the two tests can remove a file.
             std::unordered_set<uint32_t> linked(io.linked_files.begin(), io.linked_files.end());
-            files.erase(std::remove_if(files.begin(), files.end(), [&](uint32_t f) { return linked.count(f) != 0; }), files.end());
-        }
-        if (lm) {                   // vmig_migrate_layer does not re-read what it left alone: it still is its prior record
             files.erase(std::remove_if(files.begin(), files.end(), [&](uint32_t f) {
                 const TableFile* pr = plan.files[f].prior_rec;
-                return pr && !io.fs[f].wrote.load() && pr->size == man.files[f].size;
+                return linked.count(f) != 0 || (pr && !io.fs[f].wrote.load() && pr->size == man.files[f].size);
             }), files.end());
         }
         for (uint32_t f : files) { n_verified++; b_verified += man.files[f].size; }
@@ -978,7 +966,7 @@ int tree_passes(CallScope& call, const std::string& src, const std::string& dst,
     if (!sel) {
         t0 = now_ns();
         call.phase(VMIG_PHASE_TABLE);
-        if (snapshot) {
+        if (c.refresh_ids) {
             // a snapshot's table must let the next increment trust it: a linked path's ctime moved with this call's link to
             // the base inode, and a hard-linked file's with replay_metadata's link, both after block_done recorded it
             std::vector<uint32_t> moved = io.linked_files;
@@ -990,17 +978,17 @@ int tree_passes(CallScope& call, const std::string& src, const std::string& dst,
             // out_table takes it away again
             DstTree sv = static_cast<const DstTree&>(io);
             sv.ids = io.src_ids;
-            rc = write_table(sv, lm->src_out, hashes, cancel);
-            if (!rc && (rc = write_table(io, out_path, hashes, nullptr))) unlink(lm->src_out);
+            rc = write_table(sv, c.src_out_table, hashes, cancel);
+            if (!rc && (rc = write_table(io, c.out_table, hashes, nullptr))) unlink(c.src_out_table);
         } else if (!rc) {
-            rc = write_table(io, out_path, hashes, cancel);
+            rc = write_table(io, c.out_table, hashes, cancel);
         }
         if (rc) return rc;
         st.ns_table = now_ns() - t0;
     }
 
     if ((o.flags & VMIG_F_MOVE_SRC) && !hash_only) {
-        rc = finish_move(call, src, dst, man, out_path);
+        rc = finish_move(call, src, dst, man, c.out_table);
         if (rc) return rc;
     }
 
@@ -1010,23 +998,23 @@ int tree_passes(CallScope& call, const std::string& src, const std::string& dst,
     st.files = man.files.size(); st.dirs = man.dirs.size() - (sel ? 1 : 0);
     st.ns_total = now_ns() - t_begin;
     if (stats_out) *stats_out = st;
-    if (snapshot && snapshot->out) {
+    if (c.snap_out) {
         vmig_snapshot_stats ss; memset(&ss, 0, sizeof ss);
         ss.files_base_untrusted = plan.files_base_untrusted;
         ss.files_linked = io.n_linked.load(); ss.bytes_linked = io.b_linked.load();
         ss.files_backfilled = io.n_backfilled.load(); ss.bytes_backfilled = io.b_backfilled.load();
-        *snapshot->out = ss;
+        *c.snap_out = ss;
     }
-    if (snapshot && snapshot->layer_out) {
+    if (c.layer_snap_out) {
         vmig_layer_snapshot_stats ls; memset(&ls, 0, sizeof ls);
         ls.files_linked = io.n_linked.load(); ls.bytes_linked = io.b_linked.load();
         ls.files_backfilled = io.n_backfilled.load(); ls.bytes_backfilled = io.b_backfilled.load();
         ls.files_base_untrusted = plan.files_base_untrusted;
         ls.files_trusted = plan.files_trusted; ls.bytes_trusted = plan.bytes_trusted;
         ls.files_read = plan.files_read; ls.bytes_read = plan.bytes_read;
-        *snapshot->layer_out = ls;
+        *c.layer_snap_out = ls;
     }
-    if (lm && lm->out) {
+    if (c.layer_mig_out) {
         vmig_layer_migrate_stats ms; memset(&ms, 0, sizeof ms);
         ms.files_trusted = plan.files_trusted; ms.bytes_trusted = plan.bytes_trusted;
         ms.files_read = plan.files_read; ms.bytes_read = plan.bytes_read;
@@ -1034,57 +1022,80 @@ int tree_passes(CallScope& call, const std::string& src, const std::string& dst,
         ms.files_verified = n_verified; ms.bytes_verified = b_verified;
         if (src_out)
             for (const FileId& id : io.src_ids) (id.ino ? ms.src_recorded : ms.src_unrecorded)++;
-        *lm->out = ms;
+        *c.layer_mig_out = ms;
     }
     return VMIG_OK;
 }
 
-// snap_path non-null: vmig_restore_tree -- src_dir must match that block table (match_table before anything touches the
-// destination, every block's hash in the hash-waiter, hard-linked paths before metadata replay).
-// snapshot non-null: vmig_snapshot_tree (tree_passes).
-int migrate_tree_body(CallScope& call, const char* src_dir, const char* dst_dir, const char* prior_path, const char* out_path,
-                      const vmig_opts& o, vmig_stats* stats_out, const char* snap_path, const SnapshotArgs* snapshot)
+// A table a call names (path NULL or empty: none), loaded at the call's block size into *t
+struct NamedTable { const char* path; const char* what; BlockTable* t; };
+
+// The refusals of a call after its arguments, in this order: a cancelled control, a directory that is missing or not a
+// directory, a table that does not load, no GPU.  No CPU fallback: the GPU is there before anything is touched.
+int start_checks(CallScope& call, const vmig_opts& o, std::initializer_list<const char*> dirs, const std::vector<NamedTable>& tables)
 {
-    const std::atomic<int>* cancel = call.cancel();
+    if (call.cancel()->load()) return fail(VMIG_ECANCELED, "the control was cancelled before the call started");
+    for (const char* d : dirs) {
+        struct stat sb;
+        if (stat(d, &sb) != 0 || !S_ISDIR(sb.st_mode)) return fail(VMIG_ENOTDIR, "%s is missing or not a directory", d);
+    }
+    for (const NamedTable& n : tables)
+        if (n.path && *n.path) { const int rc = load_table(n.path, n.what, o.block_bytes, n.t); if (rc) return rc; }
+    std::vector<DeviceInfo> devs;
+    return ctx_select(o.gpu_mask, &devs);
+}
+
+// The tree calls' refusals after the arguments, in this order: a directory that cannot be stat'ed (VMIG_EIO) or is
+// not a directory (NULL: not checked), then start_checks' cancel and GPU
+int tree_start_checks(CallScope& call, const vmig_opts& o, std::initializer_list<const char*> dirs)
+{
+    for (const char* d : dirs) {
+        struct stat sb;
+        if (!d) continue;
+        if (stat(d, &sb) != 0) return fail(VMIG_EIO, "stat %s: %s", d, errno_str(errno).c_str());
+        if (!S_ISDIR(sb.st_mode)) return fail(VMIG_ENOTDIR, "%s is not a directory", d);
+    }
+    return start_checks(call, o, {}, {});
+}
+
+// vmig_migrate_tree, vmig_restore_tree, vmig_snapshot_tree, vmig_copy_dir and vmig_move_dir: the refusals after the
+// arguments, the walk, then the tables the call names, loaded into c in this order: snap_path (vmig_restore_tree:
+// src_dir must be the tree that table describes, checked before anything touches the destination), prior_path (not
+// under VMIG_F_HASH_ONLY), base_table.  c arrives with the rest: out_table, and a snapshot's base_dir, identity
+// refresh and stats.
+int migrate_tree_body(CallScope& call, TreeCall c, const char* src_dir, const char* dst_dir, const char* prior_path,
+                      const char* snap_path, const char* base_table, const vmig_opts& o, vmig_stats* stats_out)
+{
     vmig_stats st; memset(&st, 0, sizeof st);
     const uint64_t t_begin = now_ns();
     if (!src_dir || !*src_dir) return fail(VMIG_EINVAL, "src_dir is NULL/empty");
     const bool hash_only = (o.flags & VMIG_F_HASH_ONLY) != 0;
     if (!hash_only && (!dst_dir || !*dst_dir)) return fail(VMIG_EINVAL, "dst_dir is NULL/empty");
     int rc = check_block_bytes(o);
+    if (!rc) rc = tree_start_checks(call, o, {src_dir, hash_only ? nullptr : dst_dir});
     if (rc) return rc;
-    const std::string src(src_dir), dst(dst_dir ? dst_dir : "");
-    struct stat sst;
-    if (stat(src.c_str(), &sst) != 0) return fail(VMIG_EIO, "stat %s: %s", src.c_str(), errno_str(errno).c_str());
-    if (!S_ISDIR(sst.st_mode)) return fail(VMIG_ENOTDIR, "%s is not a directory", src.c_str());
-    if (!hash_only) {
-        if (stat(dst.c_str(), &sst) != 0) return fail(VMIG_EIO, "stat %s: %s", dst.c_str(), errno_str(errno).c_str());
-        if (!S_ISDIR(sst.st_mode)) return fail(VMIG_ENOTDIR, "%s is not a directory", dst.c_str());
-    }
-    if (cancel->load()) return fail(VMIG_ECANCELED, "the control was cancelled before the call started");
-    // make sure a GPU is there before touching the destination: no CPU fallback
-    std::vector<DeviceInfo> devs;
-    rc = ctx_select(o.gpu_mask, &devs);
-    if (rc) return rc;
+    c.src = src_dir; c.dst = dst_dir ? dst_dir : "";
 
     Manifest man;
     uint64_t t0 = now_ns();
     call.phase(VMIG_PHASE_WALK);
-    rc = walk_tree(src, o.block_bytes, (o.flags & VMIG_F_SKIP_HIDDEN_TOPDIRS) != 0, &man, cancel);
+    rc = walk_tree(c.src, o.block_bytes, (o.flags & VMIG_F_SKIP_HIDDEN_TOPDIRS) != 0, &man, call.cancel());
     if (rc) return rc;
     st.ns_walk = now_ns() - t0;
     call.ctl->bytes_total.store(man.bytes_total); call.ctl->blocks_total.store(man.n_blocks);
+    c.man = &man;
 
     t0 = now_ns();
-    std::vector<uint64_t> expect;
+    BlockTable snap, prior, base;
     if (snap_path) {
-        BlockTable snap;
         rc = load_table(snap_path, "snapshot", o.block_bytes, &snap);
-        if (!rc) rc = match_table(man, snap, &expect);
-        if (rc) return rc;
+        if (!rc) rc = match_table(man, snap, &c.expect);
     }
+    if (!rc && prior_path && *prior_path && !hash_only) { rc = load_table(prior_path, "prior", o.block_bytes, &prior); c.prior = &prior; }
+    if (!rc && base_table) { rc = load_table(base_table, "base", o.block_bytes, &base); c.base = &base; }
+    if (rc) return rc;
     st.ns_plan = now_ns() - t0;
-    return tree_passes(call, src, dst, man, expect, prior_path, out_path, o, st, snapshot, nullptr, t_begin, stats_out);
+    return tree_passes(call, c, o, st, t_begin, stats_out);
 }
 
 // vmig_restore_paths: the chosen entries of a snapshot, checked against the part of its table they cover (DESIGN.md §6)
@@ -1094,24 +1105,19 @@ int restore_paths_body(CallScope& call, const char* snap_dir, const char* snap_t
     const std::atomic<int>* cancel = call.cancel();
     vmig_stats st; memset(&st, 0, sizeof st);
     const uint64_t t_begin = now_ns();
-    const std::string src(snap_dir), dst(dst_dir);
-    struct stat sst;
-    if (stat(src.c_str(), &sst) != 0) return fail(VMIG_EIO, "stat %s: %s", src.c_str(), errno_str(errno).c_str());
-    if (!S_ISDIR(sst.st_mode)) return fail(VMIG_ENOTDIR, "%s is not a directory", src.c_str());
-    if (stat(dst.c_str(), &sst) != 0) return fail(VMIG_EIO, "stat %s: %s", dst.c_str(), errno_str(errno).c_str());
-    if (!S_ISDIR(sst.st_mode)) return fail(VMIG_ENOTDIR, "%s is not a directory", dst.c_str());
-    if (cancel->load()) return fail(VMIG_ECANCELED, "the control was cancelled before the call started");
-    std::vector<DeviceInfo> devs;                    // no CPU fallback: the GPU is there before anything is touched
-    int rc = ctx_select(o.gpu_mask, &devs);
+    int rc = tree_start_checks(call, o, {snap_dir, dst_dir});
     if (rc) return rc;
+    TreeCall c;
+    c.src = snap_dir; c.dst = dst_dir;
 
     uint64_t t0 = now_ns();
     call.phase(VMIG_PHASE_WALK);
     Selection sel;
-    rc = select_walk(src, paths, o.block_bytes, (o.flags & VMIG_F_SKIP_HIDDEN_TOPDIRS) != 0, &sel, cancel);
+    rc = select_walk(c.src, paths, o.block_bytes, (o.flags & VMIG_F_SKIP_HIDDEN_TOPDIRS) != 0, &sel, cancel);
     if (rc) return rc;
     st.ns_walk = now_ns() - t0;
     call.ctl->bytes_total.store(sel.man.bytes_total); call.ctl->blocks_total.store(sel.man.n_blocks);
+    c.man = &sel.man; c.sel = &sel;
 
     t0 = now_ns();
     BlockTable snap;
@@ -1124,57 +1130,51 @@ int restore_paths_body(CallScope& call, const char* snap_dir, const char* snap_t
             return fail(VMIG_ECORRUPT, "%s is in the block table but not in the snapshot (missing)", under.files[0].rel.c_str());
         return fail(VMIG_EINVAL, "%s is not in the snapshot", p.c_str());
     }
-    BlockTable part;                                 // records outside the selection are not looked at
+    BlockTable part, prior;                          // records outside the selection are not looked at
     table_subset(snap, sel.paths, &part);
-    std::vector<uint64_t> expect;
-    rc = match_table(sel.man, part, &expect);
+    rc = match_table(sel.man, part, &c.expect);
+    if (!rc && prior_path && *prior_path) { rc = load_table(prior_path, "prior", o.block_bytes, &prior); c.prior = &prior; }
     if (rc) return rc;
     st.ns_plan = now_ns() - t0;
-    return tree_passes(call, src, dst, sel.man, expect, prior_path, nullptr, o, st, nullptr, &sel, t_begin, stats_out);
+    return tree_passes(call, c, o, st, t_begin, stats_out);
 }
 
-// a is b, or either lies inside the other (real paths; a path that does not resolve is left to the call's own checks)
-bool real_paths_overlap(const char* a, const char* b, std::string* ra, std::string* rb)
+// The real path of p; empty when it does not resolve (errno says why)
+std::string real_path(const char* p)
 {
-    char* x = realpath(a, nullptr);
-    char* y = realpath(b, nullptr);
-    *ra = x ? x : ""; *rb = y ? y : "";
-    free(x); free(y);
-    return !ra->empty() && !rb->empty() && (path_inside(*ra, *rb) || path_inside(*rb, *ra));
+    char* r = realpath(p, nullptr);
+    const std::string s = r ? r : "";
+    free(r);
+    return s;
 }
 
-// snap_dir and dst_dir the same directory or one inside the other
-int check_restore_paths_dirs(const char* snap_dir, const char* dst_dir)
+// Refuses real paths ra and rb (named a and b, a first in the message) that are the same directory or where one lies
+// inside the other.  An empty one, a path that does not resolve, is left to the call's own checks.
+int check_apart(const char* a, const std::string& ra, const char* b, const std::string& rb)
 {
-    std::string as, bs;
-    if (real_paths_overlap(snap_dir, dst_dir, &as, &bs))
-        return fail(VMIG_EINVAL, "snap_dir %s and dst_dir %s are the same directory or one is inside the other", as.c_str(), bs.c_str());
-    return VMIG_OK;
+    if (ra.empty() || rb.empty() || !(path_inside(ra, rb) || path_inside(rb, ra))) return VMIG_OK;
+    return fail(VMIG_EINVAL, "%s %s and %s %s are the same directory or one is inside the other", a, ra.c_str(), b, rb.c_str());
 }
 
-int migrate_tree_impl(const char* src_dir, const char* dst_dir, const char* prior_path, const char* out_path,
-                      const vmig_opts* opts_in, vmig_stats* stats_out, const char* snap_path = nullptr,
-                      const SnapshotArgs* snapshot = nullptr)
+int migrate_tree_impl(const TreeCall& c, const char* src_dir, const char* dst_dir, const char* prior_path, const char* snap_path,
+                      const char* base_table, const vmig_opts* opts_in, vmig_stats* stats_out)
 {
     const vmig_opts o = norm_opts(opts_in);
     return in_call(o.ctl, [&](CallScope& call) {
-        return migrate_tree_body(call, src_dir, dst_dir, prior_path, out_path, o, stats_out, snap_path, snapshot);
+        return migrate_tree_body(call, c, src_dir, dst_dir, prior_path, snap_path, base_table, o, stats_out);
     });
 }
 
 // vmig_snapshot_tree: a base directory equal to the destination, or either one inside the other, is refused -- a
-// link or backfill would read what the same call is writing
+// link or backfill would read what the same call is writing.  A directory that does not resolve is refused too: a
+// missing base must not become a full snapshot.
 int check_snapshot_paths(const char* dst_dir, const char* base_dir)
 {
-    char* d = realpath(dst_dir, nullptr);
-    if (!d) return fail(VMIG_EIO, "realpath %s: %s", dst_dir, errno_str(errno).c_str());
-    char* b = realpath(base_dir, nullptr);
-    if (!b) { const int e = errno; free(d); return fail(VMIG_EIO, "realpath %s: %s", base_dir, errno_str(e).c_str()); }
-    const std::string ds(d), bs(b);
-    free(d); free(b);
-    if (path_inside(ds, bs) || path_inside(bs, ds))
-        return fail(VMIG_EINVAL, "base_dir %s and dst_dir %s are the same directory or one is inside the other", bs.c_str(), ds.c_str());
-    return VMIG_OK;
+    const std::string ds = real_path(dst_dir);
+    if (ds.empty()) return fail(VMIG_EIO, "realpath %s: %s", dst_dir, errno_str(errno).c_str());
+    const std::string bs = real_path(base_dir);
+    if (bs.empty()) return fail(VMIG_EIO, "realpath %s: %s", base_dir, errno_str(errno).c_str());
+    return check_apart("base_dir", bs, "dst_dir", ds);
 }
 
 // ---------------------------------------------------------------------------------------------
@@ -1227,9 +1227,7 @@ int scrub_body(CallScope& call, uint32_t n, const char* const* dirs, const char*
     vmig_stats st; memset(&st, 0, sizeof st);
     vmig_scrub_stats ss; memset(&ss, 0, sizeof ss);
     const uint64_t t_begin = now_ns();
-    if (cancel->load()) return fail(VMIG_ECANCELED, "the control was cancelled before the call started");
-    std::vector<DeviceInfo> devs;                    // no CPU fallback: the GPU is there before anything is read
-    int rc = ctx_select(o.gpu_mask, &devs);
+    int rc = start_checks(call, o, {}, {});
     if (rc) return rc;
 
     // ---- walk every version, load its table, merge the two (every difference recorded)
@@ -1396,15 +1394,11 @@ int retire_body(CallScope& call, const RetireArgs& a, const vmig_opts& o, vmig_s
     vmig_stats st; memset(&st, 0, sizeof st);
     vmig_retire_stats rs; memset(&rs, 0, sizeof rs);
     const uint64_t t_begin = now_ns();
-    if (cancel->load()) return fail(VMIG_ECANCELED, "the control was cancelled before the call started");
     const size_t n_keep = a.keep_dirs.size();
     std::vector<BlockTable> tab(n_keep);
-    for (size_t k = 0; k < n_keep; k++) {
-        const int rc = load_table(a.keep_tables[k].c_str(), "kept", o.block_bytes, &tab[k]);
-        if (rc) return rc;
-    }
-    std::vector<DeviceInfo> devs;                    // no CPU fallback: the GPU is there before anything is removed
-    int rc = ctx_select(o.gpu_mask, &devs);
+    std::vector<NamedTable> kept;
+    for (size_t k = 0; k < n_keep; k++) kept.push_back({a.keep_tables[k].c_str(), "kept", &tab[k]});
+    int rc = start_checks(call, o, {}, kept);
     if (rc) return rc;
 
     // ---- remove the retired versions, table first
@@ -1501,20 +1495,17 @@ int layer_hash_pass(CallScope& call, const vmig_opts& o, const Manifest& snap, c
     return VMIG_OK;
 }
 
-// Both calls' refusals after the arguments: a cancelled control, a missing directory, a table that does not load, no GPU
-int layer_call_checks(CallScope& call, const char* layer_dir, const char* layer_table, const char* snap_dir, const char* snap_table,
-                      const vmig_opts& o, BlockTable* snap_tab, BlockTable* layer_tab)
+// The snapshot's walk, which must be the tree its table describes: its manifest and the table's hashes in its block order
+int walk_snapshot(CallScope& call, const char* snap_dir, const BlockTable& snap_tab, const vmig_opts& o, Manifest* snap,
+                  std::vector<uint64_t>* snap_hashes, vmig_stats* st)
 {
-    if (call.cancel()->load()) return fail(VMIG_ECANCELED, "the control was cancelled before the call started");
-    for (const char* d : {layer_dir, snap_dir}) {
-        struct stat sb;
-        if (stat(d, &sb) != 0 || !S_ISDIR(sb.st_mode)) return fail(VMIG_ENOTDIR, "%s is missing or not a directory", d);
-    }
-    int rc = load_table(snap_table, "snapshot", o.block_bytes, snap_tab);
-    if (!rc && layer_table && *layer_table) rc = load_table(layer_table, "layer", o.block_bytes, layer_tab);
+    call.phase(VMIG_PHASE_WALK);
+    const uint64_t t0 = now_ns();
+    int rc = walk_tree(snap_dir, o.block_bytes, (o.flags & VMIG_F_SKIP_HIDDEN_TOPDIRS) != 0, snap, call.cancel());
+    if (!rc) rc = match_table(*snap, snap_tab, snap_hashes);
     if (rc) return rc;
-    std::vector<DeviceInfo> devs;                    // no CPU fallback: the GPU is there before anything is read
-    return ctx_select(o.gpu_mask, &devs);
+    st->ns_walk = now_ns() - t0;
+    return VMIG_OK;
 }
 
 // vmig_compare_snapshot: the plan, the merge and the report are vmig_compare.cpp's
@@ -1526,26 +1517,22 @@ int compare_body(CallScope& call, const char* layer_dir, const char* layer_table
     vmig_compare_stats cs; memset(&cs, 0, sizeof cs);
     const uint64_t t_begin = now_ns();
     BlockTable snap_tab, layer_tab;
-    int rc = layer_call_checks(call, layer_dir, layer_table, snap_dir, snap_table, o, &snap_tab, &layer_tab);
+    int rc = start_checks(call, o, {layer_dir, snap_dir}, {{snap_table, "snapshot", &snap_tab}, {layer_table, "layer", &layer_tab}});
     if (rc) return rc;
     const BlockTable* ltab = layer_table && *layer_table ? &layer_tab : nullptr;
 
-    // ---- walk both trees (the snapshot must be the tree its table describes); which layer files are read
-    call.phase(VMIG_PHASE_WALK);
-    uint64_t t0 = now_ns();
+    // ---- walk both trees; which layer files are read
     Manifest snap;
     std::vector<uint64_t> snap_hashes;
-    rc = walk_tree(snap_dir, o.block_bytes, (o.flags & VMIG_F_SKIP_HIDDEN_TOPDIRS) != 0, &snap, cancel);
-    if (!rc) rc = match_table(snap, snap_tab, &snap_hashes);
+    rc = walk_snapshot(call, snap_dir, snap_tab, o, &snap, &snap_hashes, &st);
     if (rc) return rc;
-    st.ns_walk = now_ns() - t0;
     LayerSide L;
     rc = layer_plan(layer_dir, snap, ltab, o, cancel, &L, &st);
     if (!rc) rc = layer_hash_pass(call, o, snap, snap_hashes, ltab, &L, &st);
     if (rc) return rc;
 
     // ---- the findings, compared on the host (8 bytes per block), and the report
-    t0 = now_ns();
+    const uint64_t t0 = now_ns();
     std::vector<CompareFinding> findings;
     CompareCounts c;
     compare_merge(L.man, snap, snap_hashes, L.hashes, o.block_bytes, (o.flags & VMIG_F_MTIME_NS) != 0,
@@ -1700,20 +1687,16 @@ int rollback_body(CallScope& call, const char* layer_dir, const char* layer_tabl
     vmig_stats st; memset(&st, 0, sizeof st);
     const uint64_t t_begin = now_ns();
     BlockTable snap_tab, layer_tab;
-    int rc = layer_call_checks(call, layer_dir, layer_table, snap_dir, snap_table, o, &snap_tab, &layer_tab);
+    int rc = start_checks(call, o, {layer_dir, snap_dir}, {{snap_table, "snapshot", &snap_tab}, {layer_table, "layer", &layer_tab}});
     if (rc) return rc;
     const BlockTable* ltab = layer_table && *layer_table ? &layer_tab : nullptr;
     const std::string layer(layer_dir);
 
-    // ---- the snapshot's walk, which must be the tree its table describes before the layer is touched
-    call.phase(VMIG_PHASE_WALK);
-    uint64_t t0 = now_ns();
+    // ---- the snapshot's walk, before the layer is touched
     Manifest snap;
     std::vector<uint64_t> snap_hashes;
-    rc = walk_tree(snap_dir, o.block_bytes, (o.flags & VMIG_F_SKIP_HIDDEN_TOPDIRS) != 0, &snap, cancel);
-    if (!rc) rc = match_table(snap, snap_tab, &snap_hashes);
+    rc = walk_snapshot(call, snap_dir, snap_tab, o, &snap, &snap_hashes, &st);
     if (rc) return rc;
-    st.ns_walk = now_ns() - t0;
 
     // ---- what the snapshot does not list goes first, as in a pruning restore; the layer is walked as it then stands
     call.phase(VMIG_PHASE_PRUNE);
@@ -1732,7 +1715,7 @@ int rollback_body(CallScope& call, const char* layer_dir, const char* layer_tabl
     const uint64_t hashed_bytes = st.bytes_total, hashed_blocks = st.blocks_total;
 
     // ---- the plan: one action per snapshot file, the sparse fetch list, the copy runs
-    t0 = now_ns();
+    uint64_t t0 = now_ns();
     RollbackPlan rp;
     rollback_plan(L.man, snap, snap_hashes, L.plan, L.hashes, ids, o.block_bytes, geteuid(), &rp);
     call.ctl->bytes_total.store(hashed_bytes + rp.bytes_fetched); call.ctl->blocks_total.store(hashed_blocks + rp.blocks_fetched);
@@ -1822,71 +1805,50 @@ int rollback_body(CallScope& call, const char* layer_dir, const char* layer_tabl
     return VMIG_OK;
 }
 
-// vmig_snapshot_layer: the refusals after the arguments, the layer's walk, then the snapshot's passes with the layer table
+// The layer calls after their refusals: the source's walk, then the tree passes with the source's table
+int layer_tree_passes(CallScope& call, TreeCall& c, const vmig_opts& o, vmig_stats& st, uint64_t t_begin, vmig_stats* stats_out)
+{
+    Manifest man;
+    const uint64_t t0 = now_ns();
+    call.phase(VMIG_PHASE_WALK);
+    const int rc = walk_tree(c.src, o.block_bytes, (o.flags & VMIG_F_SKIP_HIDDEN_TOPDIRS) != 0, &man, call.cancel());
+    if (rc) return rc;
+    st.ns_walk = now_ns() - t0;
+    c.man = &man;
+    return tree_passes(call, c, o, st, t_begin, stats_out);
+}
+
+// vmig_snapshot_layer: the snapshot's passes with the layer table
 int snapshot_layer_body(CallScope& call, const char* layer_dir, const char* layer_table, const char* dst_dir, const char* base_dir,
                         const char* base_table, const char* out_table, const vmig_opts& o, vmig_stats* stats_out,
                         vmig_layer_snapshot_stats* ls_out)
 {
-    const std::atomic<int>* cancel = call.cancel();
     vmig_stats st; memset(&st, 0, sizeof st);
     const uint64_t t_begin = now_ns();
-    if (cancel->load()) return fail(VMIG_ECANCELED, "the control was cancelled before the call started");
-    for (const char* d : {layer_dir, dst_dir, base_dir}) {
-        struct stat sb;
-        if (stat(d, &sb) != 0 || !S_ISDIR(sb.st_mode)) return fail(VMIG_ENOTDIR, "%s is missing or not a directory", d);
-    }
     BlockTable base, layer;
-    int rc = load_table(base_table, "base", o.block_bytes, &base);
-    if (!rc) rc = load_table(layer_table, "layer", o.block_bytes, &layer);
+    const int rc = start_checks(call, o, {layer_dir, dst_dir, base_dir}, {{base_table, "base", &base}, {layer_table, "layer", &layer}});
     if (rc) return rc;
-    std::vector<DeviceInfo> devs;                    // no CPU fallback: the GPU is there before anything is read
-    rc = ctx_select(o.gpu_mask, &devs);
-    if (rc) return rc;
-
-    Manifest man;
-    const uint64_t t0 = now_ns();
-    call.phase(VMIG_PHASE_WALK);
-    rc = walk_tree(layer_dir, o.block_bytes, (o.flags & VMIG_F_SKIP_HIDDEN_TOPDIRS) != 0, &man, cancel);
-    if (rc) return rc;
-    st.ns_walk = now_ns() - t0;
-    SnapshotArgs sa{base_dir, base_table, nullptr};
-    sa.base_loaded = &base; sa.layer = &layer; sa.layer_out = ls_out;
-    return tree_passes(call, layer_dir, dst_dir, man, {}, nullptr, out_table, o, st, &sa, nullptr, t_begin, stats_out);
+    TreeCall c;
+    c.src = layer_dir; c.dst = dst_dir; c.base = &base; c.base_dir = base_dir; c.layer = &layer;
+    c.out_table = out_table; c.refresh_ids = true; c.layer_snap_out = ls_out;
+    return layer_tree_passes(call, c, o, st, t_begin, stats_out);
 }
 
-// vmig_migrate_layer: the refusals after the arguments, the source's walk, then the migration's passes with the
-// source's table
+// vmig_migrate_layer: the migration's passes with the source's table
 int migrate_layer_body(CallScope& call, const char* src_dir, const char* src_table, const char* dst_dir, const char* prior_table,
                        const char* out_table, const char* src_out_table, const vmig_opts& o, vmig_stats* stats_out,
                        vmig_layer_migrate_stats* lm_out)
 {
-    const std::atomic<int>* cancel = call.cancel();
     vmig_stats st; memset(&st, 0, sizeof st);
     const uint64_t t_begin = now_ns();
-    if (cancel->load()) return fail(VMIG_ECANCELED, "the control was cancelled before the call started");
-    for (const char* d : {src_dir, dst_dir}) {
-        struct stat sb;
-        if (stat(d, &sb) != 0 || !S_ISDIR(sb.st_mode)) return fail(VMIG_ENOTDIR, "%s is missing or not a directory", d);
-    }
     BlockTable src_tab, prior;
-    src_tab.block_bytes = o.block_bytes;
-    const bool has_prior = prior_table && *prior_table;
-    int rc = src_table && *src_table ? load_table(src_table, "source", o.block_bytes, &src_tab) : VMIG_OK;
-    if (!rc && has_prior) rc = load_table(prior_table, "prior", o.block_bytes, &prior);
+    src_tab.block_bytes = o.block_bytes;             // no src_table: an empty table, which trusts nothing
+    const int rc = start_checks(call, o, {src_dir, dst_dir}, {{src_table, "source", &src_tab}, {prior_table, "prior", &prior}});
     if (rc) return rc;
-    std::vector<DeviceInfo> devs;                    // no CPU fallback: the GPU is there before anything is read
-    rc = ctx_select(o.gpu_mask, &devs);
-    if (rc) return rc;
-
-    Manifest man;
-    const uint64_t t0 = now_ns();
-    call.phase(VMIG_PHASE_WALK);
-    rc = walk_tree(src_dir, o.block_bytes, (o.flags & VMIG_F_SKIP_HIDDEN_TOPDIRS) != 0, &man, cancel);
-    if (rc) return rc;
-    st.ns_walk = now_ns() - t0;
-    const LayerMigrateArgs lma{&src_tab, has_prior ? &prior : nullptr, src_out_table, lm_out};
-    return tree_passes(call, src_dir, dst_dir, man, {}, has_prior ? prior_table : nullptr, out_table, o, st, nullptr, nullptr,
-                       t_begin, stats_out, &lma);
+    TreeCall c;
+    c.src = src_dir; c.dst = dst_dir; c.layer = &src_tab; c.prior = prior_table && *prior_table ? &prior : nullptr;
+    c.out_table = out_table; c.src_out_table = src_out_table; c.layer_mig_out = lm_out;
+    return layer_tree_passes(call, c, o, st, t_begin, stats_out);
 }
 
 }  // namespace
@@ -1982,14 +1944,18 @@ const char* vmig_strerror(int code)
 int vmig_migrate_tree(const char* src_dir, const char* dst_dir, const char* prior_table, const char* out_table,
                       const vmig_opts* opts, vmig_stats* stats)
 {
-    return migrate_tree_impl(src_dir, dst_dir, prior_table, out_table, opts, stats);
+    TreeCall c;
+    c.out_table = out_table;
+    return migrate_tree_impl(c, src_dir, dst_dir, prior_table, nullptr, nullptr, opts, stats);
 }
 int vmig_restore_tree(const char* snap_dir, const char* snap_table, const char* dst_dir, const char* prior_table,
                       const char* out_table, const vmig_opts* opts, vmig_stats* stats)
 {
     if (!snap_table || !*snap_table) return fail(VMIG_EINVAL, "snap_table is NULL/empty: a snapshot is only restored against its block table");
     if (opts && (opts->flags & VMIG_F_MOVE_SRC)) return fail(VMIG_EINVAL, "VMIG_F_MOVE_SRC: a restore never consumes the snapshot");
-    return migrate_tree_impl(snap_dir, dst_dir, prior_table, out_table, opts, stats, snap_table);
+    TreeCall c;
+    c.out_table = out_table;
+    return migrate_tree_impl(c, snap_dir, dst_dir, prior_table, snap_table, nullptr, opts, stats);
 }
 int vmig_restore_paths(const char* snap_dir, const char* snap_table, const char* dst_dir, uint32_t n_paths,
                        const char* const* paths, const char* prior_table, const vmig_opts* opts, vmig_stats* stats)
@@ -2005,7 +1971,7 @@ int vmig_restore_paths(const char* snap_dir, const char* snap_table, const char*
     if (o.flags & VMIG_F_HASH_ONLY) return fail(VMIG_EINVAL, "VMIG_F_HASH_ONLY: a partial restore writes its destination (vmig_scrub_store checks a version)");
     if (o.flags & VMIG_F_CUFILE) return fail(VMIG_EINVAL, "VMIG_F_CUFILE: not supported for a partial restore");
     rc = check_block_bytes(o);
-    if (!rc) rc = check_restore_paths_dirs(snap_dir, dst_dir);
+    if (!rc) rc = check_apart("snap_dir", real_path(snap_dir), "dst_dir", real_path(dst_dir));
     if (rc) return rc;
     return in_call(o.ctl, [&](CallScope& call) { return restore_paths_body(call, snap_dir, snap_table, dst_dir, sorted, prior_table, o, stats); });
 }
@@ -2022,8 +1988,9 @@ int vmig_snapshot_tree(const char* src_dir, const char* dst_dir, const char* bas
     if (!dst_dir || !*dst_dir) return fail(VMIG_EINVAL, "dst_dir is NULL/empty");
     if (has_dir) { const int rc = check_snapshot_paths(dst_dir, base_dir); if (rc) return rc; }
     if (snap_stats) memset(snap_stats, 0, sizeof *snap_stats);
-    const SnapshotArgs sa{has_dir ? base_dir : nullptr, has_table ? base_table : nullptr, snap_stats};
-    return migrate_tree_impl(src_dir, dst_dir, nullptr, out_table, opts, stats, nullptr, &sa);
+    TreeCall c;                                            // no base: a full snapshot
+    c.out_table = out_table; c.base_dir = has_dir ? base_dir : ""; c.refresh_ids = true; c.snap_out = snap_stats;
+    return migrate_tree_impl(c, src_dir, dst_dir, nullptr, nullptr, has_table ? base_table : nullptr, opts, stats);
 }
 int vmig_snapshot_layer(const char* layer_dir, const char* layer_table, const char* dst_dir, const char* base_dir,
                         const char* base_table, const char* out_table, const vmig_opts* opts, vmig_stats* stats,
@@ -2040,14 +2007,11 @@ int vmig_snapshot_layer(const char* layer_dir, const char* layer_table, const ch
         return fail(VMIG_EINVAL, "flags 0x%x: a layer snapshot takes only VMIG_F_VERIFY, VMIG_F_PRUNE, VMIG_F_DIRECT_IO, VMIG_F_MTIME_NS, "
                     "VMIG_F_NO_METADATA and VMIG_F_SKIP_HIDDEN_TOPDIRS", o.flags & ~allowed);
     int rc = check_block_bytes(o);
+    const std::string rd = real_path(dst_dir), rb = real_path(base_dir), rl = real_path(layer_dir);
+    if (!rc) rc = check_apart("dst_dir", rd, "base_dir", rb);
+    if (!rc) rc = check_apart("dst_dir", rd, "layer_dir", rl);
+    if (!rc) rc = check_apart("base_dir", rb, "layer_dir", rl);
     if (rc) return rc;
-    std::string rd, rb, rl, x, y;
-    if (real_paths_overlap(dst_dir, base_dir, &rd, &rb))
-        return fail(VMIG_EINVAL, "dst_dir %s and base_dir %s are the same directory or one is inside the other", rd.c_str(), rb.c_str());
-    if (real_paths_overlap(dst_dir, layer_dir, &x, &rl))
-        return fail(VMIG_EINVAL, "dst_dir %s and layer_dir %s are the same directory or one is inside the other", x.c_str(), rl.c_str());
-    if (real_paths_overlap(base_dir, layer_dir, &x, &y))
-        return fail(VMIG_EINVAL, "base_dir %s and layer_dir %s are the same directory or one is inside the other", x.c_str(), y.c_str());
     std::string ro, rt;
     rc = real_parent_path(out_table, &ro);
     if (!rc) rc = real_parent_path(base_table, &rt);
@@ -2071,10 +2035,9 @@ int vmig_migrate_layer(const char* src_dir, const char* src_table, const char* d
         return fail(VMIG_EINVAL, "flags 0x%x: a layer migration takes only VMIG_F_VERIFY, VMIG_F_PRUNE, VMIG_F_DIRECT_IO, VMIG_F_MTIME_NS, "
                     "VMIG_F_NO_METADATA and VMIG_F_SKIP_HIDDEN_TOPDIRS", o.flags & ~allowed);
     int rc = check_block_bytes(o);
+    const std::string rs = real_path(src_dir), rd = real_path(dst_dir);
+    if (!rc) rc = check_apart("src_dir", rs, "dst_dir", rd);
     if (rc) return rc;
-    std::string rs, rd;
-    if (real_paths_overlap(src_dir, dst_dir, &rs, &rd))
-        return fail(VMIG_EINVAL, "src_dir %s and dst_dir %s are the same directory or one is inside the other", rs.c_str(), rd.c_str());
     const bool has_out = out_table && *out_table, has_src_out = src_out_table && *src_out_table;
     std::string ro, rso;
     if (has_out && (rc = real_parent_path(out_table, &ro))) return rc;
@@ -2153,10 +2116,9 @@ int vmig_rollback_layer(const char* layer_dir, const char* layer_table, const ch
         return fail(VMIG_EINVAL, "flags 0x%x: a rollback takes only VMIG_F_DIRECT_IO, VMIG_F_SKIP_HIDDEN_TOPDIRS, VMIG_F_MTIME_NS, "
                     "VMIG_F_NO_METADATA, VMIG_F_VERIFY and VMIG_F_PRUNE", o.flags & ~allowed);
     int rc = check_block_bytes(o);
+    const std::string rs = real_path(snap_dir);
+    if (!rc) rc = check_apart("layer_dir", real_path(layer_dir), "snap_dir", rs);
     if (rc) return rc;
-    std::string rl, rs;
-    if (real_paths_overlap(layer_dir, snap_dir, &rl, &rs))
-        return fail(VMIG_EINVAL, "layer_dir %s and snap_dir %s are the same directory or one is inside the other", rl.c_str(), rs.c_str());
     if (out_table && *out_table) {
         std::string ro, rt;
         rc = real_parent_path(out_table, &ro);
@@ -2169,13 +2131,13 @@ int vmig_rollback_layer(const char* layer_dir, const char* layer_table, const ch
         return rollback_body(call, layer_dir, layer_table, snap_dir, snap_table, out_table, o, stats, rb_stats);
     });
 }
-int vmig_copy_dir(const char* src_dir, const char* dst_dir) { return migrate_tree_impl(src_dir, dst_dir, nullptr, nullptr, nullptr, nullptr); }
+int vmig_copy_dir(const char* src_dir, const char* dst_dir) { return migrate_tree_impl({}, src_dir, dst_dir, nullptr, nullptr, nullptr, nullptr, nullptr); }
 int vmig_move_dir(const char* src_dir, const char* dst_dir)
 {
     // a move destroys the only other copy: the destination is re-read through the GPU and must hash like the
     // source (VMIG_F_VERIFY) and is flushed (syncfs) before anything is unlinked
     vmig_opts o; memset(&o, 0, sizeof o); o.flags = VMIG_F_MOVE_SRC | VMIG_F_VERIFY;
-    return migrate_tree_impl(src_dir, dst_dir, nullptr, nullptr, &o, nullptr);
+    return migrate_tree_impl({}, src_dir, dst_dir, nullptr, nullptr, nullptr, &o, nullptr);
 }
 
 int vmig_thread_plan(uint32_t lanes, uint32_t n_gpus, uint32_t flags, int has_prior, uint32_t* readers, uint32_t* writers)

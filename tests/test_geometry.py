@@ -392,12 +392,12 @@ def test_block_size_limits(vm, orc, shm_tmp):
 
 
 # ------------------------------------------------------------------------------------------ settings read once per process
-def _run_child(fn: str, arg: dict, env: dict) -> dict:
-    """Run test_geometry.<fn>(arg) in a new Python process with `env` added; it prints one JSON line of results."""
+def _run_child(fn: str, arg: dict, env: dict, module: str = "test_geometry") -> dict:
+    """Run <module>.<fn>(arg) in a new Python process with `env` added; it prints one JSON line of results."""
     here = Path(__file__).resolve().parent
-    code = ("import json, sys; sys.path[:0] = sys.argv[1:3]; import test_geometry as t; "
+    code = ("import importlib, json, sys; sys.path[:0] = sys.argv[1:3]; t = importlib.import_module(sys.argv[5]); "
             "print(json.dumps(getattr(t, sys.argv[3])(json.loads(sys.argv[4]))))")
-    r = subprocess.run([sys.executable, "-c", code, str(here), str(here.parent), fn, json.dumps(arg)],
+    r = subprocess.run([sys.executable, "-c", code, str(here), str(here.parent), fn, json.dumps(arg), module],
                        env={**os.environ, **env}, capture_output=True, text=True, timeout=600)
     assert r.returncode == 0, r.stdout[-2000:] + r.stderr[-4000:]
     return json.loads(r.stdout.strip().splitlines()[-1])

@@ -611,13 +611,19 @@ def test_migrate_buffer_roundtrip_and_diff(vm, orc, pinned):
                            [min(4 * MiB, n - i * 4 * MiB) for i in range(nb)])
     assert (h == want).all()
     assert st["bytes_h2d"] == n == st["bytes_d2h"]
-    # diff: change two blocks of src, poison dst's other blocks, migrate against the prior hashes
+    # diff: change two blocks of src, poison dst's other blocks, migrate against the prior hashes: the two changed
+    # blocks are written, the poison in every skipped block stays
     src[5 * 4 * MiB + 17] ^= 1
     src[-1] ^= 0x80
     dst2 = dst.copy() if not pinned else dst
+    dst2[:] = ~data
     h2, st2 = vm.migrate_buffer(src, dst2, h, np.ones(nb, np.uint8))
     assert st2["blocks_skipped"] == nb - 2 and st2["bytes_d2h"] == 4 * MiB + (n - (nb - 1) * 4 * MiB)
-    assert (dst2 == src).all()
+    changed = [(5 * 4 * MiB, 6 * 4 * MiB), ((nb - 1) * 4 * MiB, n)]
+    for lo, hi in changed:
+        assert (dst2[lo:hi] == src[lo:hi]).all(), lo
+    for lo, hi in [(0, changed[0][0]), (changed[0][1], changed[1][0])]:
+        assert (dst2[lo:hi] == ~data[lo:hi]).all(), (lo, hi)
     assert (np.nonzero(h2 != h)[0] == [5, nb - 1]).all()
     if pinned:
         a.free(), b.free()
